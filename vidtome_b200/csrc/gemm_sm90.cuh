@@ -1,5 +1,5 @@
-// Persistent warp-specialised wgmma GEMM mainloop for sm_90a, shared by KA (similarity + row arg-max
-// epilogue) and the projection GEMMs of KD (fp16 store epilogues).
+// Persistent warp-specialised wgmma GEMM mainloop for sm_90a, shared by the projection GEMMs of KD (QKV, output,
+// GEGLU, residual: fp16 store epilogues).  KA (similarity + row arg-max) has its own kernel in sim_argmax.cu.
 //
 //   D[b][m, n] = sum_k A[b][m, k] * Bm[b][n, k]        fp16 operands (K-major), fp32 accumulators
 //
@@ -9,11 +9,6 @@
 // through shared-memory descriptors.  The producer runs ahead across tile and work-item boundaries, so the loads of
 // tile i+1 overlap the epilogue of tile i.
 // A work item is (m_tile, b, [nt0, nt1)); CTAs stride over work items (persistent grid = #SMs).
-//
-// CTA-pair build (PAIR = true, launched as clusters of two): the two CTAs of a cluster take the two m tiles of one work
-// item (m unit = 2 tiles) and sweep the same dst tiles; each loads its own A tile and HALF of every B tile, multicast to
-// both CTAs, so every B byte leaves L2 once per pair.  A stage may be refilled only when the consumers of BOTH CTAs are
-// done with it (each consumer warp arrives on both CTAs' empty barriers).
 //
 // Epilogues read one ROW per thread: after its mainloop a warpgroup writes its fp32 accumulators to a row-major
 // staging area in shared memory, and thread t of the warpgroup then owns row (t % 64) and column half (t / 64) of its
@@ -77,17 +72,13 @@ struct Work {
   int tiles_per_split, n_splits;
   int k_chunks;
   int total;
-  // Order of the work items.  0: m tile fastest (KA: the dst ranges of one src block run far apart in time, so a later
-  // range starts from the maxima the earlier ones published).  1: n split fastest (plain GEMMs): the splits of one m tile
-  // run on neighbouring CTAs at the same time, so the A tile comes from HBM once and from L2 afterwards.
+  // Order of the work items.  0: m tile fastest.  1: n split fastest (plain GEMMs): the splits of one m tile run on
+  // neighbouring CTAs at the same time, so the A tile comes from HBM once and from L2 afterwards.
   int n_fastest;
-  int m_tiles_real;     // m tiles of the problem; m_tiles counts m units (pairs of tiles in the CTA-pair build)
-  __host__ void plan(int M, int N, int K, int B, int sms, int target_items_per_sm, int min_tiles, bool pair = false) {
+  __host__ void plan(int M, int N, int K, int B, int sms, int target_items_per_sm, int min_tiles) {
     batches = B;
     n_fastest = 0;
-    m_tiles_real = (M + BM - 1) / BM;
-    m_tiles = pair ? (m_tiles_real + 1) / 2 : m_tiles_real;
-    if (pair) sms /= 2;   // work items are shared by the two CTAs of a cluster
+    m_tiles = (M + BM - 1) / BM;
     n_tiles = (N + BN - 1) / BN;
     k_chunks = (K + BK - 1) / BK;
     const long long base = static_cast<long long>(m_tiles) * B;
@@ -148,7 +139,7 @@ __device__ __forceinline__ void warp_store_rows64(uint32_t scratch, const uint32
   __syncwarp();
 }
 
-template <bool PAIR, class Epi>
+template <class Epi>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const Work wk, Epi epi) {
@@ -167,22 +158,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = warp >> 2;
-  // work-item stride: CTAs, or clusters of two in the pair build
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const int w_first = PAIR ? static_cast<int>(cluster_id_x()) : static_cast<int>(blockIdx.x);
-  const int w_step = PAIR ? static_cast<int>(cluster_count_x()) : static_cast<int>(gridDim.x);
+  const int w_first = static_cast<int>(blockIdx.x);
+  const int w_step = static_cast<int>(gridDim.x);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), PAIR ? 2 * CONSUMER_WARPS : CONSUMER_WARPS);
+      mbar_init(empty_bar(s), CONSUMER_WARPS);
     }
     fence_mbar_init();
   }
-  if constexpr (PAIR) cluster_sync_all();   // the peer's barriers are initialised before anything signals them
-  else __syncthreads();
+  __syncthreads();
 
   if (wg == 0) {
     // ===================== TMA producer =====================
@@ -193,26 +181,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       for (int w = w_first; w < wk.total; w += w_step) {
         int m_tile, b, nt0, nt1;
         wk.decode(w, &m_tile, &b, &nt0, &nt1);
-        if (PAIR) {
-          m_tile = 2 * m_tile + static_cast<int>(rank);
-          // the second tile of an odd last pair lies past M: load a real tile (its rows are never stored)
-          if (m_tile >= wk.m_tiles_real) m_tile = wk.m_tiles_real - 1;
-        }
         for (int nt = nt0; nt < nt1; ++nt) {
           for (int kc = 0; kc < wk.k_chunks; ++kc) {
             const uint32_t sa = smem_base + stage * STAGE_BYTES;
-            if constexpr (PAIR) {
-              mbar_wait_cluster(empty_bar(stage), phase ^ 1u);   // both CTAs' consumers released the slot
-              mbar_arrive_expect_tx(full_bar(stage), STAGE_BYTES);   // own A + both halves of B
-              tma_load_3d(sa, &tmap_a, full_bar(stage), kc * BK, m_tile * BM, b);
-              tma_load_3d_multicast(sa + A_BYTES + rank * (B_BYTES / 2), &tmap_b, full_bar(stage), kc * BK,
-                                    nt * BN + static_cast<int>(rank) * (BN / 2), b, 0x3);
-            } else {
-              mbar_wait(empty_bar(stage), phase ^ 1u);
-              mbar_arrive_expect_tx(full_bar(stage), STAGE_BYTES);
-              tma_load_3d(sa, &tmap_a, full_bar(stage), kc * BK, m_tile * BM, b);
-              tma_load_3d(sa + A_BYTES, &tmap_b, full_bar(stage), kc * BK, nt * BN, b);
-            }
+            mbar_wait(empty_bar(stage), phase ^ 1u);
+            mbar_arrive_expect_tx(full_bar(stage), STAGE_BYTES);
+            tma_load_3d(sa, &tmap_a, full_bar(stage), kc * BK, m_tile * BM, b);
+            tma_load_3d(sa + A_BYTES, &tmap_b, full_bar(stage), kc * BK, nt * BN, b);
             if (++stage == STAGES) { stage = 0; phase ^= 1u; }
           }
         }
@@ -236,18 +211,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     int stage = 0;
     uint32_t phase = 0;
     float d[64];
-    // smem slot reusable: this warp's MMAs reading it have retired (both CTAs' consumers gate a slot in the pair build)
+    // smem slot reusable: this warp's MMAs reading it have retired
     auto release = [&](int st) {
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(empty_bar(st));
-        if constexpr (PAIR) mbar_arrive_cluster(mapa_shared(empty_bar(st), rank ^ 1u));
-      }
+      if (lane == 0) mbar_arrive(empty_bar(st));
     };
     for (int w = w_first; w < wk.total; w += w_step) {
       int m_tile, b, nt0, nt1;
       wk.decode(w, &m_tile, &b, &nt0, &nt1);
-      if (PAIR) m_tile = 2 * m_tile + static_cast<int>(rank);   // may lie past M: the epilogues skip rows >= M
       e.begin(m_tile, b, row_in_tile);
       for (int nt = nt0; nt < nt1; ++nt) {
         // one wgmma group stays in flight: the stage of chunk kc - 1 is released once chunk kc has been issued
@@ -289,11 +260,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       e.end(m_tile, b, row_in_tile);
     }
   }
-  // the peer may still multicast into this CTA's shared memory or arrive on its barriers until it is done too
-  if constexpr (PAIR) cluster_sync_all();
 }
 
-template <class Epi, bool PAIR = false>
+template <class Epi>
 inline int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Work& wk, const Epi& epi, int sms,
                   cudaStream_t stream) {
   using C = Cfg<Epi::SCRATCH_PER_WARP>;
@@ -304,31 +273,14 @@ inline int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Work& wk, 
   int rc = cuda_rc(cudaGetDevice(&dev));
   if (rc) return rc;
   if (dev < 0 || dev >= 64 || !opted[dev]) {
-    rc = cuda_rc(cudaFuncSetAttribute(gemm_kernel<PAIR, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    rc = cuda_rc(cudaFuncSetAttribute(gemm_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       static_cast<int>(smem)));
     if (rc) return rc;
     if (dev >= 0 && dev < 64) opted[dev] = true;
   }
-  if constexpr (!PAIR) {
-    const int grid = wk.total < sms ? wk.total : sms;
-    gemm_kernel<false, Epi><<<grid, THREADS, smem, stream>>>(ta, tb, wk, epi);
-    return launch_rc();
-  } else {
-    const int pairs = wk.total < sms / 2 ? wk.total : sms / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(static_cast<unsigned>(2 * (pairs > 0 ? pairs : 1)));
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cuda_rc(cudaLaunchKernelEx(&cfg, gemm_kernel<true, Epi>, ta, tb, wk, epi));
-  }
+  const int grid = wk.total < sms ? wk.total : sms;
+  gemm_kernel<Epi><<<grid, THREADS, smem, stream>>>(ta, tb, wk, epi);
+  return launch_rc();
 }
 
 inline int device_sms(int* sms) { return cached_sm_count(sms); }
