@@ -3,16 +3,24 @@
 Prints one JSON line per (kernel, shape): CUDA-event time (median of `--iters` after warm-up, L2 flushed
 between iterations by writing a 256 MiB buffer), achieved TFLOP/s or GB/s and the fraction of the measured
 peak in MEASURED_PEAKS.json (else the H100 SXM data-sheet figures).  `--quick` runs only the BASELINE config-2 shapes;
-`--ka-only` only the KA (similarity + arg-max) shapes, `--ka-variant pair` with KA's CTA-pair build.
+`--ka-only` only the KA (similarity + arg-max) shapes, `--ka-variant pair` with KA's CTA-pair build; `--kd-only` only
+the two KD (merged-token self-attention) shapes.
 
 The KA line also gives `l2_fill_MB`: the operand bytes the kernel's tiling loads into shared memory (computed from the
 shapes, the tile sizes and the work split of csrc/sim_argmax.cu), and `l2_fill_TBs`, those bytes over the kernel time.
+
+The KD line also gives the flash-attention kernel's own time (`flash_ms`, mean over a torch.profiler pass that follows
+the timed window, with L2 flushed before every call as in the timed window) and `flash_over_mufu_floor`: that time over
+the least time the SM's exponential units need for the B·H·L² ex2 of the softmax, at 16 ex2 per clock per SM and the SM
+clock read from nvidia-smi right after the timed window (`sm_clock_mhz`; the device's maximum clock when nvidia-smi is
+not available).
 """
 from __future__ import annotations
 
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 import torch
@@ -162,25 +170,59 @@ def bench_linear(M, N, K, iters):
                       "cublas_tflops": round(flops / med_t / 1e9, 1)}), flush=True)
 
 
-def bench_attention(B, L, C, heads, iters):
+def sm_clock_mhz():
+    """Current SM clock of device 0 from nvidia-smi (read right after a timed window, i.e. the clock under load), else
+    the device's maximum SM clock."""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=clocks.sm", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        return float(r.stdout.strip().splitlines()[0]), "nvidia-smi"
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        return torch.cuda.get_device_properties(0).clock_rate / 1e3, "max"
+
+
+def flash_kernel_ms(fn, calls=10):
+    """Mean device time per call of the flash-attention kernel over `calls` calls of fn, from torch.profiler, with L2
+    flushed before every call as in time_ms."""
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            flush_l2()
+            fn()
+        torch.cuda.synchronize()
+    us = [e.device_time_total for e in prof.key_averages() if "flash_attn_kernel" in e.key]
+    return sum(us) / calls / 1e3 if us else float("nan")
+
+
+def bench_attention(B, L, C, heads, iters, kernel=False):
     g = torch.Generator(device="cuda").manual_seed(0)
     x = torch.randn((B, L, C), generator=g, device="cuda").half()
     ws = [(torch.randn((C, C), generator=g, device="cuda") / C ** 0.5).half() for _ in range(4)]
     wqkv = torch.cat(ws[:3], 0).contiguous()
     bo = torch.zeros(C, device="cuda").half()
     d = C // heads
-    med, _ = time_ms(lambda: ops.attention(x, wqkv, ws[3], bo, heads, d ** -0.5), iters)
+    kd = lambda: ops.attention(x, wqkv, ws[3], bo, heads, d ** -0.5)  # noqa: E731
+    med, _ = time_ms(kd, iters)
+    clock, clock_src = sm_clock_mhz() if kernel else (None, None)
 
     def sdpa():
         q, k, v = [torch.nn.functional.linear(x, w).view(B, L, heads, d).transpose(1, 2) for w in ws[:3]]
         o = torch.nn.functional.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, L, C)
         return torch.nn.functional.linear(o, ws[3], bo)
     med_t, _ = time_ms(sdpa, iters)
-    qkv = ops.linear(x.view(B * L, C), wqkv)
     flops = 4.0 * B * L * L * C + 8.0 * B * L * C * C
-    print(json.dumps({"kernel": "KD attention (qkv+flash+out)", "B": B, "L": L, "C": C, "heads": heads,
-                      "ms": round(med, 4), "tflops": round(flops / med / 1e9, 1), "torch_sdpa_path_ms": round(med_t, 4),
-                      "speedup_vs_torch": round(med_t / med, 2)}), flush=True)
+    row = {"kernel": "KD attention (qkv+flash+out)", "B": B, "L": L, "C": C, "heads": heads,
+           "ms": round(med, 4), "tflops": round(flops / med / 1e9, 1), "torch_sdpa_path_ms": round(med_t, 4),
+           "speedup_vs_torch": round(med_t / med, 2)}
+    if kernel:
+        fl = flash_kernel_ms(kd)
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        mufu_ms = B * heads * float(L) * L / (16.0 * sms * clock * 1e3)
+        row.update({"flash_ms": round(fl, 4), "sm_clock_mhz": clock, "sm_clock_src": clock_src,
+                    "mufu_floor_ms": round(mufu_ms, 4), "flash_over_mufu_floor": round(fl / mufu_ms, 2)})
+    print(json.dumps(row), flush=True)
 
 
 def main():
@@ -189,9 +231,16 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--ka-only", action="store_true")
     ap.add_argument("--ka-variant", default="cta", choices=["cta", "pair"])
+    ap.add_argument("--kd-only", action="store_true")
     args = ap.parse_args()
     torch.cuda.init()
     ops.KA_VARIANT = args.ka_variant
+    if args.kd_only:
+        from vidtome_b200._lib import LIB_PATH
+        print(json.dumps({"device": torch.cuda.get_device_name(0), "lib": LIB_PATH}), flush=True)
+        bench_attention(2, 10241, 320, 8, args.iters, kernel=True)
+        bench_attention(2, 2561, 640, 8, args.iters, kernel=True)
+        return
     # BASELINE config 2 shapes (SURVEY App. B): ds1 level 1/2, ds2 level 1/2
     for (Ns, Nd, C) in [(49152, 16384, 320), (12288, 9012, 320), (12288, 4096, 640), (3072, 2253, 640)]:
         bench_sim_argmax(2, Ns, Nd, C, False, args.iters)

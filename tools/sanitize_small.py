@@ -16,7 +16,7 @@ for (M, N, K) in [(333, 320, 320), (1000, 960, 320), (130, 1920, 640)]:
     b = torch.randn((N,), generator=g, device="cuda").half()
     y = ops.linear(a, w, b)
     assert torch.isfinite(y).all()
-# attention: one plain shape, one whose last wave is split over key ranges
+# attention: ragged query and key tails, head_dim 40 / 80 / 64 (three and two consumer warpgroups)
 for (B, L, C, H) in [(1, 333, 320, 8), (2, 2561, 640, 8), (3, 1500, 320, 8), (1, 700, 320, 5)]:
     x = torch.randn((B, L, C), generator=g, device="cuda").half()
     ws = [(torch.randn((C, C), generator=g, device="cuda") / C ** 0.5).half() for _ in range(4)]

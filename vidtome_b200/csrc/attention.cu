@@ -4,10 +4,10 @@
 // Reference: `self.attn1(merged_tokens)` at vidtome/patch.py:157-162 = diffusers Attention; the math is
 // restated in the reference at utils/pnp_utils.py:47-95: softmax(q k^T * scale) v per head.
 //
-// Flash-attention kernel (flash_attn_kernel below): one CTA per (128-row query tile, head, sample), a TMA producer
+// Flash-attention kernel (flash_attn_kernel below): one CTA per (64 x CW-row query tile, head, sample), a TMA producer
 // warpgroup streaming K/V tiles of one head (contiguous runs of the head-major padded buffers written by the projection
-// epilogue) through an mbarrier ring, and two wgmma consumer warpgroups running S = Q K^T, the online softmax and
-// O += P V with P kept in registers.
+// epilogue) through an mbarrier ring, and CW = 3 (head_dim <= 80) or 2 wgmma consumer warpgroups running S = Q K^T, the
+// online softmax and O += P V with P kept in registers, each overlapping its softmax with its own P V.
 #include <stdlib.h>
 
 #include "gemm_sm90.cuh"
@@ -140,10 +140,7 @@ int launch_head_proj(const void* x, const void* w, __half* out, int nb, int L, i
   return gemm::launch<HeadSplitEpi>(ta, tb, wk, epi, sms, stream);
 }
 
-constexpr int FA_BQ = 128;       // query rows per CTA: two consumer warpgroups of 64
 constexpr int FA_BKV = 64;       // keys per K/V tile
-constexpr int FA_THREADS = 384;  // producer warpgroup + two consumer warpgroups
-constexpr int FA_STAGES = 3;     // K/V ring depth
 
 struct FaParams {
   __half* o;          // [B*Lq, C]
@@ -154,38 +151,99 @@ struct FaParams {
 
 template <int KS>
 struct FaCfg {
+  // Consumer warpgroups, 64 query rows each.  Three (512 threads, at most 128 registers each) hide more of the softmax's
+  // latency than two; from head_dim 96 on, O no longer fits next to S and P in 128 registers, so those keep two.
+  static constexpr int CW = KS <= 5 ? 3 : 2;
+  static constexpr int BQ = 64 * CW;                      // query rows per CTA
+  static constexpr int THREADS = 128 * (CW + 1);          // producer warpgroup + consumers
   static constexpr int DV = 16 * KS;                      // head_dim rounded up to 16: k-steps of Q K^T, width of O
   static constexpr int ATOMS = (KS + 3) / 4;              // 64-column blocks of a padded row (one TMA box each)
-  static constexpr uint32_t Q_ATOM = FA_BQ * 128;         // [128 rows x 128 B]
+  static constexpr uint32_t Q_ATOM = BQ * 128;            // [BQ rows x 128 B]
   static constexpr uint32_t KV_ATOM = FA_BKV * 128;       // [64 rows x 128 B]
   static constexpr uint32_t Q_BYTES = ATOMS * Q_ATOM;
   static constexpr uint32_t TILE_BYTES = ATOMS * KV_ATOM;
   static constexpr uint32_t STAGE_BYTES = 2 * TILE_BYTES; // K + V
-  static constexpr size_t SMEM_BYTES = 1024 + Q_BYTES + static_cast<size_t>(FA_STAGES) * STAGE_BYTES + 256;
+  // K/V ring depth.  The consumers hold two stages at a time (Q K^T of tile j+1 is issued before P V of tile j), so
+  // four stages keep two tile loads in flight; five timed the same at both bench shapes.
+  static constexpr int STAGES = 4;
+  static constexpr size_t SMEM_BYTES = 1024 + Q_BYTES + static_cast<size_t>(STAGES) * STAGE_BYTES + 256;
 };
 
-// One CTA per (128-row query tile, head, sample).  Warpgroup 0 (one lane) loads the Q tile once and streams K/V tiles
-// of 64 keys through a TMA + mbarrier ring; warpgroups 1 and 2 each own 64 query rows: S = Q K^T (wgmma, both operands
+// Online softmax of one 64-key tile of S in the log2 domain.  The thread holds rows r0 = lane/4 (s[4n], s[4n+1]) and
+// r0 + 8 (s[4n+2], s[4n+3]), columns 8n + 2(lane%4).  On return s holds P = ex2(s * scale - m_new), m_r the new row
+// maxima, l_r the rescaled row sums with this tile's P added, alpha the factor O must be rescaled by before P V of this
+// tile is added to it.  MASK (the last tile only) sets keys at or past `kvalid` to -inf.  The roundings are spelled
+// out: scale as a separate multiply, then ex2 of a subtraction, and l = fma(l, alpha, p0 + p1) for the first pair.
+template <bool MASK>
+__device__ __forceinline__ void fa_softmax(float (&s)[32], float (&m_r)[2], float (&l_r)[2], float (&alpha)[2],
+                                           float scale_log2, int kvalid, int lane) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int n = 0; n < 8; ++n) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      float v = __fmul_rn(s[4 * n + e], scale_log2);
+      if (MASK) {
+        const int col = n * 8 + 2 * (lane & 3) + (e & 1);
+        v = col < kvalid ? v : -INFINITY;
+      }
+      s[4 * n + e] = v;
+      mx[e >> 1] = fmaxf(mx[e >> 1], v);
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+    const float m_new = fmaxf(m_r[r], mx[r]);   // finite: every tile holds at least one valid key
+    alpha[r] = ex2_approx(__fsub_rn(m_r[r], m_new));
+    m_r[r] = m_new;
+  }
+#pragma unroll
+  for (int n = 0; n < 8; ++n) {
+    const float p0 = ex2_approx(__fsub_rn(s[4 * n], m_r[0])), p1 = ex2_approx(__fsub_rn(s[4 * n + 1], m_r[0]));
+    const float p2 = ex2_approx(__fsub_rn(s[4 * n + 2], m_r[1])), p3 = ex2_approx(__fsub_rn(s[4 * n + 3], m_r[1]));
+    if (n == 0) {
+      l_r[0] = __fmaf_rn(l_r[0], alpha[0], __fadd_rn(p0, p1));
+      l_r[1] = __fmaf_rn(l_r[1], alpha[1], __fadd_rn(p2, p3));
+    } else {
+      l_r[0] = __fadd_rn(l_r[0], __fadd_rn(p0, p1));
+      l_r[1] = __fadd_rn(l_r[1], __fadd_rn(p2, p3));
+    }
+    s[4 * n] = p0; s[4 * n + 1] = p1; s[4 * n + 2] = p2; s[4 * n + 3] = p3;
+  }
+}
+
+// One CTA per (BQ-row query tile, head, sample).  Warpgroup 0 (one lane) loads the Q tile once and streams K/V tiles
+// of 64 keys through a TMA + mbarrier ring; warpgroups 1 .. CW each own 64 query rows: S = Q K^T (wgmma, both operands
 // from shared memory, ceil(d / 16) k-steps), online softmax on the S registers (log2 domain), O += P V (wgmma with P as
 // the register A operand and V read MN-major from shared memory: no transposed copy), then O / l -> fp16.  Keys past L
-// arrive as zeros (TMA out-of-bounds fill of the per-head slab) and are masked to -inf before the softmax.
+// arrive as zeros (TMA out-of-bounds fill of the per-head slab) and are masked to -inf in the last tile's softmax.
+//
+// Each consumer warpgroup runs a two-tile software pipeline: S_{j} = Q K_j^T and O += P_{j-1} V_{j-1} are issued as
+// two commit groups, the softmax of tile j runs once the first retires (wait_group 1) while P V is still on the tensor
+// cores, and O is rescaled by tile j's alpha after the second retires.  O therefore sees the same sequence of roundings
+// as a serial loop: O_j = O_{j-1} * alpha_j + P_j V_j.  The stage of tile j-1 is released once its P V has retired.
+// The consumer warpgroups take turns at issuing their MMAs (named barriers 1 .. CW, round robin), so that the MMAs of
+// one run on the tensor cores while the others are in their softmax.
 template <int KS>
-__global__ void __launch_bounds__(FA_THREADS, 1)
+__global__ void __launch_bounds__(FaCfg<KS>::THREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                   const __grid_constant__ CUtensorMap tm_v, const FaParams p) {
   using Cf = FaCfg<KS>;
   constexpr int DV = Cf::DV;
+  constexpr int STAGES = Cf::STAGES;
   extern __shared__ uint8_t fa_smem[];
   const uint32_t base = (smem_u32(fa_smem) + 1023u) & ~1023u;   // 128-byte swizzle: 1024-byte aligned tiles
   const uint32_t sq = base;
   const uint32_t skv = base + Cf::Q_BYTES;
-  const uint32_t bars = skv + FA_STAGES * Cf::STAGE_BYTES;
+  const uint32_t bars = skv + STAGES * Cf::STAGE_BYTES;
   const uint32_t q_full = bars;
   auto kv_full = [&](int s) { return bars + 8u * (1 + s); };
-  auto kv_empty = [&](int s) { return bars + 8u * (1 + FA_STAGES + s); };
+  auto kv_empty = [&](int s) { return bars + 8u * (1 + STAGES + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
-  const int q0 = blockIdx.x * FA_BQ, h = blockIdx.y, b = blockIdx.z;
+  const int q0 = blockIdx.x * Cf::BQ, h = blockIdx.y, b = blockIdx.z;
   const int sqk = (p.qk_shared ? 0 : b) * p.H + h;           // slab of q / k
   const int sv = b * p.H + h;                                // slab of v
   const int nkv = (p.L + FA_BKV - 1) / FA_BKV;
@@ -195,9 +253,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
     mbar_init(q_full, 1);
-    for (int s = 0; s < FA_STAGES; ++s) {
+    for (int s = 0; s < STAGES; ++s) {
       mbar_init(kv_full(s), 1);
-      mbar_init(kv_empty(s), 8);                              // one arrival per consumer warp
+      mbar_init(kv_empty(s), 4 * Cf::CW);                     // one arrival per consumer warp
     }
     fence_mbar_init();
   }
@@ -218,7 +276,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
           tma_load_3d(st + a * Cf::KV_ATOM, &tm_k, kv_full(stage), 64 * a, j * FA_BKV, sqk);
           tma_load_3d(st + Cf::TILE_BYTES + a * Cf::KV_ATOM, &tm_v, kv_full(stage), 64 * a, j * FA_BKV, sv);
         }
-        if (++stage == FA_STAGES) { stage = 0; phase ^= 1u; }
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
     }
     return;
@@ -230,15 +288,12 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
 #pragma unroll
   for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
   float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};   // rows 16 wq + lane/4 and + 8 of the warpgroup's 64
+  float s[32], alpha[2];
+  uint32_t pa[4][4];                                            // P as the register A operand of the four 16-key steps
   const uint32_t qa = sq + cg * 64 * 128;
-  mbar_wait(q_full, 0);
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int j = 0; j < nkv; ++j) {
-    mbar_wait(kv_full(stage), phase);
-    const uint32_t kt = skv + stage * Cf::STAGE_BYTES, vt = kt + Cf::TILE_BYTES;
-    float s[32];
-    wgmma_fence();
+
+  auto issue_qk = [&](int st) {
+    const uint32_t kt = skv + st * Cf::STAGE_BYTES;
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
       const uint32_t off = (ks & 3) * 32u;   // k-step within the 64-column atom
@@ -246,55 +301,91 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
                           wgmma_desc_sw128_kmajor(kt + (ks >> 2) * Cf::KV_ATOM + off), ks != 0 ? 1u : 0u);
     }
     wgmma_commit();
-    wgmma_wait<0>();
-
-    // online softmax: thread holds rows r0 = lane/4 (s[4j], s[4j+1]) and r0 + 8 (s[4j+2], s[4j+3]), columns 8j + 2(lane%4)
-    const int kvalid = p.L - j * FA_BKV;
-    float mx[2] = {-INFINITY, -INFINITY};
+  };
+  auto issue_pv = [&](int st) {
+    const uint32_t vt = skv + st * Cf::STAGE_BYTES + Cf::TILE_BYTES;
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb)                // 16 keys per step: +16 rows x 128 B of the V tile
+      wgmma_rs_f16_bt<DV>(o, pa[kb], wgmma_desc_sw128_mnmajor(vt + kb * 2048u, Cf::KV_ATOM), 1u);
+    wgmma_commit();
+  };
+  auto fence_s = [&]() {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) reg_fence(s[i]);
+  };
+  auto fence_o = [&]() {
+#pragma unroll
+    for (int i = 0; i < DV / 2; ++i) reg_fence(o[i]);
+  };
+  auto pack_p = [&]() {
 #pragma unroll
     for (int n = 0; n < 8; ++n) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int col = n * 8 + 2 * (lane & 3) + (e & 1);
-        s[4 * n + e] = col < kvalid ? s[4 * n + e] * p.scale_log2 : -INFINITY;
-        mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * n + e]);
-      }
+      pa[n >> 1][(n & 1) * 2] = pack_f16x2(s[4 * n], s[4 * n + 1]);
+      pa[n >> 1][(n & 1) * 2 + 1] = pack_f16x2(s[4 * n + 2], s[4 * n + 3]);
     }
-    float alpha[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float m_new = fmaxf(m_r[r], mx[r]);   // finite: every tile holds at least one valid key
-      alpha[r] = ex2_approx(m_r[r] - m_new);
-      m_r[r] = m_new;
-      l_r[r] *= alpha[r];
-    }
+  };
+  auto softmax = [&](int j) {
+    if (j == nkv - 1) fa_softmax<true>(s, m_r, l_r, alpha, p.scale_log2, p.L - j * FA_BKV, lane);
+    else fa_softmax<false>(s, m_r, l_r, alpha, p.scale_log2, FA_BKV, lane);
+  };
+  auto release = [&](int st) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(kv_empty(st));     // this warp's MMAs on the stage have retired
+  };
+  // Issue turns: warpgroup cg waits on barrier 1 + cg and hands the turn to the next by arriving on its barrier.  Every
+  // warpgroup issues nkv + 1 times; the last one grants warpgroup 0's first turn up front and skips its last hand-over,
+  // so each barrier sees exactly as many arrivals as syncs.
+  const int turns = nkv + 1;
+  if (cg == Cf::CW - 1) bar_arrive_named(1, 256);
+  auto turn_begin = [&]() { bar_sync_named(1 + cg, 256); };
+  auto turn_end = [&](int t) {
+    if (cg != Cf::CW - 1 || t + 1 < turns) bar_arrive_named(1 + (cg + 1) % Cf::CW, 256);
+  };
+
+  mbar_wait(q_full, 0);
+  // tile 0: S only (O is still zero, so its rescale is skipped: 0 * alpha = 0)
+  mbar_wait(kv_full(0), 0);
+  turn_begin();
+  wgmma_fence();
+  issue_qk(0);
+  turn_end(0);
+  wgmma_wait<0>();
+  fence_s();
+  softmax(0);
+  pack_p();
+  int prev = 0, stage = 1;
+  uint32_t phase = 0;
+  if (stage == STAGES) { stage = 0; phase ^= 1u; }
+  for (int j = 1; j < nkv; ++j) {
+    mbar_wait(kv_full(stage), phase);
+    turn_begin();
+    wgmma_fence();
+    issue_qk(stage);
+    issue_pv(prev);
+    turn_end(j);
+    wgmma_wait<1>();                              // S_j has retired; P_{j-1} V_{j-1} may still run
+    fence_s();
+    softmax(j);
+    wgmma_wait<0>();
+    fence_o();
+    release(prev);
 #pragma unroll
     for (int n = 0; n < DV / 8; ++n) {
       o[4 * n] *= alpha[0]; o[4 * n + 1] *= alpha[0];
       o[4 * n + 2] *= alpha[1]; o[4 * n + 3] *= alpha[1];
     }
-    uint32_t pa[4][4];                            // P as the register A operand of the four 16-key steps
-#pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      const float p0 = ex2_approx(s[4 * n] - m_r[0]), p1 = ex2_approx(s[4 * n + 1] - m_r[0]);
-      const float p2 = ex2_approx(s[4 * n + 2] - m_r[1]), p3 = ex2_approx(s[4 * n + 3] - m_r[1]);
-      l_r[0] += p0 + p1;
-      l_r[1] += p2 + p3;
-      pa[n >> 1][(n & 1) * 2] = pack_f16x2(p0, p1);
-      pa[n >> 1][(n & 1) * 2 + 1] = pack_f16x2(p2, p3);
-    }
-    wgmma_fence();
-#pragma unroll
-    for (int kb = 0; kb < 4; ++kb)                // 16 keys per step: +16 rows x 128 B of the V tile
-      wgmma_rs_f16_bt<DV>(o, pa[kb], wgmma_desc_sw128_mnmajor(vt + kb * 2048u, Cf::KV_ATOM), 1u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(kv_empty(stage));  // this warp's MMAs on the stage have retired
-    if (++stage == FA_STAGES) { stage = 0; phase ^= 1u; }
+    pack_p();
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
   }
+  // P V of the last tile
+  turn_begin();
+  wgmma_fence();
+  issue_pv(prev);
+  turn_end(nkv);
+  wgmma_wait<0>();
+  fence_o();
+  release(prev);
 
   // O / l -> fp16, columns < head_dim
 #pragma unroll
@@ -320,9 +411,10 @@ int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, i
               int DP, float scale, int qk_shared, cudaStream_t stream) {
   using Cf = FaCfg<KS>;
   if (H > 65535 || B > 65535 || Cf::ATOMS * 64 > DP) return VTM_E_SHAPE;
+  constexpr int BQ = Cf::BQ;
   const uint64_t BH = static_cast<uint64_t>(B) * H;
   CUtensorMap tq, tk, tv;
-  int rc = make_tmap_3d_f16(&tq, qh, DP, Lq, BH, DP, static_cast<uint64_t>(Lq) * DP, 64, FA_BQ);
+  int rc = make_tmap_3d_f16(&tq, qh, DP, Lq, BH, DP, static_cast<uint64_t>(Lq) * DP, 64, BQ);
   if (rc) return rc;
   rc = make_tmap_3d_f16(&tk, kh, DP, L, BH, DP, static_cast<uint64_t>(L) * DP, 64, FA_BKV);
   if (rc) return rc;
@@ -344,8 +436,8 @@ int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, i
   p.L = L; p.Lq = Lq; p.H = H; p.d = C / H; p.C = C;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.qk_shared = qk_shared;
-  const dim3 grid(static_cast<unsigned>((Lq + FA_BQ - 1) / FA_BQ), static_cast<unsigned>(H), static_cast<unsigned>(B));
-  flash_attn_kernel<KS><<<grid, FA_THREADS, Cf::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  const dim3 grid(static_cast<unsigned>((Lq + BQ - 1) / BQ), static_cast<unsigned>(H), static_cast<unsigned>(B));
+  flash_attn_kernel<KS><<<grid, Cf::THREADS, Cf::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   return launch_rc();
 }
 

@@ -344,6 +344,14 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128_mnmajor(uint32_t smem_addr,
 __device__ __forceinline__ void bar_sync_named(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Arrive on a named barrier without waiting for it to complete.
+__device__ __forceinline__ void bar_arrive_named(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// Pins a register in program order relative to the surrounding asm volatile statements: the compiler may neither move
+// a read or write of it across a wgmma issue / wait nor assume its value is unchanged.  Applied to
+// wgmma accumulators right after the wait_group that retires them.
+__device__ __forceinline__ void reg_fence(float& x) { asm volatile("" : "+f"(x)::"memory"); }
 // Register budget of a warpgroup (all its warps execute it): producers give registers to the MMA warpgroups.
 template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
