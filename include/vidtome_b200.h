@@ -50,6 +50,14 @@ extern "C" {
  *     F % stride == 0, so that the src / dst counts do not depend on the draw (else VTM_E_SPLIT).
  *   mode 1 (global, prefix/suffix) — bipartite_soft_matching_2s, vidtome/merge.py:371-379:
  *     src = positions [0, src_len), dst = positions [src_len, N).
+ *     With `coin_dev` != NULL the global stage's coin (vidtome/patch.py:62, `torch.rand(1) > global_rand`) stays on the
+ *     device: the sequence is stored as [local tokens (first src_len rows) | global tokens (the other N - src_len)],
+ *     and the kernels compare the fp32 draw *coin_dev, widened to double, against `coin_threshold`:
+ *       coin > threshold:     src = [0, src_len), dst = [src_len, N)  (the reference's [local | global], patch.py:63-66);
+ *       otherwise:            src = [src_len, N), dst = [0, src_len)  (its [global | local], patch.py:68-71, with
+ *                             positions numbered in storage order).
+ *     Src row i and dst row j name the same tokens as in the reference either way.  Requires N == 2 * src_len, so
+ *     that no count depends on the draw (else VTM_E_SPLIT).
  */
 typedef struct vtm_split {
   int32_t mode;
@@ -61,6 +69,8 @@ typedef struct vtm_split {
   int32_t randf;
   int32_t src_len;
   const int32_t* randf_dev; /* optional device-resident randf (mode 0), NULL = use `randf` */
+  const float* coin_dev;    /* optional device-resident global coin (mode 1), NULL = plain prefix split */
+  double coin_threshold;    /* global_rand: the halves swap roles when !(coin > coin_threshold) */
 } vtm_split_t;
 
 /* Library version (VTM_VERSION).  Pure host. */

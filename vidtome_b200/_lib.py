@@ -18,7 +18,8 @@ LIB_PATH = os.environ.get("VIDTOME_B200_LIB") or os.path.join(_HERE, "libvidtome
 class VtmSplit(C.Structure):
     """struct vtm_split (include/vidtome_b200.h)."""
     _fields_ = [(n, C.c_int32) for n in
-                ("mode", "N", "unm_pre", "F", "tnum", "stride", "randf", "src_len")] + [("randf_dev", C.c_void_p)]
+                ("mode", "N", "unm_pre", "F", "tnum", "stride", "randf", "src_len")] + [
+                    ("randf_dev", C.c_void_p), ("coin_dev", C.c_void_p), ("coin_threshold", C.c_double)]
 
     @classmethod
     def local(cls, N: int, unm_pre: int, F: int, target_stride: int, randf) -> "VtmSplit":
@@ -38,6 +39,20 @@ class VtmSplit(C.Structure):
     @classmethod
     def prefix(cls, N: int, src_len: int) -> "VtmSplit":
         return cls(1, N, 0, 0, 0, 0, 0, src_len, None)
+
+    @classmethod
+    def prefix_coin(cls, L: int, coin, global_rand: float) -> "VtmSplit":
+        """The global stage's split with its coin left on the device: the sequence is stored as [local (L rows) |
+        global (L rows)], and the kernels read `coin` (a 1-element fp32 CUDA tensor, kept alive on the descriptor)
+        to pick the roles.  coin > global_rand: src = local, dst = global; otherwise src = global, dst = local."""
+        import torch
+        if not (isinstance(coin, torch.Tensor) and coin.is_cuda and coin.dtype == torch.float32 and coin.numel() == 1):
+            raise RuntimeError("VtmSplit.prefix_coin: coin must be a 1-element float32 CUDA tensor")
+        if not isinstance(L, int) or L <= 0:
+            raise RuntimeError(f"VtmSplit.prefix_coin: L must be a positive int, got {L!r}")
+        sp = cls(1, 2 * L, 0, 0, 0, 0, 0, L, None, coin.data_ptr(), float(global_rand))
+        sp._keepalive = coin
+        return sp
 
 
 _vp, _i32, _i64, _sz = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t

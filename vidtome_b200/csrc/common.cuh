@@ -5,6 +5,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include "../../include/vidtome_b200.h"
@@ -12,16 +13,23 @@
 namespace vtm {
 
 // Device-side copy of vtm_split_t plus derived counts.
+// A mode-1 split with a device coin is stored as the mode-0 split it equals: two "frames" of src_len tokens, stride 2,
+// no carried tokens, and the coin picks the dst frame (randf = 1: dst = [src_len, N); randf = 0: dst = [0, src_len)).
+// The position algebra below then serves it unchanged.
 struct Split {
   int mode, N, unm_pre, F, tnum, stride, randf, src_len;
   int nd_frames;  // local: number of dst frames = #{f in [0,F): f % stride == randf}
   int Ns, Nd;
   const int32_t* randf_dev;  // device-resident randf (NULL = the value above); see resolve_split()
+  const float* coin_dev;     // device-resident global coin (NULL = no swap)
+  float coin_floor;          // the largest float <= coin_threshold: for a float c, c > coin_floor <=> c > coin_threshold
 };
 
 // Kernels call this first: with a device-resident draw, fetch it (the counts do not depend on it, make_split).
+// The coin decides as the host path decides, `float(coin) > global_rand` in double precision (see coin_floor).
 __device__ __forceinline__ void resolve_split(Split& s) {
   if (s.randf_dev) s.randf = __ldg(s.randf_dev);
+  if (s.coin_dev) s.randf = __ldg(s.coin_dev) > s.coin_floor ? 1 : 0;
 }
 
 __host__ inline int make_split(const vtm_split_t* s, Split* o) {
@@ -29,6 +37,11 @@ __host__ inline int make_split(const vtm_split_t* s, Split* o) {
   o->mode = s->mode; o->N = s->N; o->unm_pre = s->unm_pre; o->F = s->F; o->tnum = s->tnum;
   o->stride = s->stride; o->randf = s->randf; o->src_len = s->src_len; o->nd_frames = 0;
   o->randf_dev = s->mode == 0 ? s->randf_dev : nullptr;
+  o->coin_dev = s->mode == 1 ? s->coin_dev : nullptr;
+  // round the threshold down to a float, so that the kernels compare in fp32 and decide exactly as the double
+  // comparison does (a NaN threshold stays NaN: never greater, as in double)
+  o->coin_floor = static_cast<float>(s->coin_threshold);
+  if (static_cast<double>(o->coin_floor) > s->coin_threshold) o->coin_floor = nextafterf(o->coin_floor, -INFINITY);
   if (s->N <= 0) return VTM_E_SPLIT;
   if (s->mode == 0) {
     if (o->randf_dev) {
@@ -47,6 +60,13 @@ __host__ inline int make_split(const vtm_split_t* s, Split* o) {
     o->Ns = s->N - o->Nd;
   } else if (s->mode == 1) {
     if (s->src_len < 0 || s->src_len > s->N) return VTM_E_SPLIT;
+    if (o->coin_dev) {
+      // the coin stays on the device: both halves must be equally long, so that swapping them changes no count
+      if ((long long)s->N != 2LL * s->src_len || s->src_len == 0) return VTM_E_SPLIT;
+      o->mode = 0; o->unm_pre = 0; o->F = 2; o->tnum = s->src_len; o->stride = 2;
+      o->randf = 1;   // [src | dst] until resolve_split reads the coin
+      o->nd_frames = 1;
+    }
     o->Ns = s->src_len;
     o->Nd = s->N - s->src_len;
   } else {

@@ -37,14 +37,21 @@ class ChunkedDenoiser:
     def __init__(self, unet: torch.nn.Module, n_timesteps: int = 50, chunk_size: int = 16,
                  guidance_scale: float = 7.5, merge_global: bool = False, chunk_ord: str = "seq",
                  perm_div: float = 3.0, randomize_chunks: bool = False, cond: Optional[torch.Tensor] = None,
-                 cuda_graph: bool = False, graph_warmup: int = 2, shard: bool = False):
+                 cuda_graph: bool = False, graph_warmup: int = 2, shard: bool = False, capture_global: bool = False):
         """`cuda_graph=True`: after `graph_warmup` eager steps, the noise prediction of a whole step (every chunk:
         CFG batch, UNet forward with the merge path, guidance combine) is captured once into a CUDA graph and
         replayed; per step the host then issues one graph launch plus the DDIM update instead of ~250 kernel
         launches.  The frame draws of the local matcher stay on the device (utils.draw_randf) and come from the
         blocks' generators, which are registered with the graph, so replays produce the same sequence of draws —
-        and bit-identical latents — as eager stepping.  Needs static shapes and chunk order: local merging only
-        (`merge_global=False`), `randomize_chunks=False`, frame counts divisible by the target stride."""
+        and bit-identical latents — as eager stepping.  Needs static shapes: `randomize_chunks=False`, frame counts
+        divisible by the target stride, and local merging only (`merge_global=False`) unless `capture_global=True`.
+
+        `capture_global=True` (with `merge_global=True, cuda_graph=True`) captures global merging too.  The graph runs
+        chunk *slots*: slot k takes a static [chunk_size, ...] input, and the global-token recurrence runs slot 0 -> K-1
+        inside the graph, with the coin of every block drawn on the device (patch.DEVICE_COIN).  Each step still draws
+        the chunk order on the host with get_chunks, exactly as eager stepping does, and applies it as data: one
+        index_select of the latents into the slots, one of the noise back.  Needs every chunk to be equally long
+        (frame count divisible by chunk_size), patch.GLOBAL_EXCHANGE == "recurrence", and no sharding."""
         self.unet = unet
         # shard=True: this process is one rank of a torch.distributed job and takes chunks i % world == rank of every
         # step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
@@ -52,10 +59,15 @@ class ChunkedDenoiser:
         self.shard = bool(shard)
         self.cuda_graph = bool(cuda_graph)
         self.graph_warmup = int(graph_warmup)
-        self._graph = None          # (CUDAGraph, static x, static timestep, static noise, shape)
+        self._graph = None          # (CUDAGraph, static x, static timestep, static noise, shape[, slot index state])
         self._eager_steps = 0
-        if self.cuda_graph and (merge_global or randomize_chunks):
+        self.capture_global = bool(capture_global)
+        if self.capture_global and not (self.cuda_graph and merge_global):
+            raise ValueError("capture_global=True needs cuda_graph=True and merge_global=True")
+        if self.cuda_graph and ((merge_global and not self.capture_global) or randomize_chunks):
             raise ValueError("cuda_graph=True needs merge_global=False and randomize_chunks=False (static work)")
+        if self.capture_global and self.shard:
+            raise ValueError("capture_global=True does not capture the cross-rank exchange of shard=True")
         self.chunk_size = chunk_size
         self.guidance_scale = guidance_scale
         self.merge_global = merge_global
@@ -164,14 +176,72 @@ class ChunkedDenoiser:
             gn = self._all_noises(gx, gt)
         self._graph = (graph, gx, gt, gn, tuple(x.shape))
 
+    @staticmethod
+    def slot_index(chunks: List[torch.Tensor], flen: int) -> torch.Tensor:
+        """[2, flen] int64 for a chunk list of equally long chunks: row 0 maps slot position s (slot k covers
+        [k * chunk_size, (k + 1) * chunk_size)) to the frame it processes, in the order the chunks are visited; row 1
+        is its inverse, frame -> slot position."""
+        fwd = torch.cat([c.to(torch.int64) for c in chunks])
+        if len(fwd) != flen or len({len(c) for c in chunks}) != 1:
+            raise RuntimeError("slot_index: the chunks must be equally long and cover every frame once")
+        inv = torch.empty_like(fwd)
+        inv[fwd] = torch.arange(flen)
+        if not torch.equal(fwd[inv], torch.arange(flen)):
+            raise RuntimeError("slot_index: the chunks must cover every frame exactly once")
+        return torch.stack([fwd, inv])
+
+    def _capture_slots(self, x: torch.Tensor, t: int):
+        """Capture the noise prediction of one step over chunk slots (capture_global=True): slot k runs chunk k of the
+        step's visiting order on gx[k * chunk_size:(k + 1) * chunk_size].  get_chunks is not called here, so capturing
+        consumes no draw of the host RNG that eager stepping would not."""
+        flen, cs = len(x), self.chunk_size
+        if patch.GLOBAL_EXCHANGE != "recurrence":
+            raise RuntimeError(f"capture_global=True needs patch.GLOBAL_EXCHANGE='recurrence' (got "
+                               f"{patch.GLOBAL_EXCHANGE!r}): the cross-rank exchange is not captured")
+        gx = x.clone()
+        gt = torch.tensor(int(t), device=x.device, dtype=torch.long)
+        graph = torch.cuda.CUDAGraph()
+        for g in self._block_generators():
+            graph.register_generator_state(g)
+        patch.update_patch(self.unet, global_tokens=None)                # slot 0 starts the recurrence afresh
+        torch.cuda.synchronize(x.device)
+        with torch.cuda.graph(graph):
+            gn = torch.zeros_like(gx)
+            for k in range(flen // cs):
+                gn[k * cs:(k + 1) * cs] = self.pred_noise(gx[k * cs:(k + 1) * cs], gt)
+        idx_dev = torch.empty((2, flen), dtype=torch.int64, device=x.device)
+        idx_host = torch.empty((2, flen), dtype=torch.int64).pin_memory()
+        copied = torch.cuda.Event()          # the pinned buffer is rewritten only after its last upload has run
+        self._graph = (graph, gx, gt, gn, tuple(x.shape), idx_dev, idx_host, copied)
+
+    def _slot_noises(self, x: torch.Tensor, t: int) -> torch.Tensor:
+        flen = len(x)
+        if flen % self.chunk_size != 0:
+            raise RuntimeError(f"capture_global=True needs a frame count divisible by chunk_size (got {flen} frames, "
+                               f"chunk_size {self.chunk_size}): chunks of unequal length cannot share one graph")
+        order = self.slot_index(self.get_chunks(flen), flen)        # the same host draws as eager stepping
+        if self._graph is None or self._graph[4] != tuple(x.shape):
+            self._capture_slots(x, t)
+        graph, gx, gt, gn, _, idx_dev, idx_host, copied = self._graph
+        copied.synchronize()
+        idx_host.copy_(order)
+        idx_dev.copy_(idx_host, non_blocking=True)
+        copied.record()
+        torch.index_select(x, 0, idx_dev[0], out=gx)                # latents -> slots
+        gt.fill_(int(t))
+        graph.replay()
+        return torch.index_select(gn, 0, idx_dev[1])                # slots -> frames
+
     # one iteration of generate.py:211-224
     @torch.no_grad()
     def step(self, x: torch.Tensor, i: int) -> torch.Tensor:
         t = self.timesteps[i]
-        if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup:
+        if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.capture_global:
+            noises = self._slot_noises(x, t)
+        elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup:
             if self._graph is None or self._graph[4] != tuple(x.shape):
                 self._capture(x, t)
-            graph, gx, gt, gn, _ = self._graph
+            graph, gx, gt, gn = self._graph[:4]
             gx.copy_(x, non_blocking=True)
             gt.fill_(int(t))
             graph.replay()

@@ -252,12 +252,17 @@ def merge_reduce(x: torch.Tensor, split: VtmSplit, r: int, keys: torch.Tensor, e
 
 
 def unmerge_add(y: torch.Tensor, row_map: torch.Tensor, resid: Optional[torch.Tensor]) -> torch.Tensor:
-    """KE.  out[b, p] = y[b, map[b, p]] (+ resid[b, p]).  y [B, L, C]; map [B'|1, N] int32; resid [B, N, C]."""
+    """KE.  out[b, p] = y[b, map[b, p]] (+ resid[b, p]).  y [B, L, C]; map [B'|1, N] int32 with contiguous rows (a
+    column slice of a wider map is read in place); resid [B, N, C]."""
     _require(y, torch.float16, "y")
-    _require(row_map, torch.int32, "map")
+    N = row_map.shape[1] if isinstance(row_map, torch.Tensor) else 0
+    if N and row_map.dim() == 2 and row_map.shape[0] > 1 and row_map.stride(1) == 1 and row_map.stride(0) > N:
+        _require(row_map[0], torch.int32, "map")                  # column slice: read in place through its row stride
+        map_bs = row_map.stride(0)
+    else:
+        _require(row_map, torch.int32, "map")
+        map_bs = 0 if row_map.shape[0] == 1 else N
     B, _, Cc = y.shape
-    N = row_map.shape[1]
-    map_bs = 0 if row_map.shape[0] == 1 else N
     if resid is not None:
         _require(resid, torch.float16, "resid")
     out = torch.empty((B, N, Cc), dtype=torch.float16, device=y.device)

@@ -22,7 +22,7 @@ import torch
 
 from . import merge, ops
 from ._lib import VtmSplit
-from .utils import (draw_randf, draw_scalar, func_warper, init_generator, isinstance_str, join_frame, join_warper,
+from .utils import (draw_coin, draw_randf, func_warper, init_generator, isinstance_str, join_frame, join_warper,
                     split_frame, split_warper)
 
 
@@ -35,7 +35,7 @@ class MergePlan:
     pi: torch.Tensor                      # [B'|1, N0] int32: out[b, p] = y[b, pi[b, p]]
     levels: List[merge.LevelMatch] = field(default_factory=list)
     randf: List[Any] = field(default_factory=list)      # ints (eager) or 1-element int32 CUDA tensors (graph capture)
-    coin: Optional[float] = None
+    coin: Any = None                      # float (host coin) or 1-element fp32 CUDA tensor (device coin, DEVICE_COIN / capture)
     mu: Optional[torch.Tensor] = None     # [B'|1, L_local] int32: local merged token i = table row mu[i] (before a global stage)
 
     def unmerge(self, y: torch.Tensor, **kwarg) -> torch.Tensor:
@@ -68,6 +68,12 @@ FUSE_CROSS_ATTENTION = True
 #   "p2p_all"    — as "p2p" but into every rank's buffer (all-gather semantics; 7x the bytes on 8 GPUs).
 GLOBAL_EXCHANGE = "recurrence"
 
+# Keep the global stage's coin (patch.py:62) on the device, as CUDA-graph capture always does: the local and global
+# token sets sit in one buffer in a fixed order and the kernels read the coin to pick which half is src
+# (VtmSplit.prefix_coin), so nothing is read back to the host.  Results are bit-identical to the host coin.  It needs
+# both sets to be equally long (equal chunks); eagerly, a block whose sets differ keeps the host coin.
+DEVICE_COIN = False
+
 
 def _fusable_layer_norm(norm: torch.nn.Module, x: torch.Tensor):
     """(weight, bias, eps) if `norm` is a stock affine nn.LayerNorm over the channel dim in fp16, else None."""
@@ -76,6 +82,37 @@ def _fusable_layer_norm(norm: torch.nn.Module, x: torch.Tensor):
     if tuple(norm.normalized_shape) != (x.shape[-1],) or norm.weight.dtype != torch.float16 or not norm.weight.is_cuda:
         return None
     return (norm.weight.contiguous(), None if norm.bias is None else norm.bias.contiguous(), float(norm.eps))
+
+
+def _global_stage_device_coin(module, table, mu, pi, g, ln, args, levels):
+    """patch.py:60-80 with the coin left on the device.  The reference concatenates [local | global] or
+    [global | local] depending on the coin; here both sets are stored once as cat = [local (L rows) | global (L rows)]
+    and the coin picks which half is src (VtmSplit.prefix_coin).  Src row i and dst row j name the same tokens as in
+    the reference's concatenation, so the match, the merged tokens and the unmerge are the same; only positions are
+    numbered in storage order, which is what makes the local tokens' unmerge map tau[:, :L] independent of the coin.
+    Returns (merged tokens, composed unmerge map, coin tensor)."""
+    B, _, C = table.shape
+    L = mu.shape[1]
+    coin = draw_coin(module.generator, on_device=True)                      # patch.py:62
+    gratio = args["global_merge_ratio"]
+    if gratio <= 0:
+        raise ValueError("not enough values to unpack (expected 3, got 2)")  # as the host-coin path
+    cat = torch.empty((B, 2 * L, C), dtype=torch.float16, device=table.device)
+    ops.gather_rows(table, mu, ln=ln, out=cat[:, :L])                       # merged local tokens, straight into cat
+    cat[:, L:].copy_(g)                                                     # the stored global tokens
+    split = VtmSplit.prefix_coin(L, coin, args["global_rand"])
+    m = merge.match_level(cat, None, split, gratio, bool(args["align_batch"]))   # patch.py:73-74
+    levels.append(m)
+    # tau: position in cat -> position in the merged sequence
+    mu_g, tau = ops.compose_maps(split, m.r, m.keys, m.edge, m.rank, None, None, 0, 2 * L)
+    merged_tokens = ops.gather_rows(cat, mu_g)                               # patch.py:75
+    # patch.py:80: global_tokens <- u(merged_tokens), the local half after unmerging (kept on the device)
+    module.global_tokens = ops.unmerge_add(merged_tokens, tau[:, :L], None)
+    # compose with the local unmerge: pi_total[p] = tau[pi[p]]
+    if pi.shape[0] != tau.shape[0]:
+        pi = pi.expand(tau.shape[0], -1).contiguous()
+    _, pi = ops.compose_maps(split, m.r, m.keys, m.edge, m.rank, None, pi, 0, pi.shape[1])
+    return merged_tokens, pi, coin
 
 
 def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[str, Any],
@@ -124,6 +161,21 @@ def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[s
     coin = None
     if args["merge_global"]:                                                 # patch.py:59
         g = getattr(module, "global_tokens", None)
+        if x.is_cuda and torch.cuda.is_current_stream_capturing():
+            if GLOBAL_EXCHANGE != "recurrence":
+                raise RuntimeError(f"CUDA-graph capture of global merging needs GLOBAL_EXCHANGE='recurrence' (got "
+                                   f"{GLOBAL_EXCHANGE!r}): the cross-rank exchange is not captured")
+            if g is not None and g.shape[1] != L:
+                raise RuntimeError(f"CUDA-graph capture of global merging needs chunks of equal length, i.e. a frame "
+                                   f"count divisible by the chunk size (got {L} local and {g.shape[1]} global tokens): "
+                                   f"token counts would depend on the draw")
+            device_coin = True
+        else:
+            device_coin = DEVICE_COIN and GLOBAL_EXCHANGE == "recurrence" and g is not None and g.shape[1] == L
+        if device_coin and g is not None:
+            merged_tokens, pi, coin = _global_stage_device_coin(module, table, mu, pi, g, ln, args, levels)
+            return MergePlan(fsize=fsize, N0=N0, merged_tokens=merged_tokens, pi=pi, levels=levels, randf=randfs,
+                             coin=coin, mu=mu)
         exchanged = False
         local_tokens = None
         if GLOBAL_EXCHANGE in ("allgather", "p2p", "p2p_all"):
@@ -145,8 +197,7 @@ def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[s
         if local_tokens is None:
             local_tokens = ops.gather_rows(table, mu, ln=ln)                 # merged local tokens [B, L, C]
         if g is not None:                                                    # patch.py:60
-            coin = float(draw_scalar(generator, lambda: torch.rand(
-                1, generator=generator, device=generator.device)))                            # patch.py:62
+            coin = draw_coin(generator, on_device=False)                     # patch.py:62
             g = g.to(local_tokens).contiguous()                              # patch.py:65,70
             Lg = g.shape[1]
             if coin > args["global_rand"]:

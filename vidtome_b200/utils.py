@@ -90,3 +90,20 @@ def draw_randf(generator: torch.Generator, stride: int, frames: int):
         return fn().to(torch.int32)
     return int(draw_scalar(generator, fn))
 
+
+def draw_coin(generator: torch.Generator, on_device: bool = None):
+    """The global stage's `torch.rand(1)` of vidtome/patch.py:62 (which token set is src).  By default (on_device=None)
+    the Python float, read back through the side stream of draw_scalar, except while the current stream is being
+    captured into a CUDA graph: then the 1-element fp32 CUDA tensor itself, which the kernels dereference
+    (vtm_split_t.coin_dev; the generator must be registered with the graph).  on_device=True asks for the tensor
+    eagerly too.  Both forms are one draw that advances the generator by the same offset."""
+    def fn():
+        return torch.rand(1, generator=generator, device=generator.device)
+    if on_device is None:
+        on_device = generator.device.type == "cuda" and torch.cuda.is_current_stream_capturing()
+    if on_device:
+        if generator.device.type != "cuda":
+            raise RuntimeError("draw_coin: a device-resident coin needs a CUDA generator")
+        return fn()
+    return float(draw_scalar(generator, fn))
+
