@@ -58,6 +58,14 @@ extern "C" {
  *                             positions numbered in storage order).
  *     Src row i and dst row j name the same tokens as in the reference either way.  Requires N == 2 * src_len, so
  *     that no count depends on the draw (else VTM_E_SPLIT).
+ *   mode 2 (global, device counts) — the mode-1 coin split for token sets of different lengths, where the counts
+ *     depend on the draw: the sequence is stored as [local (src_len rows, host-known) | global (*glob_len_dev rows, at
+ *     most glob_cap)], N == src_len + glob_cap is its capacity, and coin_dev / coin_threshold pick the src half as in
+ *     mode 1 (coin > threshold: src = local; otherwise src = global; positions in storage order).  Ns, Nd, r and the
+ *     merged length live on the device (vtm_split_counts_dev) and the *_dev entry points below read them; buffers are
+ *     sized for capacity (vtm_split_counts returns cap = max(src_len, glob_cap) for both counts).  The fields
+ *     glob_len_dev and glob_cap are read only in this mode, so a caller may pass the 56-byte form of the struct
+ *     for modes 0 and 1.
  */
 typedef struct vtm_split {
   int32_t mode;
@@ -71,7 +79,12 @@ typedef struct vtm_split {
   const int32_t* randf_dev; /* optional device-resident randf (mode 0), NULL = use `randf` */
   const float* coin_dev;    /* optional device-resident global coin (mode 1), NULL = plain prefix split */
   double coin_threshold;    /* global_rand: the halves swap roles when !(coin > coin_threshold) */
+  const int32_t* glob_len_dev; /* mode 2: device-resident length of the global set, 1 <= *glob_len_dev <= glob_cap */
+  int32_t glob_cap;            /* mode 2: capacity of the global set */
 } vtm_split_t;
+
+/* Length of the device counts record written by vtm_split_counts_dev: {Ns, Nd, r, M = Ns - r + Nd}. */
+#define VTM_COUNTS_LEN 4
 
 /* Library version (VTM_VERSION).  Pure host. */
 int vtm_version(void);
@@ -85,6 +98,11 @@ int vtm_split_counts(const vtm_split_t* split, int32_t* num_src, int32_t* num_ds
 
 /* Host helper: r = min(Ns, int(Ns * ratio)) with Python-double truncation (merge.py:90, :395). */
 int32_t vtm_merge_count(int32_t num_src, double ratio);
+
+/* Device counts of a mode-2 split: one tiny kernel resolves the coin and the global length and writes
+ * counts_dev[0..3] = {Ns, Nd, r = min(Ns, int(Ns * ratio)) in double as vtm_merge_count, M = Ns - r + Nd}.
+ * Nothing is read back to the host.  Other modes: VTM_E_SPLIT. */
+int vtm_split_counts_dev(const vtm_split_t* split, double ratio, int32_t* counts_dev, void* stream);
 
 /*
  * K0 — row-normalise and split.  Replaces `metric / metric.norm(dim=-1, keepdim=True)` followed by
@@ -139,6 +157,14 @@ int vtm_sim_argmax_pair(const void* a_dev, const void* b_dev, int32_t B, int32_t
 int vtm_sim_argmax_simt(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd,
                         int32_t C, int32_t align_batch, uint64_t* keys_out_dev, void* stream);
 
+/* KA with device counts (mode-2 splits): a_dev [B, ns_cap, C] and b_dev [B, nd_cap, C] as vtm_normalize_split writes
+ * them for such a split; Ns = counts_dev[0] and Nd = counts_dev[1] are read on the device.  Src rows >= Ns publish
+ * nothing and dst columns >= Nd take no part; keys_out_dev is [B', ns_cap] (row stride ns_cap), zeroed first.  The keys
+ * of the first Ns rows equal those of vtm_sim_argmax called with the same counts as host values.  Only the default
+ * one-CTA build has this path. */
+int vtm_sim_argmax_dev(const void* a_dev, const void* b_dev, int32_t B, int32_t ns_cap, int32_t nd_cap, int32_t C,
+                       int32_t align_batch, const int32_t* counts_dev, uint64_t* keys_out_dev, void* stream);
+
 /* Unpack helpers for KA keys (pure host; the same bit rules are used on the device). */
 uint16_t vtm_key_score_half_bits(uint64_t key); /* fp16 bit pattern of the row maximum */
 uint32_t vtm_key_arg(uint64_t key);             /* arg as defined above */
@@ -175,6 +201,16 @@ int vtm_compose_maps(const vtm_split_t* split, int32_t r, int32_t Ns, int32_t Nd
                      const int32_t* mu_in_dev, const int32_t* pi_in_dev, int32_t pi_offset, int32_t N0,
                      int32_t* mu_out_dev, int32_t* pi_out_dev, void* stream);
 
+/* KB1 / KB2 with device counts (mode-2 splits).  keys, edge and rank are [Bp, ns_cap] with row stride ns_cap and only
+ * their first counts_dev[0] entries per row take part.  vtm_compose_maps_dev reads Ns, Nd and r from counts_dev; mu_out is
+ * [Bp, split->N] (its first M entries are meaningful), pi_out is [Bp, N0]; with pi_in_dev == NULL only the first
+ * src_len + *glob_len_dev entries of pi_out are written.  mu_in_dev is not supported (NULL). */
+int vtm_topr_sort_dev(const uint64_t* keys_dev, int32_t Bp, int32_t ns_cap, const int32_t* counts_dev, int32_t* edge_dev,
+                      int32_t* rank_dev, void* ws_dev, size_t ws_bytes, void* stream);
+int vtm_compose_maps_dev(const vtm_split_t* split, const int32_t* counts_dev, int32_t Bp, const uint64_t* keys_dev,
+                         const int32_t* edge_dev, const int32_t* rank_dev, const int32_t* pi_in_dev, int32_t N0,
+                         int32_t* mu_out_dev, int32_t* pi_out_dev, void* stream);
+
 /* Decode KA/KB1 results into the reference's own index tensors (int64, as torch returns them):
  * unm_idx = edge[r:], src_idx = edge[:r], dst_idx = node_idx[src_idx] (% Nd when align_batch)
  * (vidtome/merge.py:100-108,115-117).  node_max_dev (fp16 bits) / node_idx_dev may be NULL. */
@@ -207,6 +243,12 @@ int vtm_gather_rows_peers(const void* x_dev, int64_t x_batch_stride, const int32
 int vtm_gather_rows_ln(const void* x_dev, int64_t x_batch_stride, const int32_t* map_dev,
                        int64_t map_batch_stride, int32_t B, int32_t L, int32_t C, const void* ln_weight_dev,
                        const void* ln_bias_dev, float ln_eps, void* y_dev, int64_t y_batch_stride, void* stream);
+
+/* KC with a device row count: rows i < *len_dev are gathered as in vtm_gather_rows, rows [*len_dev, L_cap) are written
+ * as zeros (so that nothing stale or non-finite reaches a kernel that runs over capacity). */
+int vtm_gather_rows_dev(const void* x_dev, int64_t x_batch_stride, const int32_t* map_dev, int64_t map_batch_stride,
+                        int32_t B, int32_t L_cap, int32_t C, const int32_t* len_dev, void* y_dev, int64_t y_batch_stride,
+                        void* stream);
 
 /*
  * Merge with a reduction — the non-"replace" modes of the merge closure, vidtome/merge.py:126-131:
@@ -256,6 +298,15 @@ int vtm_attention(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev,
 int vtm_attention_ex(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
                      int32_t B, int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, void* y_dev,
                      void* ws_dev, size_t ws_bytes, void* stream);
+
+/* KD with a device sequence length: x_dev / y_dev are [B, L_cap, C] and the sequence is the first *len_dev rows of each
+ * sample (1 <= *len_dev <= L_cap).  The projections run over all L_cap rows (rows are independent; rows past the length
+ * must be finite, e.g. the zeros of vtm_gather_rows_dev), the flash kernel reads the length on the device, and rows
+ * < *len_dev of y equal those of vtm_attention_ex called with L = *len_dev, bit for bit.  Rows past it are unspecified.
+ * Workspace: vtm_attention_workspace_bytes(B, L_cap, C, heads). */
+int vtm_attention_dev(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
+                      int32_t B, int32_t L_cap, int32_t C, int32_t heads, float scale, int32_t flags,
+                      const int32_t* len_dev, void* y_dev, void* ws_dev, size_t ws_bytes, void* stream);
 
 /* Plain wgmma GEMM used by KD's projections, exported for tests and the microbench:
  * D[M, N] = A[M, K] * W[N, K]^T (+ bias[N]), fp16 in, fp32 accumulate, fp16 out.  K % 8 == 0,

@@ -55,6 +55,33 @@ class VtmSplit(C.Structure):
         return sp
 
 
+    @classmethod
+    def prefix_coin_dev(cls, L: int, glob_len_dev, glob_cap: int, coin, global_rand: float) -> "VtmSplitDev":
+        """The global stage's split when the two token sets may differ in length (mode 2): the sequence is stored as
+        [local (L rows) | global (*glob_len_dev rows, at most glob_cap)], and the coin picks the src half as in
+        prefix_coin.  The counts that follow from the draw (Ns, Nd, r, the merged length) stay on the device
+        (ops.split_counts_dev); `glob_len_dev` is a 1-element int32 CUDA tensor, kept alive on the descriptor with
+        the coin."""
+        import torch
+        if not (isinstance(coin, torch.Tensor) and coin.is_cuda and coin.dtype == torch.float32 and coin.numel() == 1):
+            raise RuntimeError("VtmSplit.prefix_coin_dev: coin must be a 1-element float32 CUDA tensor")
+        if not (isinstance(glob_len_dev, torch.Tensor) and glob_len_dev.is_cuda and glob_len_dev.dtype == torch.int32
+                and glob_len_dev.numel() == 1):
+            raise RuntimeError("VtmSplit.prefix_coin_dev: glob_len_dev must be a 1-element int32 CUDA tensor")
+        if not isinstance(L, int) or L <= 0 or not isinstance(glob_cap, int) or glob_cap <= 0:
+            raise RuntimeError(f"VtmSplit.prefix_coin_dev: L and glob_cap must be positive ints, got {L!r}, {glob_cap!r}")
+        sp = VtmSplitDev(2, L + glob_cap, 0, 0, 0, 0, 0, L, None, coin.data_ptr(), float(global_rand),
+                         glob_len_dev.data_ptr(), glob_cap)
+        sp._keepalive = (coin, glob_len_dev)
+        return sp
+
+
+class VtmSplitDev(VtmSplit):
+    """struct vtm_split with its mode-2 tail (glob_len_dev, glob_cap): the full C layout.  The library reads the tail
+    only for mode 2, so VtmSplit itself keeps the shorter layout for modes 0 and 1."""
+    _fields_ = [("glob_len_dev", C.c_void_p), ("glob_cap", C.c_int32)]
+
+
 _vp, _i32, _i64, _sz = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
 _SPL = C.POINTER(VtmSplit)
 
@@ -89,6 +116,13 @@ SIGNATURES = {
     "vtm_cross_attention_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32]),
     "vtm_cross_attention": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, C.c_float,
                                       _vp, _vp, _sz, _vp]),
+    "vtm_split_counts_dev": (C.c_int, [_SPL, C.c_double, _vp, _vp]),
+    "vtm_sim_argmax_dev": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "vtm_topr_sort_dev": (C.c_int, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "vtm_compose_maps_dev": (C.c_int, [_SPL, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "vtm_gather_rows_dev": (C.c_int, [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
+    "vtm_attention_dev": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, C.c_float, _i32, _vp, _vp, _vp, _sz,
+                                    _vp]),
     "vtm_linear_f16": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _i64, _vp]),
     "vtm_linear_geglu_f16": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _i64, _vp]),
     "vtm_linear_residual_f16": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp]),

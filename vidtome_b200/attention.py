@@ -7,6 +7,8 @@ projections) goes through the module itself, exactly as the reference does at pa
 """
 from __future__ import annotations
 
+from typing import Optional
+
 import torch
 
 from . import _lib, ops
@@ -30,13 +32,15 @@ def _packed_weights(attn: torch.nn.Module, like: torch.Tensor):
     return cache[1:]
 
 
-def self_attention(attn: torch.nn.Module, x: torch.Tensor, shared_qk: bool = False) -> torch.Tensor:
+def self_attention(attn: torch.nn.Module, x: torch.Tensor, shared_qk: bool = False,
+                   seq_len: Optional[torch.Tensor] = None) -> torch.Tensor:
     """softmax(q k^T * scale) v with q,k,v = to_q/to_k/to_v(x), then to_out[0] (utils/pnp_utils.py:47-95).
-    shared_qk: PnP injection — q and k of sample 0 for every sample (utils/pnp_utils.py:57-68,87-91)."""
+    shared_qk: PnP injection — q and k of sample 0 for every sample (utils/pnp_utils.py:57-68,87-91).
+    seq_len: the sequence is the first seq_len (a 1-element int32 CUDA tensor) rows of x (GlobalTokenStore stage)."""
     w_qkv, w_o, b_o = _packed_weights(attn, x)
     heads = int(attn.heads)
     scale = float(getattr(attn, "scale", (x.shape[-1] // heads) ** -0.5))
-    return ops.attention(x, w_qkv, w_o, b_o, heads, scale, shared_qk=shared_qk)
+    return ops.attention(x, w_qkv, w_o, b_o, heads, scale, shared_qk=shared_qk, seq_len=seq_len)
 
 
 def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:

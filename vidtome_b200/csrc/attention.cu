@@ -145,6 +145,7 @@ constexpr int FA_BKV = 64;       // keys per K/V tile
 struct FaParams {
   __half* o;          // [B*Lq, C]
   int L, Lq, H, d, C;
+  const int* len_dev; // DL: the sequence length on the device (self-attention, <= L == Lq, the buffers' row count)
   float scale_log2;   // softmax scale * log2(e)
   int qk_shared;      // PnP injection (utils/pnp_utils.py:57-68,87-91): q and k of sample 0 for every sample, v per sample
 };
@@ -226,7 +227,9 @@ __device__ __forceinline__ void fa_softmax(float (&s)[32], float (&m_r)[2], floa
 // as a serial loop: O_j = O_{j-1} * alpha_j + P_j V_j.  The stage of tile j-1 is released once its P V has retired.
 // The consumer warpgroups take turns at issuing their MMAs (named barriers 1 .. CW, round robin), so that the MMAs of
 // one run on the tensor cores while the others are in their softmax.
-template <int KS>
+// DL (device length): the buffers hold p.L rows per head and sample, of which the first *p.len_dev are the sequence.  Query
+// tiles at or past it exit, and only keys below it take part, masked in the last tile exactly as keys past p.L are.
+template <int KS, bool DL = false>
 __global__ void __launch_bounds__(FaCfg<KS>::THREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                   const __grid_constant__ CUtensorMap tm_v, const FaParams p) {
@@ -244,9 +247,12 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const int q0 = blockIdx.x * Cf::BQ, h = blockIdx.y, b = blockIdx.z;
+  const int seq = DL ? __ldg(p.len_dev) : p.L;               // keys that take part
+  const int q_valid = DL ? seq : p.Lq;                       // query rows that are written
+  if (DL && q0 >= q_valid) return;
   const int sqk = (p.qk_shared ? 0 : b) * p.H + h;           // slab of q / k
   const int sv = b * p.H + h;                                // slab of v
-  const int nkv = (p.L + FA_BKV - 1) / FA_BKV;
+  const int nkv = (seq + FA_BKV - 1) / FA_BKV;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_q);
@@ -325,7 +331,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     }
   };
   auto softmax = [&](int j) {
-    if (j == nkv - 1) fa_softmax<true>(s, m_r, l_r, alpha, p.scale_log2, p.L - j * FA_BKV, lane);
+    if (j == nkv - 1) fa_softmax<true>(s, m_r, l_r, alpha, p.scale_log2, seq - j * FA_BKV, lane);
     else fa_softmax<false>(s, m_r, l_r, alpha, p.scale_log2, FA_BKV, lane);
   };
   auto release = [&](int st) {
@@ -395,7 +401,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = 1.f / l;
     const int row = q0 + cg * 64 + wq * 16 + (lane >> 2) + 8 * r;
-    if (row >= p.Lq) continue;
+    if (row >= q_valid) continue;
     __half* dst = p.o + (static_cast<size_t>(b) * p.Lq + row) * p.C + h * p.d;
 #pragma unroll
     for (int n = 0; n < DV / 8; ++n) {
@@ -406,9 +412,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
   }
 }
 
-template <int KS>
+template <int KS, bool DL = false>
 int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, int B, int Lq, int L, int C, int H,
-              int DP, float scale, int qk_shared, cudaStream_t stream) {
+              int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev = nullptr) {
   using Cf = FaCfg<KS>;
   if (H > 65535 || B > 65535 || Cf::ATOMS * 64 > DP) return VTM_E_SHAPE;
   constexpr int BQ = Cf::BQ;
@@ -426,7 +432,7 @@ int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, i
   rc = cuda_rc(cudaGetDevice(&dev));
   if (rc) return rc;
   if (dev < 0 || dev >= 64 || !opted[dev]) {
-    rc = cuda_rc(cudaFuncSetAttribute(flash_attn_kernel<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    rc = cuda_rc(cudaFuncSetAttribute(flash_attn_kernel<KS, DL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       static_cast<int>(Cf::SMEM_BYTES)));
     if (rc) return rc;
     if (dev >= 0 && dev < 64) opted[dev] = true;
@@ -436,23 +442,30 @@ int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, i
   p.L = L; p.Lq = Lq; p.H = H; p.d = C / H; p.C = C;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.qk_shared = qk_shared;
+  p.len_dev = len_dev;
   const dim3 grid(static_cast<unsigned>((Lq + BQ - 1) / BQ), static_cast<unsigned>(H), static_cast<unsigned>(B));
-  flash_attn_kernel<KS><<<grid, Cf::THREADS, Cf::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  flash_attn_kernel<KS, DL><<<grid, Cf::THREADS, Cf::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   return launch_rc();
 }
 
 int launch_fa_any(const __half* qh, const __half* kh, const __half* vh, __half* o, int B, int Lq, int L, int C, int H,
-                  int DP, float scale, int qk_shared, cudaStream_t stream) {
+                  int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev = nullptr) {
+#define VTM_FA_CASE(KS)                                                                                       \
+  case KS:                                                                                                    \
+    return len_dev ? launch_fa<KS, true>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream, len_dev) \
+                   : launch_fa<KS>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
   switch ((C / H + 15) / 16) {
-    case 1: return launch_fa<1>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
-    case 2: return launch_fa<2>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
-    case 3: return launch_fa<3>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
-    case 4: return launch_fa<4>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
-    case 5: return launch_fa<5>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
-    case 6: return launch_fa<6>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
-    case 7: return launch_fa<7>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
-    default: return launch_fa<8>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
+    VTM_FA_CASE(1)
+    VTM_FA_CASE(2)
+    VTM_FA_CASE(3)
+    VTM_FA_CASE(4)
+    VTM_FA_CASE(5)
+    VTM_FA_CASE(6)
+    VTM_FA_CASE(7)
+    default:
+    VTM_FA_CASE(8)
   }
+#undef VTM_FA_CASE
 }
 
 }  // namespace
@@ -468,10 +481,12 @@ extern "C" size_t vtm_attention_workspace_bytes(int32_t B, int32_t L, int32_t C,
   return (static_cast<size_t>(3) * B * heads * L * DP + static_cast<size_t>(B) * L * C) * 2 + 256;
 }
 
-extern "C" int vtm_attention_ex(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
-                                int32_t B, int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, void* y_dev,
-                                void* ws_dev, size_t ws_bytes, void* stream_) {
-  using namespace vtm;
+namespace vtm {
+namespace {
+// len_dev: NULL, or the sequence length on the device with L the rows of the buffers (vtm_attention_dev)
+int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev, int32_t B,
+                   int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, const int32_t* len_dev, void* y_dev,
+                   void* ws_dev, size_t ws_bytes, void* stream_) {
   if (!x_dev || !w_qkv_dev || !w_o_dev || !y_dev || !ws_dev) return VTM_E_NULL;
   if (B <= 0 || L <= 0 || C <= 0 || heads <= 0 || C % heads != 0) return VTM_E_SHAPE;
   const int d = C / heads;
@@ -487,9 +502,26 @@ extern "C" int vtm_attention_ex(const void* x_dev, const void* w_qkv_dev, const 
   if (rc) return rc;
   const __half* kh = qkv + static_cast<size_t>(B) * heads * L * DP;
   const __half* vh = kh + static_cast<size_t>(B) * heads * L * DP;
-  rc = launch_fa_any(qkv, kh, vh, o, B, L, L, C, heads, DP, scale, flags & 1, stream);
+  rc = launch_fa_any(qkv, kh, vh, o, B, L, L, C, heads, DP, scale, flags & 1, stream, len_dev);
   if (rc) return rc;
   return vtm_linear_f16(o, w_o_dev, b_o_dev, M, C, C, y_dev, C, stream_);
+}
+}  // namespace
+}  // namespace vtm
+
+extern "C" int vtm_attention_ex(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
+                                int32_t B, int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, void* y_dev,
+                                void* ws_dev, size_t ws_bytes, void* stream_) {
+  return vtm::attention_impl(x_dev, w_qkv_dev, w_o_dev, b_o_dev, B, L, C, heads, scale, flags, nullptr, y_dev, ws_dev,
+                             ws_bytes, stream_);
+}
+
+extern "C" int vtm_attention_dev(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
+                                 int32_t B, int32_t L_cap, int32_t C, int32_t heads, float scale, int32_t flags,
+                                 const int32_t* len_dev, void* y_dev, void* ws_dev, size_t ws_bytes, void* stream_) {
+  if (!len_dev) return VTM_E_NULL;
+  return vtm::attention_impl(x_dev, w_qkv_dev, w_o_dev, b_o_dev, B, L_cap, C, heads, scale, flags, len_dev, y_dev,
+                             ws_dev, ws_bytes, stream_);
 }
 
 extern "C" int vtm_attention(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,

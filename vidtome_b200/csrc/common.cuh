@@ -23,13 +23,27 @@ struct Split {
   const int32_t* randf_dev;  // device-resident randf (NULL = the value above); see resolve_split()
   const float* coin_dev;     // device-resident global coin (NULL = no swap)
   float coin_floor;          // the largest float <= coin_threshold: for a float c, c > coin_floor <=> c > coin_threshold
+  // mode 2 (device counts): src_len = L local rows, the global set's length is *glob_len_dev (<= gcap); randf = 1 when the
+  // local half is src.  On the host N, Ns and Nd hold capacities (src_len + gcap, cap, cap); resolve_split sets them.
+  const int32_t* glob_len_dev;
+  int gcap;
+  int cap;                   // mode 2: max(src_len, gcap), the row stride of the src / dst buffers (0 in other modes)
 };
 
 // Kernels call this first: with a device-resident draw, fetch it (the counts do not depend on it, make_split).
 // The coin decides as the host path decides, `float(coin) > global_rand` in double precision (see coin_floor).
+// DC: the kernel serves device-count (mode 2) splits; without it that code is compiled out, so the kernels that never see
+// one keep their register budgets.
+template <bool DC = false>
 __device__ __forceinline__ void resolve_split(Split& s) {
   if (s.randf_dev) s.randf = __ldg(s.randf_dev);
   if (s.coin_dev) s.randf = __ldg(s.coin_dev) > s.coin_floor ? 1 : 0;
+  if (DC && s.glob_len_dev) {
+    const int lg = __ldg(s.glob_len_dev);
+    s.N = s.src_len + lg;
+    s.Ns = s.randf ? s.src_len : lg;
+    s.Nd = s.randf ? lg : s.src_len;
+  }
 }
 
 __host__ inline int make_split(const vtm_split_t* s, Split* o) {
@@ -37,7 +51,8 @@ __host__ inline int make_split(const vtm_split_t* s, Split* o) {
   o->mode = s->mode; o->N = s->N; o->unm_pre = s->unm_pre; o->F = s->F; o->tnum = s->tnum;
   o->stride = s->stride; o->randf = s->randf; o->src_len = s->src_len; o->nd_frames = 0;
   o->randf_dev = s->mode == 0 ? s->randf_dev : nullptr;
-  o->coin_dev = s->mode == 1 ? s->coin_dev : nullptr;
+  o->coin_dev = s->mode == 1 || s->mode == 2 ? s->coin_dev : nullptr;
+  o->glob_len_dev = nullptr; o->gcap = 0; o->cap = 0;
   // round the threshold down to a float, so that the kernels compare in fp32 and decide exactly as the double
   // comparison does (a NaN threshold stays NaN: never greater, as in double)
   o->coin_floor = static_cast<float>(s->coin_threshold);
@@ -69,6 +84,17 @@ __host__ inline int make_split(const vtm_split_t* s, Split* o) {
     }
     o->Ns = s->src_len;
     o->Nd = s->N - s->src_len;
+  } else if (s->mode == 2) {
+    // the tail fields exist only in this mode (modes 0 and 1 may pass the shorter form of the struct)
+    if (!s->coin_dev || !s->glob_len_dev || s->src_len <= 0 || s->glob_cap <= 0 ||
+        (long long)s->N != (long long)s->src_len + s->glob_cap)
+      return VTM_E_SPLIT;
+    o->glob_len_dev = s->glob_len_dev;
+    o->gcap = s->glob_cap;
+    o->cap = s->src_len > s->glob_cap ? s->src_len : s->glob_cap;
+    o->randf = 1;
+    o->Ns = o->cap;
+    o->Nd = o->cap;
   } else {
     return VTM_E_SPLIT;
   }
@@ -76,26 +102,36 @@ __host__ inline int make_split(const vtm_split_t* s, Split* o) {
 }
 
 // position (in the level's sequence) of src token i  — `a_idx[i]`, merge.py:63 / :375
+template <bool DC = false>
 __host__ __device__ __forceinline__ int src_pos(const Split& s, int i) {
   if (s.mode == 1) return i;
+  if (DC && s.mode == 2) return s.randf ? i : s.src_len + i;
   const int q = i / s.tnum, t = i - q * s.tnum;        // q-th src frame
   const int g = q / (s.stride - 1), w = q - g * (s.stride - 1);
   const int f = g * s.stride + (w < s.randf ? w : w + 1);
   return s.unm_pre + f * s.tnum + t;
 }
 // position of dst token j — `b_idx[j]`, merge.py:64-69 (dst frames then the unm_pre carried tokens) / :376
+template <bool DC = false>
 __host__ __device__ __forceinline__ int dst_pos(const Split& s, int j) {
   if (s.mode == 1) return s.src_len + j;
+  if (DC && s.mode == 2) return s.randf ? s.src_len + j : j;
   const int nf = s.nd_frames * s.tnum;
   if (j >= nf) return j - nf;
   const int q = j / s.tnum, t = j - q * s.tnum;
   return s.unm_pre + (q * s.stride + s.randf) * s.tnum + t;
 }
 // inverse: position -> (is_dst, index within src or dst)
+template <bool DC = false>
 __host__ __device__ __forceinline__ bool pos_to_part(const Split& s, int p, int* idx) {
   if (s.mode == 1) {
     if (p < s.src_len) { *idx = p; return false; }
     *idx = p - s.src_len; return true;
+  }
+  if (DC && s.mode == 2) {   // local rows [0, src_len) are src when randf == 1, global rows [src_len, N) the other half
+    const bool local = p < s.src_len;
+    *idx = local ? p : p - s.src_len;
+    return local != (s.randf != 0);
   }
   if (p < s.unm_pre) { *idx = s.nd_frames * s.tnum + p; return true; }
   const int pp = p - s.unm_pre;

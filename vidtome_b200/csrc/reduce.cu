@@ -118,6 +118,7 @@ extern "C" int vtm_merge_reduce(const void* x_dev, int64_t x_batch_stride, const
   Split sp;
   int rc = make_split(split, &sp);
   if (rc) return rc;
+  if (sp.glob_len_dev) return VTM_E_SPLIT;   // device counts: only the replace-mode row gathers have that path
   if (!x_dev || !y_dev || !ws_dev) return VTM_E_NULL;
   if (sp.Ns > 0 && (!keys_dev || !edge_dev)) return VTM_E_NULL;
   if (B <= 0 || C <= 0 || (C % 8) != 0 || r < 0 || r > sp.Ns || sp.Nd <= 0 || (Bp != 1 && Bp != B)) return VTM_E_SHAPE;

@@ -132,7 +132,8 @@ __device__ __forceinline__ void layer_norm_row(uint4 (&v)[P], int sub, int vecs,
 #ifndef VTM_K0_PREFETCH
 #define VTM_K0_PREFETCH 0
 #endif
-template <int G, int P, bool LN, bool FULL = false>
+// DC: device-count (mode 2) split, src / dst rows at the capacity's row stride (vtm_split_t mode 2)
+template <int G, int P, bool LN, bool FULL = false, bool DC = false>
 __global__ void __launch_bounds__(ROW_THREADS, VTM_K0_PREFETCH ? (LN ? 2 : 3) : (LN ? 3 : 4))
 normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* __restrict__ rowmap,
                        long long map_bs, Split sp, int B, int C, LnParams ln, __half* __restrict__ a_out,
@@ -140,7 +141,7 @@ normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* 
   __shared__ __align__(16) float s_gamma[LN ? LN_MAX_C : 4];
   __shared__ __align__(16) float s_beta[LN ? LN_MAX_C : 4];
   if (LN) stage_ln_params(ln, C, s_gamma, s_beta);
-  resolve_split(sp);
+  resolve_split<DC>(sp);
   constexpr int RPW = 32 / G;                       // rows per warp
   const int lane = threadIdx.x & 31;
   const int sub = lane % G, grp = lane / G;
@@ -149,6 +150,8 @@ normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* 
   const int vecs = C >> 3;
   const long long rows_per_b = static_cast<long long>(sp.Ns) + sp.Nd;
   const long long total = rows_per_b * B;
+  // per-sample row strides of a_out / b_out: the counts, or the capacity of a device-count split
+  const long long lda = DC ? sp.cap : sp.Ns, ldb = DC ? sp.cap : sp.Nd;
   // where row group o0 comes from and goes to
   auto locate = [&](long long o0, const __half*& src, __half*& dst) -> bool {
     const long long o = o0 + grp;
@@ -159,11 +162,11 @@ normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* 
     const int q = static_cast<int>(o - b * rows_per_b);
     int pos;
     if (q < sp.Ns) {
-      pos = src_pos(sp, q);
-      dst = a_out + (static_cast<long long>(b) * sp.Ns + q) * C;
+      pos = src_pos<DC>(sp, q);
+      dst = a_out + (b * lda + q) * C;
     } else {
-      pos = dst_pos(sp, q - sp.Ns);
-      dst = b_out + (static_cast<long long>(b) * sp.Nd + (q - sp.Ns)) * C;
+      pos = dst_pos<DC>(sp, q - sp.Ns);
+      dst = b_out + (b * ldb + (q - sp.Ns)) * C;
     }
     const int row = rowmap ? rowmap[b * map_bs + pos] : pos;
     src = x + b * x_bs + static_cast<long long>(row) * C;
@@ -262,11 +265,12 @@ struct PeerDsts {
   int n;
 };
 
-template <int G, int P, bool ADD, bool LN>
+// DL (device length): rows i >= *len_dev of each sample are written as zeros instead of gathered.
+template <int G, int P, bool ADD, bool LN, bool DL = false>
 __global__ void __launch_bounds__(ROW_THREADS, LN ? 3 : 4)
 gather_rows_kernel(const __half* __restrict__ x, long long x_bs, const int* __restrict__ map, long long map_bs,
                    const __half* __restrict__ resid, int B, int L, int C, LnParams ln, __half* __restrict__ y,
-                   long long y_bs, PeerDsts peers) {
+                   long long y_bs, PeerDsts peers, const int* __restrict__ len_dev = nullptr) {
   __shared__ __align__(16) float s_gamma[LN ? LN_MAX_C : 4];
   __shared__ __align__(16) float s_beta[LN ? LN_MAX_C : 4];
   if (LN) stage_ln_params(ln, C, s_gamma, s_beta);
@@ -277,9 +281,10 @@ gather_rows_kernel(const __half* __restrict__ x, long long x_bs, const int* __re
   const long long n_warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
   const int vecs = C >> 3;
   const long long total = static_cast<long long>(B) * L;
+  const int l_valid = DL ? __ldg(len_dev) : L;
   for (long long o0 = warp_id * RPW; o0 < total; o0 += n_warps * RPW) {
     const long long o = o0 + grp;
-    const bool live = o < total;
+    bool live = o < total;
     const __half* src = x;
     __half* dst = y;
     int b = 0, i = 0;
@@ -287,6 +292,12 @@ gather_rows_kernel(const __half* __restrict__ x, long long x_bs, const int* __re
       b = static_cast<int>(o / L);
       i = static_cast<int>(o - static_cast<long long>(b) * L);
       dst = y + b * y_bs + static_cast<long long>(i) * C;
+    }
+    if (DL && live && i >= l_valid) {
+#pragma unroll
+      for (int k = 0; k < P; ++k)
+        if (sub + G * k < vecs) st_16(dst + (sub + G * k) * 8, make_uint4(0, 0, 0, 0));
+      live = false;
     }
     uint4 v[P], rr[P];
     // residual rows do not depend on the map: get them in flight before the (dependent) map lookup
@@ -383,14 +394,22 @@ extern "C" int vtm_normalize_split_ln(const void* x_dev, int64_t x_batch_stride,
   const int vecs = C / 8;
   LnParams ln{static_cast<const __half*>(ln_weight_dev), static_cast<const __half*>(ln_bias_dev), ln_eps};
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
-#define CALL_K0_(G, P, LN, FULL)                                                                                   \
-  normalize_split_kernel<G, P, LN, FULL>                                                                          \
-      <<<grid_for_rows(normalize_split_kernel<G, P, LN, FULL>, rows, 32 / G, sms), ROW_THREADS, 0, st>>>(         \
+#define CALL_K0_(G, P, LN, FULL, DC)                                                                               \
+  normalize_split_kernel<G, P, LN, FULL, DC>                                                                      \
+      <<<grid_for_rows(normalize_split_kernel<G, P, LN, FULL, DC>, rows, 32 / G, sms), ROW_THREADS, 0, st>>>(     \
           static_cast<const __half*>(x_dev), x_batch_stride, rowmap_dev, rowmap_batch_stride, sp, B, C, ln,       \
           static_cast<__half*>(a_out_dev), static_cast<__half*>(b_out_dev));
+  if (sp.glob_len_dev) {
+    // the global stage's tokens are already normalised by norm1 (KC wrote them): no fused LayerNorm on this path
+    if (ln.w) return VTM_E_UNSUPPORTED;
+#define CALL(G, P) CALL_K0_(G, P, false, false, true)
+    VTM_DISPATCH_GP(vecs, CALL)
+#undef CALL
+    return launch_rc();
+  }
 #define CALL_K0(G, P, LN)                                   \
-  if (vecs == (G) * (P)) { CALL_K0_(G, P, LN, true) }       \
-  else { CALL_K0_(G, P, LN, false) }
+  if (vecs == (G) * (P)) { CALL_K0_(G, P, LN, true, false) }       \
+  else { CALL_K0_(G, P, LN, false, false) }
   if (ln.w) {
 #define CALL(G, P) CALL_K0(G, P, true)
     VTM_DISPATCH_GP_LN(vecs, CALL)
@@ -465,6 +484,30 @@ extern "C" int vtm_gather_rows(const void* x_dev, int64_t x_batch_stride, const 
                                int64_t y_batch_stride, void* stream_) {
   return vtm_gather_rows_ln(x_dev, x_batch_stride, map_dev, map_batch_stride, B, L, C, nullptr, nullptr, 0.f,
                             y_dev, y_batch_stride, stream_);
+}
+
+extern "C" int vtm_gather_rows_dev(const void* x_dev, int64_t x_batch_stride, const int32_t* map_dev,
+                                   int64_t map_batch_stride, int32_t B, int32_t L_cap, int32_t C, const int32_t* len_dev,
+                                   void* y_dev, int64_t y_batch_stride, void* stream_) {
+  using namespace vtm;
+  if (!x_dev || !y_dev || !map_dev || !len_dev) return VTM_E_NULL;
+  if (B <= 0 || L_cap < 0 || C <= 0 || (C % 8) != 0 || C > 32 * 8 * 8) return VTM_E_SHAPE;
+  if (L_cap == 0) return VTM_OK;
+  int sms = 0;
+  int rc = sm_count(&sms);
+  if (rc) return rc;
+  const long long rows = static_cast<long long>(B) * L_cap;
+  const int vecs = C / 8;
+  LnParams ln{nullptr, nullptr, 0.f};
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+#define CALL(G, P)                                                                                                \
+  gather_rows_kernel<G, P, false, false, true>                                                                    \
+      <<<grid_for_rows(gather_rows_kernel<G, P, false, false, true>, rows, 32 / G, sms), ROW_THREADS, 0, st>>>(   \
+          static_cast<const __half*>(x_dev), x_batch_stride, map_dev, map_batch_stride, nullptr, B, L_cap, C, ln, \
+          static_cast<__half*>(y_dev), y_batch_stride, PeerDsts{}, len_dev);
+  VTM_DISPATCH_GP(vecs, CALL)
+#undef CALL
+  return launch_rc();
 }
 
 extern "C" int vtm_unmerge_add(const void* y_dev, int64_t y_batch_stride, const int32_t* map_dev,

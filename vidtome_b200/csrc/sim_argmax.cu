@@ -103,8 +103,10 @@ struct Items {
 };
 
 struct Args {
-  unsigned long long* keys;  // [B', Ns]
+  unsigned long long* keys;  // [B', ld]
   int Ns, Nd, align_batch;
+  int ld;                    // row stride of keys: Ns, or the src capacity with device counts
+  const int* counts;         // device counts {Ns, Nd, ...} (vtm_sim_argmax_dev), NULL = the values above
 };
 
 __device__ __forceinline__ float round_f16(float x) { return __half2float(__float2half_rn(x)); }
@@ -122,7 +124,7 @@ struct RowBest {
     best = -INFINITY;
     idx = 0xFFFFFFFFu;
     if (row < p.Ns) {
-      const size_t o = (p.align_batch ? 0 : static_cast<size_t>(b) * p.Ns) + row;
+      const size_t o = (p.align_batch ? 0 : static_cast<size_t>(b) * p.ld) + row;
       const unsigned long long k = *reinterpret_cast<const volatile unsigned long long*>(p.keys + o);
       uint32_t ord = static_cast<uint32_t>(k >> 32);
       if (k != 0ull && ord > 0x0400u) {          // published and above -inf
@@ -146,7 +148,7 @@ struct RowBest {
     if (row < p.Ns && idx != 0xFFFFFFFFu) {
       const uint32_t hb = static_cast<uint32_t>(__half_as_ushort(__float2half_rn(best)));
       const uint32_t arg = p.align_batch ? static_cast<uint32_t>(b) * static_cast<uint32_t>(p.Nd) + idx : idx;
-      const size_t o = (p.align_batch ? 0 : static_cast<size_t>(b) * p.Ns) + row;
+      const size_t o = (p.align_batch ? 0 : static_cast<size_t>(b) * p.ld) + row;
       atomicMax(p.keys + o, static_cast<unsigned long long>(pack_key(hb, arg)));
     }
   }
@@ -213,8 +215,16 @@ __device__ __forceinline__ void tile_argmax(const float (&d)[128], RowBest (&rb)
 template <bool PAIR>
 __global__ void __launch_bounds__(THREADS, 1)
 sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                  const Items wk, const Layout lay, const Args p) {
+                  const Items wk, const Layout lay, const Args p_in) {
   extern __shared__ uint8_t smem_raw[];
+  // with device counts the grid is planned for capacity: src blocks at or past Ns and dst tiles at or past Nd are
+  // skipped (by the producer and the consumers alike, so the barrier phases stay paired)
+  Args p = p_in;
+  if (p.counts) {
+    p.Ns = __ldg(p.counts);
+    p.Nd = __ldg(p.counts + 1);
+  }
+  const int nt_end = (p.Nd + BN - 1) / BN;
   // 1024-byte alignment: required by the 128-byte swizzle pattern shared by TMA and wgmma descriptors
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;                   // resident src block: k_chunks x A_BYTES
@@ -265,6 +275,8 @@ sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       for (int w = w_first; w < wk.total; w += w_step) {
         int m_tile, b, nt0, nt1;
         wk.decode(w, &m_tile, &b, &nt0, &nt1);
+        if (nt1 > nt_end) nt1 = nt_end;
+        if (nt0 >= nt1 || m_tile * BM >= p.Ns) continue;
         if (PAIR) {
           m_tile = 2 * m_tile + static_cast<int>(rank);
           // the second block of an odd last pair lies past M: load a real block (its rows are never published)
@@ -318,6 +330,8 @@ sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     for (int w = w_first; w < wk.total; w += w_step) {
       int m_tile, b, nt0, nt1;
       wk.decode(w, &m_tile, &b, &nt0, &nt1);
+      if (nt1 > nt_end) nt1 = nt_end;
+      if (nt0 >= nt1 || m_tile * BM >= p.Ns) continue;
       if (PAIR) m_tile = 2 * m_tile + static_cast<int>(rank);   // may lie past M: rows >= Ns are never published
       const int row = m_tile * BM + r0;
       RowBest rb[2];
@@ -450,10 +464,13 @@ int check_args(const void* a, const void* b, int B, int Ns, int Nd, int C, const
 
 namespace vtm {
 namespace {
+// Ns, Nd: the counts, or with counts_dev (device counts) the capacities the buffers and the grid are sized for
 int sim_argmax_impl(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd, int32_t C,
-                    int32_t align_batch, uint64_t* keys_out_dev, void* stream_, bool use_pair) {
+                    int32_t align_batch, uint64_t* keys_out_dev, void* stream_, bool use_pair,
+                    const int32_t* counts_dev = nullptr) {
   int rc = check_args(a_dev, b_dev, B, Ns, Nd, C, keys_out_dev);
   if (rc) return rc;
+  if (counts_dev && use_pair) return VTM_E_SPLIT;   // only the one-CTA build reads device counts
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int Bp = align_batch ? 1 : B;
   rc = cuda_rc(cudaMemsetAsync(keys_out_dev, 0, sizeof(uint64_t) * static_cast<size_t>(Bp) * Ns, stream));
@@ -476,6 +493,7 @@ int sim_argmax_impl(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns,
   ka::Args p;
   p.keys = reinterpret_cast<unsigned long long*>(keys_out_dev);
   p.Ns = Ns; p.Nd = Nd; p.align_batch = align_batch ? 1 : 0;
+  p.ld = Ns; p.counts = counts_dev;
   if (use_pair) return ka::launch<true>(ta, tb, wk, lay, p, sms, stream);
   return ka::launch<false>(ta, tb, wk, lay, p, sms, stream);
 }
@@ -485,6 +503,13 @@ int sim_argmax_impl(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns,
 extern "C" int vtm_sim_argmax(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd,
                               int32_t C, int32_t align_batch, uint64_t* keys_out_dev, void* stream_) {
   return vtm::sim_argmax_impl(a_dev, b_dev, B, Ns, Nd, C, align_batch, keys_out_dev, stream_, false);
+}
+
+extern "C" int vtm_sim_argmax_dev(const void* a_dev, const void* b_dev, int32_t B, int32_t ns_cap, int32_t nd_cap,
+                                  int32_t C, int32_t align_batch, const int32_t* counts_dev, uint64_t* keys_out_dev,
+                                  void* stream_) {
+  if (!counts_dev) return VTM_E_NULL;
+  return vtm::sim_argmax_impl(a_dev, b_dev, B, ns_cap, nd_cap, C, align_batch, keys_out_dev, stream_, false, counts_dev);
 }
 
 extern "C" int vtm_sim_argmax_pair(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd,

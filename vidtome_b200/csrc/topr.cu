@@ -54,16 +54,17 @@ __device__ __forceinline__ int tile_rank(int bucket, bool valid, uint32_t (*s_cn
 template <int PASS>
 __global__ void __launch_bounds__(TILE)
 radix_hist_kernel(const unsigned long long* __restrict__ keys, const uint16_t* __restrict__ k_in, int Ns,
-                  int tiles, uint32_t* __restrict__ hist /* [Bp][256][tiles] */) {
+                  int tiles, uint32_t* __restrict__ hist /* [Bp][256][tiles] */, int ld, const int* __restrict__ ns_dev) {
   __shared__ uint32_t s_cnt[NW][256];
   __shared__ uint32_t s_tot[256];
+  if (ns_dev) Ns = __ldg(ns_dev);
   const int b = blockIdx.y, tile = blockIdx.x;
   const int e = tile * TILE + threadIdx.x;
   const bool valid = e < Ns;
   uint32_t k16 = 0;
   if (valid)
-    k16 = PASS == 0 ? static_cast<uint32_t>(keys[static_cast<size_t>(b) * Ns + e] >> 32) & 0xFFFFu
-                    : k_in[static_cast<size_t>(b) * Ns + e];
+    k16 = PASS == 0 ? static_cast<uint32_t>(keys[static_cast<size_t>(b) * ld + e] >> 32) & 0xFFFFu
+                    : k_in[static_cast<size_t>(b) * ld + e];
   tile_rank(digit_of(k16, PASS), valid, s_cnt, s_tot);
   if (threadIdx.x < 256)
     hist[(static_cast<size_t>(b) * 256 + threadIdx.x) * tiles + tile] = s_tot[threadIdx.x];
@@ -100,9 +101,11 @@ template <int PASS>
 __global__ void __launch_bounds__(TILE)
 radix_scatter_kernel(const unsigned long long* __restrict__ keys, const uint16_t* __restrict__ k_in,
                      const int* __restrict__ id_in, int Ns, int tiles, const uint32_t* __restrict__ base,
-                     uint16_t* __restrict__ k_out, int* __restrict__ id_out, int* __restrict__ rank_out) {
+                     uint16_t* __restrict__ k_out, int* __restrict__ id_out, int* __restrict__ rank_out, int ld,
+                     const int* __restrict__ ns_dev) {
   __shared__ uint32_t s_cnt[NW][256];
   __shared__ uint32_t s_tot[256];
+  if (ns_dev) Ns = __ldg(ns_dev);
   const int b = blockIdx.y, tile = blockIdx.x;
   const int e = tile * TILE + threadIdx.x;
   const bool valid = e < Ns;
@@ -110,23 +113,23 @@ radix_scatter_kernel(const unsigned long long* __restrict__ keys, const uint16_t
   int id = e;
   if (valid) {
     if (PASS == 0) {
-      k16 = static_cast<uint32_t>(keys[static_cast<size_t>(b) * Ns + e] >> 32) & 0xFFFFu;
+      k16 = static_cast<uint32_t>(keys[static_cast<size_t>(b) * ld + e] >> 32) & 0xFFFFu;
     } else {
-      k16 = k_in[static_cast<size_t>(b) * Ns + e];
-      id = id_in[static_cast<size_t>(b) * Ns + e];
+      k16 = k_in[static_cast<size_t>(b) * ld + e];
+      id = id_in[static_cast<size_t>(b) * ld + e];
     }
   }
   const int bucket = digit_of(k16, PASS);
   const int r = tile_rank(bucket, valid, s_cnt, s_tot);
   if (valid) {
     const uint32_t pos = base[(static_cast<size_t>(b) * 256 + bucket) * tiles + tile] + r;
-    const size_t o = static_cast<size_t>(b) * Ns + pos;
+    const size_t o = static_cast<size_t>(b) * ld + pos;
     if (PASS == 0) {
       k_out[o] = static_cast<uint16_t>(k16);
       id_out[o] = id;
     } else {
       id_out[o] = id;                                         // edge[pos] = src row
-      rank_out[static_cast<size_t>(b) * Ns + id] = static_cast<int>(pos);  // rank[src row] = pos
+      rank_out[static_cast<size_t>(b) * ld + id] = static_cast<int>(pos);  // rank[src row] = pos
     }
   }
 }
@@ -136,29 +139,33 @@ __global__ void __launch_bounds__(256)
 compose_maps_kernel(Split sp, int r, int Bp, const unsigned long long* __restrict__ keys,
                     const int* __restrict__ edge, const int* __restrict__ rank, const int* __restrict__ mu_in,
                     const int* __restrict__ pi_in, int pi_offset, int N0, int* __restrict__ mu_out,
-                    int* __restrict__ pi_out) {
-  resolve_split(sp);
+                    int* __restrict__ pi_out, const int* __restrict__ counts = nullptr) {
+  // device counts (mode 2): keys / edge / rank have row stride cap, mu_out row stride src_len + gcap
+  const int ldk = sp.cap ? sp.cap : sp.Ns;
+  const int ldmu = sp.cap ? sp.src_len + sp.gcap : (sp.Ns - r) + sp.Nd;
+  resolve_split<true>(sp);
+  if (counts) r = __ldg(counts + 2);
   const int b = blockIdx.y;
   const int Ns = sp.Ns, Nd = sp.Nd;
   const int unm = Ns - r;
   const int Lnext = unm + Nd;
-  const unsigned long long* kb = keys + static_cast<size_t>(b) * Ns;
-  const int* eb = edge + static_cast<size_t>(b) * Ns;
-  const int* rb = rank + static_cast<size_t>(b) * Ns;
+  const unsigned long long* kb = keys + static_cast<size_t>(b) * ldk;
+  const int* eb = edge + static_cast<size_t>(b) * ldk;
+  const int* rb = rank + static_cast<size_t>(b) * ldk;
   const int* mub = mu_in ? mu_in + static_cast<size_t>(b) * sp.N : nullptr;
   const int* pib = pi_in ? pi_in + static_cast<size_t>(b) * N0 : nullptr;
   const int n_iter = Lnext > N0 ? Lnext : N0;
   for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_iter; t += gridDim.x * blockDim.x) {
     if (t < Lnext) {
       // merged sequence = [unmerged src in edge order | dst]  (merge.py:124,133)
-      const int pos = t < unm ? src_pos(sp, eb[r + t]) : dst_pos(sp, t - unm);
-      mu_out[static_cast<size_t>(b) * Lnext + t] = mub ? mub[pos] : pos;
+      const int pos = t < unm ? src_pos<true>(sp, eb[r + t]) : dst_pos<true>(sp, t - unm);
+      mu_out[static_cast<size_t>(b) * ldmu + t] = mub ? mub[pos] : pos;
     }
-    if (t < N0) {
+    if (t < N0 && (pib || t < sp.N)) {             // without pi_in, positions past the sequence have no image
       const int p = (pib ? pib[t] : t) + pi_offset;  // position in this level's sequence
       int idx;
       int np;
-      if (pos_to_part(sp, p, &idx)) {
+      if (pos_to_part<true>(sp, p, &idx)) {
         np = unm + idx;                                // dst j -> merged[unm + j]      (merge.py:146)
       } else {
         const int k = rb[idx];
@@ -276,7 +283,7 @@ __device__ __forceinline__ uint32_t bucket_base(const uint32_t* __restrict__ h /
 __global__ void __launch_bounds__(TILE)
 radix_sort_fused_kernel(const unsigned long long* __restrict__ keys, int Ns, int tiles, uint32_t* hist0,
                         uint32_t* hist1, uint16_t* k_tmp, int* id_tmp, int* __restrict__ edge,
-                        int* __restrict__ rank_out, unsigned int* barrier_ctr) {
+                        int* __restrict__ rank_out, unsigned int* barrier_ctr, int ld, const int* __restrict__ ns_dev) {
   __shared__ uint32_t s_cnt[NW][256];
   __shared__ uint32_t s_tot[256];
   __shared__ uint32_t s_base[256];
@@ -284,7 +291,8 @@ radix_sort_fused_kernel(const unsigned long long* __restrict__ keys, int Ns, int
   __shared__ uint32_t s_part[8][256];
   const int b = blockIdx.y, tile = blockIdx.x;
   const unsigned int nblk = gridDim.x * gridDim.y;
-  const size_t row0 = static_cast<size_t>(b) * Ns;
+  if (ns_dev) Ns = __ldg(ns_dev);
+  const size_t row0 = static_cast<size_t>(b) * ld;
   const int e = tile * TILE + threadIdx.x;
   const bool valid = e < Ns;
   // ---- pass 0 (low byte)
@@ -357,9 +365,11 @@ extern "C" size_t vtm_topr_workspace_bytes(int32_t Bp, int32_t Ns) {
   return vtm::sort_ws_layout(Bp, Ns, nullptr, nullptr);
 }
 
-extern "C" int vtm_topr_sort(const uint64_t* keys_dev, int32_t Bp, int32_t Ns, int32_t* edge_dev,
-                             int32_t* rank_dev, void* ws_dev, size_t ws_bytes, void* stream_) {
-  using namespace vtm;
+namespace vtm {
+namespace {
+// Ns: the count (ns_dev == NULL) or the capacity and row stride (ns_dev: the count on the device, <= Ns)
+int topr_sort_impl(const uint64_t* keys_dev, int32_t Bp, int32_t Ns, const int32_t* ns_dev, int32_t* edge_dev,
+                   int32_t* rank_dev, void* ws_dev, size_t ws_bytes, void* stream_) {
   if (!keys_dev || !edge_dev || !rank_dev || !ws_dev) return VTM_E_NULL;
   if (Bp <= 0 || Ns <= 0) return VTM_E_SHAPE;
   SortWs ws;
@@ -393,19 +403,32 @@ extern "C" int vtm_topr_sort(const uint64_t* keys_dev, int32_t Bp, int32_t Ns, i
       // heavier launch path; measured r02.
       (void)ns; (void)tl;
       radix_sort_fused_kernel<<<grid, TILE, 0, st>>>(keys, Ns, tiles, ws.hist, ws.hist1, ws.k_tmp, ws.id_tmp, edge_dev,
-                                                    rank_dev, ws.barrier);
+                                                    rank_dev, ws.barrier, Ns, ns_dev);
       return launch_rc();
     }
   }
-  radix_hist_kernel<0><<<grid, TILE, 0, st>>>(keys, nullptr, Ns, tiles, ws.hist);
+  radix_hist_kernel<0><<<grid, TILE, 0, st>>>(keys, nullptr, Ns, tiles, ws.hist, Ns, ns_dev);
   radix_scan_kernel<<<Bp, 1024, 0, st>>>(ws.hist, tiles);
   radix_scatter_kernel<0><<<grid, TILE, 0, st>>>(keys, nullptr, nullptr, Ns, tiles, ws.hist, ws.k_tmp,
-                                                 ws.id_tmp, nullptr);
-  radix_hist_kernel<1><<<grid, TILE, 0, st>>>(nullptr, ws.k_tmp, Ns, tiles, ws.hist);
+                                                 ws.id_tmp, nullptr, Ns, ns_dev);
+  radix_hist_kernel<1><<<grid, TILE, 0, st>>>(nullptr, ws.k_tmp, Ns, tiles, ws.hist, Ns, ns_dev);
   radix_scan_kernel<<<Bp, 1024, 0, st>>>(ws.hist, tiles);
   radix_scatter_kernel<1><<<grid, TILE, 0, st>>>(nullptr, ws.k_tmp, ws.id_tmp, Ns, tiles, ws.hist, nullptr,
-                                                 edge_dev, rank_dev);
+                                                 edge_dev, rank_dev, Ns, ns_dev);
   return launch_rc();
+}
+}  // namespace
+}  // namespace vtm
+
+extern "C" int vtm_topr_sort(const uint64_t* keys_dev, int32_t Bp, int32_t Ns, int32_t* edge_dev,
+                             int32_t* rank_dev, void* ws_dev, size_t ws_bytes, void* stream_) {
+  return vtm::topr_sort_impl(keys_dev, Bp, Ns, nullptr, edge_dev, rank_dev, ws_dev, ws_bytes, stream_);
+}
+
+extern "C" int vtm_topr_sort_dev(const uint64_t* keys_dev, int32_t Bp, int32_t ns_cap, const int32_t* counts_dev,
+                                 int32_t* edge_dev, int32_t* rank_dev, void* ws_dev, size_t ws_bytes, void* stream_) {
+  if (!counts_dev) return VTM_E_NULL;
+  return vtm::topr_sort_impl(keys_dev, Bp, ns_cap, counts_dev, edge_dev, rank_dev, ws_dev, ws_bytes, stream_);
 }
 
 extern "C" int vtm_compose_maps(const vtm_split_t* split, int32_t r, int32_t Ns, int32_t Nd, int32_t Bp,
@@ -416,6 +439,7 @@ extern "C" int vtm_compose_maps(const vtm_split_t* split, int32_t r, int32_t Ns,
   Split sp;
   int rc = make_split(split, &sp);
   if (rc) return rc;
+  if (sp.glob_len_dev) return VTM_E_SPLIT;   // device counts: vtm_compose_maps_dev
   if (!mu_out_dev || !pi_out_dev) return VTM_E_NULL;
   if (Ns > 0 && (!keys_dev || !edge_dev || !rank_dev)) return VTM_E_NULL;   // Ns == 0: nothing was matched
   if (sp.Ns != Ns || sp.Nd != Nd || r < 0 || r > Ns || Bp <= 0 || N0 <= 0 || Nd <= 0) return VTM_E_SHAPE;
@@ -426,6 +450,48 @@ extern "C" int vtm_compose_maps(const vtm_split_t* split, int32_t r, int32_t Ns,
   compose_maps_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream_)>>>(
       sp, r, Bp, reinterpret_cast<const unsigned long long*>(keys_dev), edge_dev, rank_dev, mu_in_dev,
       pi_in_dev, pi_offset, N0, mu_out_dev, pi_out_dev);
+  return launch_rc();
+}
+
+extern "C" int vtm_compose_maps_dev(const vtm_split_t* split, const int32_t* counts_dev, int32_t Bp,
+                                    const uint64_t* keys_dev, const int32_t* edge_dev, const int32_t* rank_dev,
+                                    const int32_t* pi_in_dev, int32_t N0, int32_t* mu_out_dev, int32_t* pi_out_dev,
+                                    void* stream_) {
+  using namespace vtm;
+  Split sp;
+  int rc = make_split(split, &sp);
+  if (rc) return rc;
+  if (!sp.glob_len_dev) return VTM_E_SPLIT;
+  if (!counts_dev || !keys_dev || !edge_dev || !rank_dev || !mu_out_dev || !pi_out_dev) return VTM_E_NULL;
+  if (Bp <= 0 || N0 <= 0 || (!pi_in_dev && N0 > sp.N)) return VTM_E_SHAPE;
+  const int n_iter = sp.N > N0 ? sp.N : N0;     // sp.N = src_len + gcap bounds the merged length
+  dim3 grid((n_iter + 255) / 256, Bp);
+  compose_maps_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream_)>>>(
+      sp, 0, Bp, reinterpret_cast<const unsigned long long*>(keys_dev), edge_dev, rank_dev, nullptr, pi_in_dev, 0, N0,
+      mu_out_dev, pi_out_dev, counts_dev);
+  return launch_rc();
+}
+
+__global__ void split_counts_dev_kernel(vtm::Split sp, double ratio, int* __restrict__ counts) {
+  vtm::resolve_split<true>(sp);
+  // vtm_merge_count on the device: Python's int(Ns * ratio) in double, then min(Ns, .)
+  long long r = static_cast<long long>(trunc(static_cast<double>(sp.Ns) * ratio));
+  if (r > sp.Ns) r = sp.Ns;
+  counts[0] = sp.Ns;
+  counts[1] = sp.Nd;
+  counts[2] = static_cast<int>(r);
+  counts[3] = sp.Ns - static_cast<int>(r) + sp.Nd;
+}
+
+extern "C" int vtm_split_counts_dev(const vtm_split_t* split, double ratio, int32_t* counts_dev, void* stream_) {
+  using namespace vtm;
+  Split sp;
+  int rc = make_split(split, &sp);
+  if (rc) return rc;
+  if (!sp.glob_len_dev) return VTM_E_SPLIT;
+  if (!counts_dev) return VTM_E_NULL;
+  if (!(ratio >= 0.0)) return VTM_E_SHAPE;
+  split_counts_dev_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream_)>>>(sp, ratio, counts_dev);
   return launch_rc();
 }
 

@@ -37,7 +37,8 @@ class ChunkedDenoiser:
     def __init__(self, unet: torch.nn.Module, n_timesteps: int = 50, chunk_size: int = 16,
                  guidance_scale: float = 7.5, merge_global: bool = False, chunk_ord: str = "seq",
                  perm_div: float = 3.0, randomize_chunks: bool = False, cond: Optional[torch.Tensor] = None,
-                 cuda_graph: bool = False, graph_warmup: int = 2, shard: bool = False, capture_global: bool = False):
+                 cuda_graph: bool = False, graph_warmup: int = 2, shard: bool = False, capture_global: bool = False,
+                 chunk_graphs: bool = False):
         """`cuda_graph=True`: after `graph_warmup` eager steps, the noise prediction of a whole step (every chunk:
         CFG batch, UNet forward with the merge path, guidance combine) is captured once into a CUDA graph and
         replayed; per step the host then issues one graph launch plus the DDIM update instead of ~250 kernel
@@ -51,7 +52,18 @@ class ChunkedDenoiser:
         inside the graph, with the coin of every block drawn on the device (patch.DEVICE_COIN).  Each step still draws
         the chunk order on the host with get_chunks, exactly as eager stepping does, and applies it as data: one
         index_select of the latents into the slots, one of the noise back.  Needs every chunk to be equally long
-        (frame count divisible by chunk_size), patch.GLOBAL_EXCHANGE == "recurrence", and no sharding."""
+        (frame count divisible by chunk_size), patch.GLOBAL_EXCHANGE == "recurrence", and no sharding.
+
+        `chunk_graphs=True` (with `cuda_graph=True`) captures one graph per chunk instead of one per step, keyed by
+        (chunk length, first chunk of the step?), lazily on first use: at most 2 * chunk_size graphs.  Each step calls
+        get_chunks once on the host, as eager stepping does, and replays the graph of every chunk in visiting order on
+        its contiguous frame range.  So the reference's own chunking runs from graphs: `randomize_chunks=True`, any frame
+        count, `merge_global` true or false.  With `merge_global=True` every block keeps its global tokens in a
+        patch.GlobalTokenStore (installed before the warm-up steps, emptied where eager stepping calls
+        `update_patch(global_tokens=None)`), whose global stage keeps the counts that depend on the coin on the device.
+        Needs chunk lengths whose local counts do not depend on the frame draw (every length up to chunk_size when
+        chunk_size <= target_stride; see draw_dependent_lengths), patch.GLOBAL_EXCHANGE == "recurrence", the library's
+        self-attention (KD) in every merged block, and no sharding."""
         self.unet = unet
         # shard=True: this process is one rank of a torch.distributed job and takes chunks i % world == rank of every
         # step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
@@ -62,12 +74,23 @@ class ChunkedDenoiser:
         self._graph = None          # (CUDAGraph, static x, static timestep, static noise, shape[, slot index state])
         self._eager_steps = 0
         self.capture_global = bool(capture_global)
+        self.chunk_graphs = bool(chunk_graphs)
         if self.capture_global and not (self.cuda_graph and merge_global):
             raise ValueError("capture_global=True needs cuda_graph=True and merge_global=True")
-        if self.cuda_graph and ((merge_global and not self.capture_global) or randomize_chunks):
+        if self.chunk_graphs and (not self.cuda_graph or self.capture_global):
+            raise ValueError("chunk_graphs=True needs cuda_graph=True and capture_global=False")
+        if self.chunk_graphs and merge_global and self.graph_warmup < 1:
+            raise ValueError("chunk_graphs=True with merge_global=True needs graph_warmup >= 1: the blocks' global token "
+                             "stores are allocated by an eager step, outside the graphs' memory pools")
+        if self.chunk_graphs and self.shard:
+            raise ValueError("chunk_graphs=True does not capture the cross-rank chunk sharding of shard=True")
+        if self.cuda_graph and not self.chunk_graphs and ((merge_global and not self.capture_global) or randomize_chunks):
             raise ValueError("cuda_graph=True needs merge_global=False and randomize_chunks=False (static work)")
         if self.capture_global and self.shard:
             raise ValueError("capture_global=True does not capture the cross-rank exchange of shard=True")
+        self._chunk_graphs = {}     # (chunk length, first in step, frame shape) -> (CUDAGraph, static x, static noise)
+        self._chunk_t = None        # the UNet's timestep input shared by the chunk graphs
+        self._stores = []           # patch.GlobalTokenStore of every block (chunk_graphs with merge_global)
         self.chunk_size = chunk_size
         self.guidance_scale = guidance_scale
         self.merge_global = merge_global
@@ -232,11 +255,109 @@ class ChunkedDenoiser:
         graph.replay()
         return torch.index_select(gn, 0, idx_dev[1])                # slots -> frames
 
+    @staticmethod
+    def draw_dependent_lengths(chunk_size: int, target_stride: int) -> List[int]:
+        """Chunk lengths in 1..chunk_size whose local token counts depend on the frame draw: some local level has a
+        frame count F with F % min(target_stride, F) != 0 (merge.py:55-57), so its number of dst frames, and every
+        count after it, follows the draw.  A level with F % stride == 0 leaves F / stride frames for the next."""
+        out = []
+        for n in range(1, chunk_size + 1):
+            f = n
+            while f > 1:
+                stride = min(target_stride, f)
+                if f % stride:
+                    out.append(n)
+                    break
+                f //= stride
+        return out
+
+    def possible_lengths(self, flen: int) -> List[int]:
+        """Every chunk length get_chunks can produce for `flen` frames, over all draws."""
+        firsts = range(1, self.chunk_size + 1) if self.randomize_chunks else (self.chunk_size,)
+        lens = set()
+        for f in firsts:
+            first = min(f, flen)
+            lens.add(first)
+            rest = flen - first
+            if rest >= self.chunk_size:
+                lens.add(self.chunk_size)
+            if rest % self.chunk_size:
+                lens.add(rest % self.chunk_size)
+        return sorted(lens)
+
+    def _check_chunk_lengths(self, flen: int):
+        args = self.unet._tome_info["args"] if hasattr(self.unet, "_tome_info") else None
+        if patch.GLOBAL_EXCHANGE != "recurrence":
+            raise RuntimeError(f"chunk_graphs=True needs patch.GLOBAL_EXCHANGE='recurrence' (got "
+                               f"{patch.GLOBAL_EXCHANGE!r}): the cross-rank exchange is not captured")
+        if args is None or args["local_merge_ratio"] <= 0:
+            return
+        bad = sorted(set(self.possible_lengths(flen)) & set(self.draw_dependent_lengths(self.chunk_size,
+                                                                                      args["target_stride"])))
+        if bad:
+            raise RuntimeError(f"chunk_graphs=True: chunks of {bad} frames (possible with {flen} frames and chunk_size "
+                               f"{self.chunk_size}) have local token counts that depend on the frame draw (target_stride "
+                               f"{args['target_stride']}); they cannot be captured")
+
+    def _install_stores(self):
+        self._stores = []
+        for m in self.unet.modules():
+            if type(m).__name__ == "ToMeBlock":
+                m.global_tokens = patch.GlobalTokenStore(self.chunk_size)
+                self._stores.append(m.global_tokens)
+
+    def _reset_global(self):
+        if self._stores:
+            for st in self._stores:                                         # generate.py:233-236 on the stores
+                st.reset()
+        else:
+            patch.update_patch(self.unet, global_tokens=None)               # generate.py:233-236
+
+    def _capture_chunk(self, key, x: torch.Tensor):
+        """Capture the noise prediction of one chunk shaped like `x`; `key[1]` says whether it is the first chunk of a
+        step, i.e. whether the blocks' stores are empty when it runs."""
+        gx = x.clone()
+        graph = torch.cuda.CUDAGraph()
+        for g in self._block_generators():
+            graph.register_generator_state(g)
+        for st in self._stores:
+            st.filled = not key[1]
+        torch.cuda.synchronize(x.device)
+        with torch.cuda.graph(graph):
+            gn = self.pred_noise(gx, self._chunk_t)
+        self._chunk_graphs[key] = (graph, gx, gn)
+        return self._chunk_graphs[key]
+
+    def _chunk_graph_noises(self, x: torch.Tensor, t: int) -> torch.Tensor:
+        flen = len(x)
+        chunks = self.get_chunks(flen)                                      # the same host draws as eager stepping
+        if not self._chunk_graphs:
+            self._check_chunk_lengths(flen)                                 # before anything is captured
+        if self._chunk_t is None:
+            self._chunk_t = torch.tensor(int(t), device=x.device, dtype=torch.long)
+        self._chunk_t.fill_(int(t))
+        noises = torch.empty_like(x)
+        for k, chunk in enumerate(chunks):
+            lo, hi = int(chunk[0]), int(chunk[-1]) + 1
+            key = (hi - lo, self.merge_global and k == 0, tuple(x.shape[1:]))
+            entry = self._chunk_graphs.get(key)
+            if entry is None:
+                entry = self._capture_chunk(key, x[lo:hi])
+            graph, gx, gn = entry
+            gx.copy_(x[lo:hi])
+            graph.replay()
+            noises[lo:hi].copy_(gn)
+        return noises
+
     # one iteration of generate.py:211-224
     @torch.no_grad()
     def step(self, x: torch.Tensor, i: int) -> torch.Tensor:
         t = self.timesteps[i]
-        if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.capture_global:
+        if self.chunk_graphs and self.merge_global and x.is_cuda and not self._stores:
+            self._install_stores()
+        if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.chunk_graphs:
+            noises = self._chunk_graph_noises(x, t)
+        elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.capture_global:
             noises = self._slot_noises(x, t)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup:
             if self._graph is None or self._graph[4] != tuple(x.shape):
@@ -251,7 +372,7 @@ class ChunkedDenoiser:
             noises = self._all_noises(x, t)
         x = self.pred_next_x(x, noises, i)
         if self.merge_global:
-            patch.update_patch(self.unet, global_tokens=None)                # generate.py:233-236
+            self._reset_global()
         return x
 
     @torch.no_grad()

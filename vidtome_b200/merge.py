@@ -42,6 +42,8 @@ class LevelMatch:
     keys: torch.Tensor   # [Bp, Ns] packed (ordered fp16 max, ~arg) — KA output
     edge: torch.Tensor   # [Bp, Ns] int32 stable descending order of the row maxima
     rank: torch.Tensor   # [Bp, Ns] int32 inverse of edge
+    # device counts [Ns, Nd, r, M] of a mode-2 split (match_level_dev); Ns / Nd above are then capacities and r is None
+    counts: Optional[torch.Tensor] = None
 
     @property
     def unm_num(self) -> int:
@@ -84,6 +86,19 @@ def match_level(table: torch.Tensor, rowmap: Optional[torch.Tensor], split: VtmS
     keys = ops.sim_argmax(a, b, align_batch)                    # merge.py:87,93-97,112
     edge, rank = ops.topr_sort(keys)                            # merge.py:98,113
     return LevelMatch(split=split, B=B, Bp=keys.shape[0], Ns=Ns, Nd=Nd, r=r, keys=keys, edge=edge, rank=rank)
+
+
+def match_level_dev(tokens: torch.Tensor, split: VtmSplit, ratio: float, align_batch: bool) -> LevelMatch:
+    """K0 + KA + KB1 for a mode-2 split (VtmSplit.prefix_coin_dev): the counts are derived on the device first and every
+    kernel reads them from there, so nothing depends on a value read back to the host."""
+    B = tokens.shape[0]
+    Ns, Nd = ops.split_counts(split)                            # capacities
+    counts = ops.split_counts_dev(split, ratio)
+    a, b = ops.normalize_split(tokens, None, split)
+    keys = ops.sim_argmax(a, b, align_batch, counts=counts)
+    edge, rank = ops.topr_sort(keys, counts=counts)
+    return LevelMatch(split=split, B=B, Bp=keys.shape[0], Ns=Ns, Nd=Nd, r=None, keys=keys, edge=edge, rank=rank,
+                      counts=counts)
 
 
 def _closures(m: LevelMatch, N: int, unmerge_slice: Optional[Tuple[int, int]], merge_mode: str):

@@ -79,6 +79,17 @@ def merge_count(num_src: int, ratio: float) -> int:
     return int(_lib.load().vtm_merge_count(num_src, float(ratio)))
 
 
+def split_counts_dev(split: VtmSplit, ratio: float) -> torch.Tensor:
+    """Device counts of a mode-2 split (VtmSplit.prefix_coin_dev): an int32 CUDA tensor [Ns, Nd, r, M] written by one
+    kernel; nothing is read back to the host."""
+    dev = split._keepalive[0].device
+    counts = torch.empty(4, dtype=torch.int32, device=dev)
+    check(_lib.load().vtm_split_counts_dev(C.byref(split), float(ratio), counts.data_ptr(), _stream()),
+          "vtm_split_counts_dev")
+    STATS.launches += 1
+    return counts
+
+
 def _ln_args(ln):
     """ln = None or (weight [C] fp16, bias [C] fp16 | None, eps)."""
     if ln is None:
@@ -114,14 +125,25 @@ def normalize_split(x: torch.Tensor, rowmap: Optional[torch.Tensor], split: VtmS
 KA_VARIANT = "cta"     # "cta" (default) | "pair" (2-CTA cluster build, A/B measurements and tests)
 
 
-def sim_argmax(a: torch.Tensor, b: torch.Tensor, align_batch: bool, simt: bool = False) -> torch.Tensor:
-    """KA.  Returns the packed keys [B'|Ns] as an int64 tensor (bit pattern of the uint64 keys)."""
+def sim_argmax(a: torch.Tensor, b: torch.Tensor, align_batch: bool, simt: bool = False,
+               counts: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """KA.  Returns the packed keys [B'|Ns] as an int64 tensor (bit pattern of the uint64 keys).  With `counts` (the
+    device counts of a mode-2 split) a and b are sized for capacity and Ns / Nd are read on the device."""
     _require(a, torch.float16, "a")
     _require(b, torch.float16, "b")
     B, Ns, Cc = a.shape
     Nd = b.shape[1]
     keys = torch.empty((1 if align_batch else B, Ns), dtype=torch.int64, device=a.device)
     lib = _lib.load()
+    if counts is not None:
+        _require(counts, torch.int32, "counts")
+        if simt or KA_VARIANT != "cta":
+            check(-3, "KA with device counts (only the default one-CTA build reads them)")
+        with _Timed("KA", 2.0 * B * Ns * Nd * Cc, 2.0 * B * (Ns + Nd) * Cc + 8.0 * keys.shape[0] * Ns):
+            check(lib.vtm_sim_argmax_dev(a.data_ptr(), b.data_ptr(), B, Ns, Nd, Cc, int(bool(align_batch)),
+                                         counts.data_ptr(), keys.data_ptr(), _stream()), "vtm_sim_argmax_dev")
+        STATS.launches += 1
+        return keys
     fn = lib.vtm_sim_argmax_simt if simt else (lib.vtm_sim_argmax_pair if KA_VARIANT == "pair" else lib.vtm_sim_argmax)
     with _Timed("KA", 2.0 * B * Ns * Nd * Cc, 2.0 * B * (Ns + Nd) * Cc + 8.0 * keys.shape[0] * Ns):
         check(fn(a.data_ptr(), b.data_ptr(), B, Ns, Nd, Cc, int(bool(align_batch)), keys.data_ptr(), _stream()),
@@ -130,8 +152,9 @@ def sim_argmax(a: torch.Tensor, b: torch.Tensor, align_batch: bool, simt: bool =
     return keys
 
 
-def topr_sort(keys: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-    """KB1.  keys [Bp, Ns] -> (edge [Bp, Ns] int32, rank [Bp, Ns] int32)."""
+def topr_sort(keys: torch.Tensor, counts: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """KB1.  keys [Bp, Ns] -> (edge [Bp, Ns] int32, rank [Bp, Ns] int32).  With `counts` (device counts), Ns is the
+    capacity and only the first counts[0] entries of each row are sorted."""
     _require(keys, torch.int64, "keys")
     Bp, Ns = keys.shape
     lib = _lib.load()
@@ -140,8 +163,13 @@ def topr_sort(keys: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     edge = torch.empty((Bp, Ns), dtype=torch.int32, device=keys.device)
     rank = torch.empty((Bp, Ns), dtype=torch.int32, device=keys.device)
     with _Timed("KB1", 0.0, 24.0 * Bp * Ns):
-        check(lib.vtm_topr_sort(keys.data_ptr(), Bp, Ns, edge.data_ptr(), rank.data_ptr(), ws.data_ptr(),
-                                ws_bytes, _stream()), "vtm_topr_sort")
+        if counts is not None:
+            _require(counts, torch.int32, "counts")
+            check(lib.vtm_topr_sort_dev(keys.data_ptr(), Bp, Ns, counts.data_ptr(), edge.data_ptr(), rank.data_ptr(),
+                                        ws.data_ptr(), ws_bytes, _stream()), "vtm_topr_sort_dev")
+        else:
+            check(lib.vtm_topr_sort(keys.data_ptr(), Bp, Ns, edge.data_ptr(), rank.data_ptr(), ws.data_ptr(),
+                                    ws_bytes, _stream()), "vtm_topr_sort")
     # one cooperative launch when all (tiles x Bp) CTAs are co-resident (2 per SM), else 6 small launches
     STATS.launches += 1 if ((Ns + 1023) // 1024) * Bp <= 2 * torch.cuda.get_device_properties(keys.device).multi_processor_count else 6
     return edge, rank
@@ -162,6 +190,23 @@ def compose_maps(split: VtmSplit, r: int, keys: torch.Tensor, edge: torch.Tensor
     kp, ep, rp = (None, None, None) if Ns == 0 else (keys.data_ptr(), edge.data_ptr(), rank.data_ptr())
     check(_lib.load().vtm_compose_maps(C.byref(split), r, Ns, nd, Bp, kp, ep, rp, _ptr(mu_in), _ptr(pi_in), pi_offset, N0,
                                        mu_out.data_ptr(), pi_out.data_ptr(), _stream()), "vtm_compose_maps")
+    STATS.launches += 1
+    return mu_out, pi_out
+
+
+def compose_maps_dev(split: VtmSplit, counts: torch.Tensor, keys: torch.Tensor, edge: torch.Tensor,
+                     rank: torch.Tensor, pi_in: Optional[torch.Tensor], N0: int):
+    """KB2 with device counts (mode-2 split).  Returns (mu_out [Bp, split.N]: first M entries meaningful, pi_out
+    [Bp, N0]: without pi_in only the first L + Lg entries are)."""
+    _require(counts, torch.int32, "counts")
+    Bp = keys.shape[0]
+    mu_out = torch.empty((Bp, split.N), dtype=torch.int32, device=keys.device)
+    pi_out = torch.empty((Bp, N0), dtype=torch.int32, device=keys.device)
+    if pi_in is not None:
+        _require(pi_in, torch.int32, "pi_in")
+    check(_lib.load().vtm_compose_maps_dev(C.byref(split), counts.data_ptr(), Bp, keys.data_ptr(), edge.data_ptr(),
+                                           rank.data_ptr(), _ptr(pi_in), N0, mu_out.data_ptr(), pi_out.data_ptr(),
+                                           _stream()), "vtm_compose_maps_dev")
     STATS.launches += 1
     return mu_out, pi_out
 
@@ -202,6 +247,24 @@ def gather_rows(x: torch.Tensor, row_map: Optional[torch.Tensor], L: Optional[in
     with _Timed("KC", 0.0, 4.0 * B * L * Cc + 4.0 * B * L):       # read L rows, write L rows, + map
         check(_lib.load().vtm_gather_rows_ln(x.data_ptr(), x.stride(0), _ptr(row_map), map_bs, B, L, Cc, lw, lb, eps,
                                              out.data_ptr(), out.stride(0), _stream()), "vtm_gather_rows_ln")
+    STATS.launches += 1
+    return out
+
+
+def gather_rows_dev(x: torch.Tensor, row_map: torch.Tensor, length: torch.Tensor) -> torch.Tensor:
+    """KC with a device row count: y[b, i] = x[b, map[b, i]] for i < *length, zeros up to the map's width (the
+    capacity).  x [B, N, C]; map [B'|1, L_cap] int32; length a 1-element int32 CUDA tensor."""
+    _require(x, torch.float16, "x")
+    _require(row_map, torch.int32, "map")
+    _require(length, torch.int32, "length")
+    B, _, Cc = x.shape
+    L = row_map.shape[1]
+    map_bs = 0 if row_map.shape[0] == 1 else L
+    out = torch.empty((B, L, Cc), dtype=torch.float16, device=x.device)
+    with _Timed("KC", 0.0, 4.0 * B * L * Cc + 4.0 * B * L):
+        check(_lib.load().vtm_gather_rows_dev(x.data_ptr(), x.stride(0), row_map.data_ptr(), map_bs, B, L, Cc,
+                                              length.data_ptr(), out.data_ptr(), out.stride(0), _stream()),
+              "vtm_gather_rows_dev")
     STATS.launches += 1
     return out
 
@@ -345,8 +408,10 @@ def layer_norm(x: torch.Tensor, ln) -> torch.Tensor:
 
 
 def attention(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, b_o: Optional[torch.Tensor], heads: int,
-              scale: float, shared_qk: bool = False) -> torch.Tensor:
-    """KD.  x [B, L, C] fp16 -> [B, L, C].  shared_qk: PnP injection — the attention map of sample 0 for every sample."""
+              scale: float, shared_qk: bool = False, seq_len: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """KD.  x [B, L, C] fp16 -> [B, L, C].  shared_qk: PnP injection — the attention map of sample 0 for every sample.
+    seq_len: a 1-element int32 CUDA tensor; the sequence is then the first seq_len rows of x (rows past it must be
+    finite) and only those rows of the result are defined."""
     _require(x, torch.float16, "x")
     _require(w_qkv, torch.float16, "w_qkv")
     _require(w_o, torch.float16, "w_o")
@@ -355,6 +420,14 @@ def attention(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, b_o: Opti
     ws_bytes = lib.vtm_attention_workspace_bytes(B, L, Cc, heads)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
     y = torch.empty_like(x)
+    if seq_len is not None:
+        _require(seq_len, torch.int32, "seq_len")
+        with _Timed("KD", 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc, 4.0 * B * L * Cc + 8.0 * Cc * Cc):
+            check(lib.vtm_attention_dev(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), B, L, Cc, heads,
+                                        float(scale), 1 if shared_qk else 0, seq_len.data_ptr(), y.data_ptr(),
+                                        ws.data_ptr(), ws_bytes, _stream()), "vtm_attention_dev")
+        STATS.launches += 3
+        return y
     with _Timed("KD", 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc, 4.0 * B * L * Cc + 8.0 * Cc * Cc):
         check(lib.vtm_attention_ex(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), B, L, Cc, heads,
                                    float(scale), 1 if shared_qk else 0, y.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),

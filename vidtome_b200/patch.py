@@ -37,6 +37,9 @@ class MergePlan:
     randf: List[Any] = field(default_factory=list)      # ints (eager) or 1-element int32 CUDA tensors (graph capture)
     coin: Any = None                      # float (host coin) or 1-element fp32 CUDA tensor (device coin, DEVICE_COIN / capture)
     mu: Optional[torch.Tensor] = None     # [B'|1, L_local] int32: local merged token i = table row mu[i] (before a global stage)
+    # GlobalTokenStore stage: merged_tokens is sized for capacity and its first seq_len rows (a 1-element int32 CUDA
+    # tensor) are the merged sequence; KD reads the length on the device
+    seq_len: Optional[torch.Tensor] = None
 
     def unmerge(self, y: torch.Tensor, **kwarg) -> torch.Tensor:
         """u_a of the reference (patch.py:85,168): all unmerges + split_frame, one gather pass."""
@@ -73,6 +76,102 @@ GLOBAL_EXCHANGE = "recurrence"
 # (VtmSplit.prefix_coin), so nothing is read back to the host.  Results are bit-identical to the host coin.  It needs
 # both sets to be equally long (equal chunks); eagerly, a block whose sets differ keeps the host coin.
 DEVICE_COIN = False
+
+
+class GlobalTokenStore:
+    """A block's global tokens at a fixed address: `tokens` [B, cap, C] fp16 and their count `length` (a 1-element int32
+    CUDA tensor), allocated once, eagerly, outside any CUDA-graph pool.  Set it as `module.global_tokens` and
+    build_merge_plan runs the global stage of patch.py:59-82 with the counts that depend on the coin kept on the device
+    (VtmSplit.prefix_coin_dev), eagerly or under capture, so that chunks of different lengths can follow each other in
+    one captured sequence.  `cap` is the local merged length of a chunk of `max_frames` frames.  `filled` is the host's
+    knowledge of whether the store holds tokens (the reference's `global_tokens is not None`); `reset()` empties it,
+    as `update_patch(global_tokens=None)` does for a plain tensor."""
+
+    def __init__(self, max_frames: int):
+        if not isinstance(max_frames, int) or max_frames <= 0:
+            raise ValueError(f"GlobalTokenStore: max_frames must be a positive int, got {max_frames!r}")
+        self.max_frames = max_frames
+        self.tokens: Optional[torch.Tensor] = None
+        self.length: Optional[torch.Tensor] = None
+        self.filled = False
+
+    @property
+    def cap(self) -> int:
+        return 0 if self.tokens is None else self.tokens.shape[1]
+
+    def reset(self) -> None:
+        """Empty the store (host state only: `length` is meaningful while `filled`, and the next write sets it)."""
+        self.filled = False
+
+    def ensure(self, B: int, C: int, tsize: int, args: Dict[str, Any], device) -> None:
+        if self.tokens is not None and tuple(self.tokens.shape[::2]) == (B, C) and self.tokens.device == device:
+            return
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("GlobalTokenStore: the store is allocated by an eager call, before any capture")
+        cap = local_merged_len(self.max_frames, tsize, args)
+        self.tokens = torch.zeros((B, cap, C), dtype=torch.float16, device=device)
+        self.length = torch.zeros(1, dtype=torch.int32, device=device)
+        self.filled = False
+
+    def write(self, rows: torch.Tensor) -> None:
+        """global_tokens <- rows [B, L, C] (L <= cap): the first L rows and the length."""
+        self.tokens[:, :rows.shape[1]].copy_(rows)
+        self.length.fill_(rows.shape[1])
+        self.filled = True
+
+
+def local_merged_len(frames: int, tsize: int, args: Dict[str, Any]) -> int:
+    """Length of the local merged token set of a chunk of `frames` frames of `tsize` tokens (the counts of
+    build_merge_plan's local levels, computed on the host; with F % stride != 0 they assume the draw randf = 0)."""
+    L, unm, curF = frames * tsize, 0, frames
+    ratio = args["local_merge_ratio"]
+    while curF > 1:
+        if ratio <= 0:
+            unm += (L - unm) // curF
+        else:
+            ns, nd = ops.split_counts(VtmSplit.local(L, unm, curF, args["target_stride"], 0))
+            r = ops.merge_count(ns, ratio)
+            unm += ns - r
+            L = ns - r + nd
+        curF = (L - unm) // tsize
+    return L
+
+
+def _global_stage_store(module, store: GlobalTokenStore, table, mu, pi, ln, args, levels, tsize):
+    """patch.py:59-82 on a GlobalTokenStore.  As in _global_stage_device_coin the sets are stored as cat = [local (L
+    rows) | global (store.cap rows, the first *store.length valid)] and the coin picks the src half, but the lengths may
+    differ, so Ns, Nd, r and the merged length M are derived and read on the device (VtmSplit.prefix_coin_dev).  The
+    merged tokens are [B, L + cap, C], zero past M.  Returns (merged tokens, composed unmerge map, coin, M tensor)."""
+    B, _, C = table.shape
+    L = mu.shape[1]
+    store.ensure(B, C, tsize, args, table.device)
+    if L > store.cap:
+        raise RuntimeError(f"GlobalTokenStore: {L} local tokens exceed the store's capacity of {store.cap} "
+                           f"(max_frames={store.max_frames})")
+    if not store.filled:                                                    # patch.py:81-82: no global tokens yet
+        local = ops.gather_rows(table, mu, ln=ln)
+        store.write(local)
+        return local, pi, None, None
+    coin = draw_coin(module.generator, on_device=True)                      # patch.py:62
+    gratio = args["global_merge_ratio"]
+    if gratio <= 0:
+        raise ValueError("not enough values to unpack (expected 3, got 2)")  # as the host-coin path
+    cap = store.cap
+    cat = torch.empty((B, L + cap, C), dtype=torch.float16, device=table.device)
+    ops.gather_rows(table, mu, ln=ln, out=cat[:, :L])                       # merged local tokens, straight into cat
+    cat[:, L:].copy_(store.tokens)
+    split = VtmSplit.prefix_coin_dev(L, store.length, cap, coin, args["global_rand"])
+    m = merge.match_level_dev(cat, split, gratio, bool(args["align_batch"]))   # patch.py:73-74
+    levels.append(m)
+    merged_len = m.counts[3:4]
+    mu_g, tau = ops.compose_maps_dev(split, m.counts, m.keys, m.edge, m.rank, None, L + cap)
+    merged_tokens = ops.gather_rows_dev(cat, mu_g, merged_len)             # patch.py:75
+    if pi.shape[0] != tau.shape[0]:
+        pi = pi.expand(tau.shape[0], -1).contiguous()
+    _, pi = ops.compose_maps_dev(split, m.counts, m.keys, m.edge, m.rank, pi, pi.shape[1])
+    # patch.py:80, the local half.  Last: the split reads the global length from the store, which this rewrites.
+    store.write(ops.unmerge_add(merged_tokens, tau[:, :L], None))
+    return merged_tokens, pi, coin, merged_len
 
 
 def _fusable_layer_norm(norm: torch.nn.Module, x: torch.Tensor):
@@ -161,6 +260,13 @@ def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[s
     coin = None
     if args["merge_global"]:                                                 # patch.py:59
         g = getattr(module, "global_tokens", None)
+        if isinstance(g, GlobalTokenStore):
+            if GLOBAL_EXCHANGE != "recurrence":
+                raise RuntimeError(f"GlobalTokenStore needs GLOBAL_EXCHANGE='recurrence' (got {GLOBAL_EXCHANGE!r}): "
+                                   f"the cross-rank exchange modes keep their own global tokens")
+            merged_tokens, pi, coin, seq_len = _global_stage_store(module, g, table, mu, pi, ln, args, levels, tsize)
+            return MergePlan(fsize=fsize, N0=N0, merged_tokens=merged_tokens, pi=pi, levels=levels, randf=randfs,
+                             coin=coin, mu=mu, seq_len=seq_len)
         if x.is_cuda and torch.cuda.is_current_stream_capturing():
             if GLOBAL_EXCHANGE != "recurrence":
                 raise RuntimeError(f"CUDA-graph capture of global merging needs GLOBAL_EXCHANGE='recurrence' (got "
@@ -351,7 +457,12 @@ def make_diffusers_tome_block(block_class: Type[torch.nn.Module]) -> Type[torch.
                     shared = _pnp.injection_active(self.attn1)
                     if shared and norm_hidden_states.shape[0] != self.attn1._vtm_pnp:
                         raise RuntimeError("PnP injection needs one merged token set per input (batch_size == num_inputs)")
-                attn_output = _attention.self_attention(self.attn1, norm_hidden_states, shared_qk=shared)  # KD
+                attn_output = _attention.self_attention(self.attn1, norm_hidden_states, shared_qk=shared,
+                                                        seq_len=plan.seq_len)                             # KD
+            elif plan is not None and plan.seq_len is not None:
+                raise RuntimeError("GlobalTokenStore: the merged tokens are sized for capacity with their length on the "
+                                   "device, which only the library's self-attention (KD) reads; this block's attn1 "
+                                   "runs its own forward")
             else:
                 attn_output = self.attn1(
                     norm_hidden_states,
