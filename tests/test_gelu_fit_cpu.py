@@ -1,0 +1,55 @@
+"""CPU emulation of GegluEpi's gelu (`gelu_x2` in csrc/linear.cu) over every finite fp16 gate.  The coefficients are read
+from the source, so a refit is checked here before it reaches a GPU: every gate must be within one ulp of the correctly
+rounded gelu, and zero wherever that is zero, allowing for ex2.approx's relative error of 2^-22 either way."""
+import os
+import re
+
+import pytest
+import torch
+
+SRC = os.path.join(os.path.dirname(__file__), "..", "vidtome_b200", "csrc", "linear.cu")
+
+
+def _gelu_source():
+    src = open(SRC).read()
+    body = src[src.index("void gelu_x2("):]
+    return body[:body.index("\n}")]
+
+
+def _f32(x):
+    return x.float().double()
+
+
+def _emulate(g, coefs, ex2_rel):
+    """The kernel's fp32 steps for fp16 gates g (float64 tensor): FMAs rounded once, ex2 scaled by (1 + ex2_rel)."""
+    t = g.abs()
+    p = torch.full_like(t, coefs[0])
+    for c in coefs[1:]:
+        p = _f32(p * t + c)
+    assert torch.isfinite(p).all(), "the polynomial overflows fp32"
+    h = _f32(torch.exp2(p) * (1 + ex2_rel))
+    gh = _f32(g * h)
+    return torch.where(g >= 0, _f32(g - gh), gh).float().half()
+
+
+def _ordered(h):
+    b = h.view(torch.int16).int()
+    return torch.where(b < 0, -(b & 0x7FFF), b)
+
+
+@pytest.mark.parametrize("ex2_rel", (0.0, 2.0 ** -22, -2.0 ** -22))
+def test_gelu_fit_within_one_ulp(ex2_rel):
+    body = _gelu_source()
+    coefs = [float(torch.tensor(float(c)).float()) for c in re.findall(r"f32x2_pack\((-?[0-9][0-9.e+-]*)f,", body)]
+    assert len(coefs) >= 3 and coefs[-1] == -1.0, coefs
+    h = torch.arange(-32768, 32768, dtype=torch.int32).to(torch.int16).view(torch.float16)
+    g = h[torch.isfinite(h)].double()
+    ref = (g * torch.special.ndtr(g)).numpy().astype("float16")   # numpy rounds float64 -> fp16 once
+    ref = torch.from_numpy(ref)
+    y = _emulate(g, coefs, ex2_rel)
+    dist = (_ordered(y) - _ordered(ref)).abs()
+    i = int(dist.argmax())
+    assert dist[i] <= 1, f"gelu({g[i].item()!r}) = {y[i].item()!r}, correctly rounded {ref[i].item()!r}"
+    # the flushed negative tail (near g = 0 a zero result sits at a rounding midpoint, where ex2's error decides)
+    tail = (ref == 0) & (g < -1)
+    assert (y[tail] == 0).all(), f"non-zero gelu at g = {g[tail][y[tail] != 0][:4].tolist()}"

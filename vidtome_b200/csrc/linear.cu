@@ -103,21 +103,27 @@ struct StoreEpi {
   __device__ __forceinline__ void end(int, int, int) {}
 };
 
-// gelu(g) = 0.5 g (1 + erf(g / sqrt 2)) with ONE MUFU op: for z = |g| / sqrt 2, log2(erfc(z)) is smooth and close to a
-// parabola, so h = erfc(z) / 2 = 2^(p(z) - 1) with a degree-5 polynomial p (p(0) = 0; fitted for minimal error of erf on
-// [0, 4.2]: |erf error| <= 6e-7, |gelu error| <= 1.1e-6 — four orders below fp16 resolution), z clamped at 4.2
-// (erfc(4.2) = 3e-9).  Then gelu(g) = g (1 - h) for g >= 0 and g h for g < 0.  Two values at a time.
+// gelu(g) = 0.5 g (1 + erf(g / sqrt 2)) with ONE MUFU op: for t = |g|, log2(erfc(t / sqrt 2)) is smooth and close to a
+// parabola, so h = erfc(t / sqrt 2) / 2 = 2^(p(t) - 1) with a degree-7 polynomial p (p(0) = 0), fitted minimax to
+// log2(erfc(t / sqrt 2)) on [0, 5.94].  The fit bounds the exponent's absolute error (5.7e-6), i.e. h's RELATIVE error
+// (4e-6), so g h stays accurate in the negative tail where h is tiny.  t is not clamped: past 5.94 p keeps falling
+// (its leading coefficient is negative and it is monotonic up to 65504, with no fp32 overflow), so |g| h < 2^-26 and
+// g h rounds to -0 in fp16 as gelu does, and ex2 flushes h to 0 once p < -126.  Holding h at its value at a clamp instead
+// would let g h grow with |g|.  Then gelu(g) = g (1 - h) for g >= 0 and g h for g < 0: over every finite fp16 gate the
+// fp16 result is within one ulp of the correctly rounded gelu, and zero wherever that is (+0 at g = -0).  Two values at
+// a time.
 __device__ __forceinline__ void gelu_x2(float g0, float g1, float& y0, float& y1) {
-  const float z0 = fminf(fabsf(g0) * 0.7071067811865476f, 4.2f), z1 = fminf(fabsf(g1) * 0.7071067811865476f, 4.2f);
-  const uint64_t z2 = f32x2_pack(z0, z1);
-  uint64_t p2 = f32x2_fma(f32x2_pack(-0.00294415686f, -0.00294415686f), z2, f32x2_pack(0.0295900391f, 0.0295900391f));
-  p2 = f32x2_fma(p2, z2, f32x2_pack(-0.148665626f, -0.148665626f));
-  p2 = f32x2_fma(p2, z2, f32x2_pack(-0.918509366f, -0.918509366f));
-  p2 = f32x2_fma(p2, z2, f32x2_pack(-1.62788901f, -1.62788901f));
-  p2 = f32x2_fma(p2, z2, f32x2_pack(-1.f, -1.f));                      // p(z) - 1
+  const uint64_t t2 = f32x2_pack(fabsf(g0), fabsf(g1));
+  uint64_t p2 = f32x2_fma(f32x2_pack(-1.79155074e-06f, -1.79155074e-06f), t2, f32x2_pack(6.06881658e-05f, 6.06881658e-05f));
+  p2 = f32x2_fma(p2, t2, f32x2_pack(-0.000922937703f, -0.000922937703f));
+  p2 = f32x2_fma(p2, t2, f32x2_pack(0.00847607013f, 0.00847607013f));
+  p2 = f32x2_fma(p2, t2, f32x2_pack(-0.0538897403f, -0.0538897403f));
+  p2 = f32x2_fma(p2, t2, f32x2_pack(-0.458542407f, -0.458542407f));
+  p2 = f32x2_fma(p2, t2, f32x2_pack(-1.15121424f, -1.15121424f));
+  p2 = f32x2_fma(p2, t2, f32x2_pack(-1.f, -1.f));                      // p(t) - 1
   float p0, p1;
   f32x2_unpack(p2, p0, p1);
-  const float h0 = ex2_approx(p0), h1 = ex2_approx(p1);                 // erfc(z) / 2
+  const float h0 = ex2_approx(p0), h1 = ex2_approx(p1);                 // erfc(t / sqrt 2) / 2
   const float gh0 = g0 * h0, gh1 = g1 * h1;
   y0 = g0 >= 0.f ? g0 - gh0 : gh0;
   y1 = g1 >= 0.f ? g1 - gh1 : gh1;
