@@ -293,7 +293,9 @@ int vtm_attention(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev,
 
 /* KD with options.  flags bit 0 (VTM_ATTN_SHARED_QK): PnP's source-sample injection (utils/pnp_utils.py:57-68,87-91: the
  * attention map softmax(q k^T) is computed from sample 0 only and `repeat`ed over the batch): every sample b uses the
- * queries and keys of sample 0 and its own values.  Other bits must be zero (VTM_E_UNSUPPORTED). */
+ * queries and keys of sample 0 and its own values.  q and k of samples 1..B-1 are not computed (their part of the
+ * workspace is left as it was), and the map is computed once for a group of samples.  Other bits must be zero
+ * (VTM_E_UNSUPPORTED). */
 #define VTM_ATTN_SHARED_QK 1
 int vtm_attention_ex(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
                      int32_t B, int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, void* y_dev,

@@ -7,7 +7,8 @@
 // Flash-attention kernel (flash_attn_kernel below): one CTA per (64 x CW-row query tile, head, sample), a TMA producer
 // warpgroup streaming K/V tiles of one head (contiguous runs of the head-major padded buffers written by the projection
 // epilogue) through an mbarrier ring, and CW = 3 (head_dim <= 80) or 2 wgmma consumer warpgroups running S = Q K^T, the
-// online softmax and O += P V with P kept in registers, each overlapping its softmax with its own P V.
+// online softmax and O += P V with P kept in registers, each overlapping its softmax with its own P V.  A shared (PnP)
+// call serves G samples per CTA with one softmax (see flash_attn_kernel).
 #include <stdlib.h>
 
 #include "gemm_sm90.cuh"
@@ -33,7 +34,7 @@ struct HeadSplitEpi {
   int M, C, H, d, L, DP, nb; // M = nb*L rows, C = H*d
   int dread;                 // columns of a padded row that the flash kernel reads: 16 x (its k-step count) <= DP
   int which0, n_proj;        // this GEMM produces projections which0 .. which0 + n_proj - 1 of (q, k, v); N = n_proj * C
-  long long which_stride;    // B*H*L*DP
+  long long which_stride;    // distance between the projections: B*H*L*DP
   int row0;                  // first of the warp's 32 rows
   int b0, l0;                // (sample, position) of row0 + lane / 8, this lane's first row in the store phase
   uint32_t scratch;
@@ -117,9 +118,9 @@ struct HeadSplitEpi {
 inline int fa_columns_read(int d) { return 16 * ((d + 15) / 16); }
 
 // x [nb * L, K] -> projections which0 .. which0 + n_proj - 1 of (q, k, v), head-major padded, at `out`
-// ([n_proj][nb][H][L][DP]); w [n_proj * C, K].
+// ([n_proj][nb][H][L][DP], or projections `which_stride` halfs apart when it is > 0); w [n_proj * C, K].
 int launch_head_proj(const void* x, const void* w, __half* out, int nb, int L, int K, int C, int H, int DP, int which0,
-                     int n_proj, cudaStream_t stream) {
+                     int n_proj, cudaStream_t stream, long long which_stride = 0) {
   int sms = 0;
   int rc = gemm::device_sms(&sms);
   if (rc) return rc;
@@ -128,7 +129,7 @@ int launch_head_proj(const void* x, const void* w, __half* out, int nb, int L, i
   epi.qkvh = out; epi.M = M; epi.C = C; epi.H = H; epi.d = C / H; epi.L = L; epi.DP = DP;
   epi.dread = fa_columns_read(C / H);
   epi.which0 = which0; epi.n_proj = n_proj;
-  epi.which_stride = static_cast<long long>(nb) * H * L * DP; epi.row0 = 0; epi.scratch = 0; epi.b0 = 0; epi.l0 = 0; epi.nb = nb;
+  epi.which_stride = which_stride > 0 ? which_stride : static_cast<long long>(nb) * H * L * DP; epi.row0 = 0; epi.scratch = 0; epi.b0 = 0; epi.l0 = 0; epi.nb = nb;
   epi.bw = 0; epi.lw = 0; epi.inv_c = 1.f / static_cast<float>(C); epi.inv_d = 1.f / static_cast<float>(C / H);
   CUtensorMap ta, tb;
   rc = make_tmap_3d_f16(&ta, x, K, M, 1, K, static_cast<uint64_t>(M) * K, gemm::BK, gemm::BM);
@@ -145,17 +146,20 @@ constexpr int FA_BKV = 64;       // keys per K/V tile
 
 struct FaParams {
   __half* o;          // [B*Lq, C]
-  int L, Lq, H, d, C;
+  int L, Lq, H, d, C, B;
   const int* len_dev; // DL: the sequence length on the device (self-attention, <= L == Lq, the buffers' row count)
   float scale_log2;   // softmax scale * log2(e)
   int qk_shared;      // PnP injection (utils/pnp_utils.py:57-68,87-91): q and k of sample 0 for every sample, v per sample
 };
 
-template <int KS>
+constexpr size_t FA_SMEM_MAX = 227 * 1024;   // dynamic shared memory a CTA may opt in to on sm_90
+
+template <int KS, int G = 1>
 struct FaCfg {
   // Consumer warpgroups, 64 query rows each.  Three (512 threads, at most 128 registers each) hide more of the softmax's
-  // latency than two; from head_dim 96 on, O no longer fits next to S and P in 128 registers, so those keep two.
-  static constexpr int CW = KS <= 5 ? 3 : 2;
+  // latency than two; from head_dim 96 on, O no longer fits next to S and P in 128 registers, so those keep two.  A
+  // CTA that serves G > 1 samples holds G accumulators O and keeps two (up to 168 registers each).
+  static constexpr int CW = G == 1 && KS <= 5 ? 3 : 2;
   static constexpr int BQ = 64 * CW;                      // query rows per CTA
   static constexpr int THREADS = 128 * (CW + 1);          // producer warpgroup + consumers
   static constexpr int DV = 16 * KS;                      // head_dim rounded up to 16: k-steps of Q K^T, width of O
@@ -164,12 +168,19 @@ struct FaCfg {
   static constexpr uint32_t KV_ATOM = FA_BKV * 128;       // [64 rows x 128 B]
   static constexpr uint32_t Q_BYTES = ATOMS * Q_ATOM;
   static constexpr uint32_t TILE_BYTES = ATOMS * KV_ATOM;
-  static constexpr uint32_t STAGE_BYTES = 2 * TILE_BYTES; // K + V
+  static constexpr uint32_t STAGE_BYTES = (1 + G) * TILE_BYTES; // K + the V tiles of G samples
   // K/V ring depth.  The consumers hold two stages at a time (Q K^T of tile j+1 is issued before P V of tile j), so
-  // four stages keep two tile loads in flight; five timed the same at both bench shapes.
-  static constexpr int STAGES = 4;
+  // four stages keep two tile loads in flight; five timed the same at both bench shapes.  Wide grouped stages get as
+  // many as fit (three at head_dim > 64 and G = 3: one load in flight).
+  static constexpr int STAGES_FIT = static_cast<int>((FA_SMEM_MAX - 1024 - Q_BYTES - 256) / STAGE_BYTES);
+  static constexpr int STAGES = STAGES_FIT < 4 ? STAGES_FIT : 4;
+  static_assert(STAGES >= 3, "the consumers hold two stages: a third keeps a load in flight");
   static constexpr size_t SMEM_BYTES = 1024 + Q_BYTES + static_cast<size_t>(STAGES) * STAGE_BYTES + 256;
 };
+
+// Largest number of samples one CTA serves in a shared (PnP) call at KS k-steps: G accumulators O of DV / 2 registers
+// each next to S and P without spills (ptxas -v; DESIGN §4).
+constexpr int fa_group_max(int KS) { return KS <= 2 ? 4 : KS == 3 ? 3 : KS <= 5 ? 2 : 1; }
 
 // Online softmax of one 64-key tile of S in the log2 domain.  The thread holds rows r0 = lane/4 (s[4n], s[4n+1]) and
 // r0 + 8 (s[4n+2], s[4n+3]), columns 8n + 2(lane%4).  On return s holds P = ex2(s * scale - m_new), m_r the new row
@@ -230,11 +241,17 @@ __device__ __forceinline__ void fa_softmax(float (&s)[32], float (&m_r)[2], floa
 // one run on the tensor cores while the others are in their softmax.
 // DL (device length): the buffers hold p.L rows per head and sample, of which the first *p.len_dev are the sequence.  Query
 // tiles at or past it exit, and only keys below it take part, masked in the last tile exactly as keys past p.L are.
-template <int KS, bool DL = false>
-__global__ void __launch_bounds__(FaCfg<KS>::THREADS, 1)
+//
+// G > 1 (shared calls only: every sample has the attention map of sample 0): the CTA serves samples G z .. G z + G - 1.
+// Each stage holds K of sample 0 and the V tiles of its G samples; S and the softmax are computed once and each sample's
+// O_g += P V_g is one wgmma per 16-key step, with the same shape as at G = 1, so every output element sees the same
+// roundings as in the CTA of its own sample.  Samples past B (the last group of a ragged split) read the V of sample
+// B - 1 and write nothing.
+template <int KS, int G, bool DL>
+__global__ void __launch_bounds__(FaCfg<KS, G>::THREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                   const __grid_constant__ CUtensorMap tm_v, const FaParams p) {
-  using Cf = FaCfg<KS>;
+  using Cf = FaCfg<KS, G>;
   constexpr int DV = Cf::DV;
   constexpr int STAGES = Cf::STAGES;
   extern __shared__ uint8_t fa_smem[];
@@ -247,12 +264,11 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
   auto kv_empty = [&](int s) { return bars + 8u * (1 + STAGES + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
-  const int q0 = blockIdx.x * Cf::BQ, h = blockIdx.y, b = blockIdx.z;
+  const int q0 = blockIdx.x * Cf::BQ, h = blockIdx.y, b0 = blockIdx.z * G;
   const int seq = DL ? __ldg(p.len_dev) : p.L;               // keys that take part
   const int q_valid = DL ? seq : p.Lq;                       // query rows that are written
   if (DL && q0 >= q_valid) return;
-  const int sqk = (p.qk_shared ? 0 : b) * p.H + h;           // slab of q / k
-  const int sv = b * p.H + h;                                // slab of v
+  const int sqk = (p.qk_shared ? 0 : b0) * p.H + h;          // slab of q / k
   const int nkv = (seq + FA_BKV - 1) / FA_BKV;
 
   if (threadIdx.x == 0) {
@@ -281,7 +297,10 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
         mbar_arrive_expect_tx(kv_full(stage), Cf::STAGE_BYTES);
         for (int a = 0; a < Cf::ATOMS; ++a) {
           tma_load_3d(st + a * Cf::KV_ATOM, &tm_k, kv_full(stage), 64 * a, j * FA_BKV, sqk);
-          tma_load_3d(st + Cf::TILE_BYTES + a * Cf::KV_ATOM, &tm_v, kv_full(stage), 64 * a, j * FA_BKV, sv);
+          for (int g = 0; g < G; ++g) {
+            const int sv = (G == 1 ? b0 : min(b0 + g, p.B - 1)) * p.H + h;   // slab of v
+            tma_load_3d(st + (1 + g) * Cf::TILE_BYTES + a * Cf::KV_ATOM, &tm_v, kv_full(stage), 64 * a, j * FA_BKV, sv);
+          }
         }
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
@@ -291,9 +310,11 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
 
   // ===================== consumers: 64 query rows per warpgroup =====================
   const int cg = wg - 1, wq = warp & 3;
-  float o[DV / 2];
+  float o[G][DV / 2];
 #pragma unroll
-  for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
+  for (int g = 0; g < G; ++g)
+#pragma unroll
+    for (int i = 0; i < DV / 2; ++i) o[g][i] = 0.f;
   float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};   // rows 16 wq + lane/4 and + 8 of the warpgroup's 64
   float s[32], alpha[2];
   uint32_t pa[4][4];                                            // P as the register A operand of the four 16-key steps
@@ -310,10 +331,13 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     wgmma_commit();
   };
   auto issue_pv = [&](int st) {
-    const uint32_t vt = skv + st * Cf::STAGE_BYTES + Cf::TILE_BYTES;
 #pragma unroll
-    for (int kb = 0; kb < 4; ++kb)                // 16 keys per step: +16 rows x 128 B of the V tile
-      wgmma_rs_f16_bt<DV>(o, pa[kb], wgmma_desc_sw128_mnmajor(vt + kb * 2048u, Cf::KV_ATOM), 1u);
+    for (int g = 0; g < G; ++g) {
+      const uint32_t vt = skv + st * Cf::STAGE_BYTES + (1 + g) * Cf::TILE_BYTES;
+#pragma unroll
+      for (int kb = 0; kb < 4; ++kb)              // 16 keys per step: +16 rows x 128 B of the V tile
+        wgmma_rs_f16_bt<DV>(o[g], pa[kb], wgmma_desc_sw128_mnmajor(vt + kb * 2048u, Cf::KV_ATOM), 1u);
+    }
     wgmma_commit();
   };
   auto fence_s = [&]() {
@@ -322,7 +346,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
   };
   auto fence_o = [&]() {
 #pragma unroll
-    for (int i = 0; i < DV / 2; ++i) reg_fence(o[i]);
+    for (int g = 0; g < G; ++g)
+#pragma unroll
+      for (int i = 0; i < DV / 2; ++i) reg_fence(o[g][i]);
   };
   auto pack_p = [&]() {
 #pragma unroll
@@ -377,10 +403,12 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     fence_o();
     release(prev);
 #pragma unroll
-    for (int n = 0; n < DV / 8; ++n) {
-      o[4 * n] *= alpha[0]; o[4 * n + 1] *= alpha[0];
-      o[4 * n + 2] *= alpha[1]; o[4 * n + 3] *= alpha[1];
-    }
+    for (int g = 0; g < G; ++g)
+#pragma unroll
+      for (int n = 0; n < DV / 8; ++n) {
+        o[g][4 * n] *= alpha[0]; o[g][4 * n + 1] *= alpha[0];
+        o[g][4 * n + 2] *= alpha[1]; o[g][4 * n + 3] *= alpha[1];
+      }
     pack_p();
     prev = stage;
     if (++stage == STAGES) { stage = 0; phase ^= 1u; }
@@ -403,21 +431,26 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     const float inv = 1.f / l;
     const int row = q0 + cg * 64 + wq * 16 + (lane >> 2) + 8 * r;
     if (row >= q_valid) continue;
-    __half* dst = p.o + (static_cast<size_t>(b) * p.Lq + row) * p.C + h * p.d;
 #pragma unroll
-    for (int n = 0; n < DV / 8; ++n) {
-      const int col = n * 8 + 2 * (lane & 3);
-      if (col < p.d)
-        *reinterpret_cast<uint32_t*>(dst + col) = pack_f16x2(o[4 * n + 2 * r] * inv, o[4 * n + 2 * r + 1] * inv);
+    for (int g = 0; g < G; ++g) {
+      if (G > 1 && b0 + g >= p.B) break;
+      __half* dst = p.o + (static_cast<size_t>(b0 + g) * p.Lq + row) * p.C + h * p.d;
+#pragma unroll
+      for (int n = 0; n < DV / 8; ++n) {
+        const int col = n * 8 + 2 * (lane & 3);
+        if (col < p.d)
+          *reinterpret_cast<uint32_t*>(dst + col) = pack_f16x2(o[g][4 * n + 2 * r] * inv, o[g][4 * n + 2 * r + 1] * inv);
+      }
     }
   }
 }
 
-template <int KS, bool DL = false>
+template <int KS, int G, bool DL>
 int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, int B, int Lq, int L, int C, int H,
-              int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev = nullptr) {
-  using Cf = FaCfg<KS>;
+              int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev) {
+  using Cf = FaCfg<KS, G>;
   if (H > 65535 || B > 65535 || Cf::ATOMS * 64 > DP) return VTM_E_SHAPE;
+  if (G > 1 && !qk_shared) return VTM_E_UNSUPPORTED;
   constexpr int BQ = Cf::BQ;
   const uint64_t BH = static_cast<uint64_t>(B) * H;
   CUtensorMap tq, tk, tv;
@@ -433,29 +466,53 @@ int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, i
   rc = cuda_rc(cudaGetDevice(&dev));
   if (rc) return rc;
   if (dev < 0 || dev >= 64 || !opted[dev]) {
-    rc = cuda_rc(cudaFuncSetAttribute(flash_attn_kernel<KS, DL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    rc = cuda_rc(cudaFuncSetAttribute(flash_attn_kernel<KS, G, DL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       static_cast<int>(Cf::SMEM_BYTES)));
     if (rc) return rc;
     if (dev >= 0 && dev < 64) opted[dev] = true;
   }
   FaParams p;
   p.o = o;
-  p.L = L; p.Lq = Lq; p.H = H; p.d = C / H; p.C = C;
+  p.L = L; p.Lq = Lq; p.H = H; p.d = C / H; p.C = C; p.B = B;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.qk_shared = qk_shared;
   p.len_dev = len_dev;
-  const dim3 grid(static_cast<unsigned>((Lq + BQ - 1) / BQ), static_cast<unsigned>(H), static_cast<unsigned>(B));
-  flash_attn_kernel<KS, DL><<<grid, Cf::THREADS, Cf::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  const dim3 grid(static_cast<unsigned>((Lq + BQ - 1) / BQ), static_cast<unsigned>(H),
+                  static_cast<unsigned>((B + G - 1) / G));
+  flash_attn_kernel<KS, G, DL><<<grid, Cf::THREADS, Cf::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   return launch_rc();
+}
+
+// launch_fa<KS, g, DL> for a run-time group size 1 <= g <= G
+template <int KS, int G, bool DL>
+int launch_fa_group(int g, const __half* qh, const __half* kh, const __half* vh, __half* o, int B, int Lq, int L, int C,
+                    int H, int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev) {
+  if constexpr (G > 1) {
+    if (g < G) return launch_fa_group<KS, G - 1, DL>(g, qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream, len_dev);
+  }
+  return launch_fa<KS, G, DL>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream, len_dev);
+}
+
+// Samples per CTA: 1, or for a shared call the fewest groups of at most fa_group_max(KS) samples, equally sized (so
+// that the last group reads as few clamped V tiles as possible).
+inline int fa_group(int KS, int B, int qk_shared) {
+  if (!qk_shared) return 1;
+  const int gmax = fa_group_max(KS);
+  const int groups = (B + gmax - 1) / gmax;
+  return (B + groups - 1) / groups;
 }
 
 int launch_fa_any(const __half* qh, const __half* kh, const __half* vh, __half* o, int B, int Lq, int L, int C, int H,
                   int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev = nullptr) {
-#define VTM_FA_CASE(KS)                                                                                       \
-  case KS:                                                                                                    \
-    return len_dev ? launch_fa<KS, true>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream, len_dev) \
-                   : launch_fa<KS>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream);
-  switch ((C / H + 15) / 16) {
+  const int ks = (C / H + 15) / 16;
+  const int g = fa_group(ks, B, qk_shared);
+#define VTM_FA_CASE(KS)                                                                                               \
+  case KS:                                                                                                            \
+    return len_dev ? launch_fa_group<KS, fa_group_max(KS), true>(g, qh, kh, vh, o, B, Lq, L, C, H, DP, scale,         \
+                                                                 qk_shared, stream, len_dev)                         \
+                   : launch_fa_group<KS, fa_group_max(KS), false>(g, qh, kh, vh, o, B, Lq, L, C, H, DP, scale,        \
+                                                                  qk_shared, stream, nullptr);
+  switch (ks) {
     VTM_FA_CASE(1)
     VTM_FA_CASE(2)
     VTM_FA_CASE(3)
@@ -499,10 +556,20 @@ int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev
   __half* qkv = static_cast<__half*>(ws_dev);
   __half* o = qkv + static_cast<size_t>(3) * B * heads * L * DP;
   const int M = B * L;
-  int rc = launch_head_proj(x_dev, w_qkv_dev, qkv, B, L, C, C, heads, DP, 0, 3, stream);
+  const size_t slab = static_cast<size_t>(B) * heads * L * DP;    // one of q, k, v for all samples
+  __half* kh = qkv + slab;
+  __half* vh = kh + slab;
+  int rc;
+  if (flags & 1) {
+    // shared: q and k of sample 0 (the only ones the flash kernel reads), v of every sample
+    rc = launch_head_proj(x_dev, w_qkv_dev, qkv, 1, L, C, C, heads, DP, 0, 2, stream, static_cast<long long>(slab));
+    if (rc) return rc;
+    rc = launch_head_proj(x_dev, static_cast<const __half*>(w_qkv_dev) + static_cast<size_t>(2) * C * C, vh, B, L, C, C,
+                          heads, DP, 2, 1, stream);
+  } else {
+    rc = launch_head_proj(x_dev, w_qkv_dev, qkv, B, L, C, C, heads, DP, 0, 3, stream);
+  }
   if (rc) return rc;
-  const __half* kh = qkv + static_cast<size_t>(B) * heads * L * DP;
-  const __half* vh = kh + static_cast<size_t>(B) * heads * L * DP;
   rc = launch_fa_any(qkv, kh, vh, o, B, L, L, C, heads, DP, scale, flags & 1, stream, len_dev);
   if (rc) return rc;
   return vtm_linear_f16(o, w_o_dev, b_o_dev, M, C, C, y_dev, C, stream_);

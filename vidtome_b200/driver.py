@@ -6,16 +6,18 @@ Restates, on synthetic latents, the parts of the reference's Generator that sit 
   pred_noise      generate.py:238-279   (CFG batch cat([x, x]), UNet forward, guidance combine)
   pred_next_x     generate.py:281-311   (closed-form DDIM step)
   post_iter       generate.py:233-236   (reset global tokens after each step)
-Text conditioning, VAE, ControlNet, PnP injection and file IO are outside the hot path and not restated.
+  init_pnp        generate.py:313-319   (PnP self-attention injection schedule; with `source_latents`)
+  pre_iter        generate.py:226-231   (PnP: set the timestep, fetch the source latents of the step)
+Text conditioning, VAE, ControlNet, PnP's conv-feature injection and file IO are outside the hot path and not restated.
 """
 from __future__ import annotations
 
-from typing import List, Optional
+from typing import Callable, Iterable, List, Optional
 
 import numpy as np
 import torch
 
-from . import patch
+from . import patch, pnp
 
 
 def ddim_alphas_cumprod(num_train_timesteps: int = 1000, beta_start: float = 0.00085,
@@ -38,7 +40,8 @@ class ChunkedDenoiser:
                  guidance_scale: float = 7.5, merge_global: bool = False, chunk_ord: str = "seq",
                  perm_div: float = 3.0, randomize_chunks: bool = False, cond: Optional[torch.Tensor] = None,
                  cuda_graph: bool = False, graph_warmup: int = 2, shard: bool = False, capture_global: bool = False,
-                 chunk_graphs: bool = False):
+                 chunk_graphs: bool = False, source_latents: Optional[Callable[[int], torch.Tensor]] = None,
+                 pnp_attn_t: float = 0.5, pnp_modules: Optional[Iterable[torch.nn.Module]] = None):
         """`cuda_graph=True`: after `graph_warmup` eager steps, the noise prediction of a whole step (every chunk:
         CFG batch, UNet forward with the merge path, guidance combine) is captured once into a CUDA graph and
         replayed; per step the host then issues one graph launch plus the DDIM update instead of ~250 kernel
@@ -63,7 +66,16 @@ class ChunkedDenoiser:
         `update_patch(global_tokens=None)`), whose global stage keeps the counts that depend on the coin on the device.
         Needs chunk lengths whose local counts do not depend on the frame draw (every length up to chunk_size when
         chunk_size <= target_stride; see draw_dependent_lengths), patch.GLOBAL_EXCHANGE == "recurrence", the library's
-        self-attention (KD) in every merged block, and no sharding."""
+        self-attention (KD) in every merged block, and no sharding.
+
+        `source_latents` (a callable t -> [flen, 4, h, w], the inverted source latents at timestep t; the reference's
+        load_latent) switches on PnP control, the reference's default generation (generate.py:60-68, `control: "pnp"`):
+        every UNet call gets the batch [source | x | x] with `cond` = [3, 77, D] (the pnp guidance "", uncond, cond text
+        embeddings, generate.py:101-109), and the first int(n_timesteps * pnp_attn_t) steps take the attention map of
+        the decoder self-attention modules from the source sample (pnp.register_attention_control; `pnp_modules` names
+        those modules for a model without the diffusers up_blocks hierarchy).  The model must be patched with
+        batch_size=3 and align_batch=True.  In every graph mode the injection is decided on the host when a graph is
+        captured, so graphs are keyed by it as well; the injected ones are released once the schedule has passed."""
         self.unet = unet
         # shard=True: this process is one rank of a torch.distributed job and takes chunks i % world == rank of every
         # step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
@@ -88,7 +100,8 @@ class ChunkedDenoiser:
             raise ValueError("cuda_graph=True needs merge_global=False and randomize_chunks=False (static work)")
         if self.capture_global and self.shard:
             raise ValueError("capture_global=True does not capture the cross-rank exchange of shard=True")
-        self._chunk_graphs = {}     # (chunk length, first in step, frame shape) -> (CUDAGraph, static x, static noise)
+        # (chunk length, first in step, frame shape, PnP injection) -> (CUDAGraph, static x, static noise, static source)
+        self._chunk_graphs = {}
         self._chunk_t = None        # the UNet's timestep input shared by the chunk graphs
         self._stores = []           # patch.GlobalTokenStore of every block (chunk_graphs with merge_global)
         self.chunk_size = chunk_size
@@ -104,6 +117,29 @@ class ChunkedDenoiser:
         self.alphas_cumprod = ddim_alphas_cumprod()
         self.final_alpha_cumprod = self.alphas_cumprod[0]     # set_alpha_to_one=False in SD's config
         self.timesteps = ddim_timesteps(n_timesteps)
+        self.source_latents = source_latents
+        self.pnp_schedule: List[int] = []
+        self._pnp_targets: List[torch.nn.Module] = []
+        if source_latents is not None:
+            self._init_pnp(n_timesteps, pnp_attn_t, pnp_modules)
+
+    # generate.py:60-68,313-319 (the attention half of init_pnp; conv injection is not restated)
+    def _init_pnp(self, n_timesteps: int, pnp_attn_t: float, modules):
+        args = self.unet._tome_info["args"] if hasattr(self.unet, "_tome_info") else None
+        if args is None or args["batch_size"] != 3 or not args["align_batch"]:
+            raise ValueError("PnP (source_latents) needs a model patched with batch_size=3 and align_batch=True "
+                             "(generate.py:96-98): the source, uncond and cond samples of every UNet call")
+        if self.cond is None or self.cond.dim() != 3 or self.cond.shape[0] != 3 or self.cond.shape[1] != 77:
+            raise ValueError("PnP (source_latents) needs cond = [3, 77, D]: the pnp guidance, uncond and cond text "
+                             "embeddings (generate.py:101-109)")
+        qk_t = int(n_timesteps * pnp_attn_t)
+        self.pnp_schedule = self.timesteps[:qk_t] if qk_t >= 0 else []
+        pnp.register_attention_control(self.unet, self.pnp_schedule, num_inputs=3, modules=modules)
+        self._pnp_targets = pnp._targets(self.unet, modules)
+
+    def injecting(self, t: int) -> bool:
+        """True if the self-attention of step t takes its map from the source sample (pnp.injection_active)."""
+        return self.source_latents is not None and (int(t) in self.pnp_schedule or int(t) == 1000)
 
     # generate.py:172-203
     def get_chunks(self, flen: int) -> List[torch.Tensor]:
@@ -135,12 +171,15 @@ class ChunkedDenoiser:
 
     # generate.py:238-279
     @torch.no_grad()
-    def pred_noise(self, x: torch.Tensor, t: int) -> torch.Tensor:
+    def pred_noise(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`src`: the source latents of the chunk (PnP), prepended to the batch."""
         flen = len(x)
         text = None if self.cond is None else self.cond.repeat_interleave(flen, dim=0)
         latent_model_input = torch.cat([x, x])                                # classifier-free guidance
+        if src is not None:
+            latent_model_input = torch.cat([src.to(x), latent_model_input])
         eps = self.unet(latent_model_input, t, encoder_hidden_states=text).sample
-        noise_pred_uncond, noise_pred_cond = eps.chunk(2)
+        noise_pred_uncond, noise_pred_cond = eps.chunk(2 if src is None else 3)[-2:]
         return noise_pred_uncond + self.guidance_scale * (noise_pred_cond - noise_pred_uncond)
 
     # generate.py:281-311 (inversion=False branch)
@@ -167,13 +206,13 @@ class ChunkedDenoiser:
                                    "use 'allgather' for ragged chunks")
         return chunks
 
-    def _all_noises(self, x: torch.Tensor, t) -> torch.Tensor:
+    def _all_noises(self, x: torch.Tensor, t, src: Optional[torch.Tensor] = None) -> torch.Tensor:
         noises = torch.zeros_like(x)
         for chunk in self._step_chunks(len(x)):
             # chunks are contiguous frame ranges (possibly visited in another order): slice instead of indexing with
             # a host tensor, which would cost a synchronous host->device copy per chunk per step
             lo, hi = int(chunk[0]), int(chunk[-1]) + 1
-            noises[lo:hi] = self.pred_noise(x[lo:hi], t)
+            noises[lo:hi] = self.pred_noise(x[lo:hi], t, None if src is None else src[lo:hi])
         return noises
 
     def _block_generators(self) -> List[torch.Generator]:
@@ -185,19 +224,24 @@ class ChunkedDenoiser:
                 gens.append(g)
         return gens
 
-    def _capture(self, x: torch.Tensor, t: int):
+    def _graph_key(self, x: torch.Tensor, t: int):
+        return tuple(x.shape), self.injecting(t)
+
+    def _capture(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor]):
         """Capture `_all_noises` for inputs shaped like `x` (called after the eager warm-up steps, so that every
         lazily created piece of state — generators forked by the hook, cached packed weights, the library handle,
         allocator pools — already exists)."""
+        self._graph = None                                                   # release the previous graph first
         gx = x.clone()
+        gsrc = None if src is None else src.to(x).clone()                    # the source latents, set per replay
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)      # the UNet's timestep input, set per replay
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = self._all_noises(gx, gt)
-        self._graph = (graph, gx, gt, gn, tuple(x.shape))
+            gn = self._all_noises(gx, gt, gsrc)
+        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gsrc)
 
     @staticmethod
     def slot_index(chunks: List[torch.Tensor], flen: int) -> torch.Tensor:
@@ -213,7 +257,7 @@ class ChunkedDenoiser:
             raise RuntimeError("slot_index: the chunks must cover every frame exactly once")
         return torch.stack([fwd, inv])
 
-    def _capture_slots(self, x: torch.Tensor, t: int):
+    def _capture_slots(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor]):
         """Capture the noise prediction of one step over chunk slots (capture_global=True): slot k runs chunk k of the
         step's visiting order on gx[k * chunk_size:(k + 1) * chunk_size].  get_chunks is not called here, so capturing
         consumes no draw of the host RNG that eager stepping would not."""
@@ -221,7 +265,9 @@ class ChunkedDenoiser:
         if patch.GLOBAL_EXCHANGE != "recurrence":
             raise RuntimeError(f"capture_global=True needs patch.GLOBAL_EXCHANGE='recurrence' (got "
                                f"{patch.GLOBAL_EXCHANGE!r}): the cross-rank exchange is not captured")
+        self._graph = None                                                   # release the previous graph first
         gx = x.clone()
+        gsrc = None if src is None else src.to(x).clone()                   # source latents in slot order
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
@@ -231,26 +277,29 @@ class ChunkedDenoiser:
         with torch.cuda.graph(graph):
             gn = torch.zeros_like(gx)
             for k in range(flen // cs):
-                gn[k * cs:(k + 1) * cs] = self.pred_noise(gx[k * cs:(k + 1) * cs], gt)
+                gn[k * cs:(k + 1) * cs] = self.pred_noise(gx[k * cs:(k + 1) * cs], gt,
+                                                          None if gsrc is None else gsrc[k * cs:(k + 1) * cs])
         idx_dev = torch.empty((2, flen), dtype=torch.int64, device=x.device)
         idx_host = torch.empty((2, flen), dtype=torch.int64).pin_memory()
         copied = torch.cuda.Event()          # the pinned buffer is rewritten only after its last upload has run
-        self._graph = (graph, gx, gt, gn, tuple(x.shape), idx_dev, idx_host, copied)
+        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), idx_dev, idx_host, copied, gsrc)
 
-    def _slot_noises(self, x: torch.Tensor, t: int) -> torch.Tensor:
+    def _slot_noises(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None) -> torch.Tensor:
         flen = len(x)
         if flen % self.chunk_size != 0:
             raise RuntimeError(f"capture_global=True needs a frame count divisible by chunk_size (got {flen} frames, "
                                f"chunk_size {self.chunk_size}): chunks of unequal length cannot share one graph")
         order = self.slot_index(self.get_chunks(flen), flen)        # the same host draws as eager stepping
-        if self._graph is None or self._graph[4] != tuple(x.shape):
-            self._capture_slots(x, t)
-        graph, gx, gt, gn, _, idx_dev, idx_host, copied = self._graph
+        if self._graph is None or self._graph[4] != self._graph_key(x, t):
+            self._capture_slots(x, t, src)
+        graph, gx, gt, gn, _, idx_dev, idx_host, copied, gsrc = self._graph
         copied.synchronize()
         idx_host.copy_(order)
         idx_dev.copy_(idx_host, non_blocking=True)
         copied.record()
         torch.index_select(x, 0, idx_dev[0], out=gx)                # latents -> slots
+        if gsrc is not None:
+            torch.index_select(src.to(x), 0, idx_dev[0], out=gsrc)
         gt.fill_(int(t))
         graph.replay()
         return torch.index_select(gn, 0, idx_dev[1])                # slots -> frames
@@ -313,10 +362,11 @@ class ChunkedDenoiser:
         else:
             patch.update_patch(self.unet, global_tokens=None)               # generate.py:233-236
 
-    def _capture_chunk(self, key, x: torch.Tensor):
+    def _capture_chunk(self, key, x: torch.Tensor, src: Optional[torch.Tensor]):
         """Capture the noise prediction of one chunk shaped like `x`; `key[1]` says whether it is the first chunk of a
         step, i.e. whether the blocks' stores are empty when it runs."""
         gx = x.clone()
+        gsrc = None if src is None else src.to(x).clone()
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
@@ -324,27 +374,33 @@ class ChunkedDenoiser:
             st.filled = not key[1]
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = self.pred_noise(gx, self._chunk_t)
-        self._chunk_graphs[key] = (graph, gx, gn)
+            gn = self.pred_noise(gx, self._chunk_t, gsrc)
+        self._chunk_graphs[key] = (graph, gx, gn, gsrc)
         return self._chunk_graphs[key]
 
-    def _chunk_graph_noises(self, x: torch.Tensor, t: int) -> torch.Tensor:
+    def _chunk_graph_noises(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None) -> torch.Tensor:
         flen = len(x)
         chunks = self.get_chunks(flen)                                      # the same host draws as eager stepping
         if not self._chunk_graphs:
             self._check_chunk_lengths(flen)                                 # before anything is captured
+        inject = self.injecting(t)
+        if not inject and any(k[3] for k in self._chunk_graphs):
+            # the schedule is a prefix of the steps: the injected graphs never run again
+            self._chunk_graphs = {k: v for k, v in self._chunk_graphs.items() if not k[3]}
         if self._chunk_t is None:
             self._chunk_t = torch.tensor(int(t), device=x.device, dtype=torch.long)
         self._chunk_t.fill_(int(t))
         noises = torch.empty_like(x)
         for k, chunk in enumerate(chunks):
             lo, hi = int(chunk[0]), int(chunk[-1]) + 1
-            key = (hi - lo, self.merge_global and k == 0, tuple(x.shape[1:]))
+            key = (hi - lo, self.merge_global and k == 0, tuple(x.shape[1:]), inject)
             entry = self._chunk_graphs.get(key)
             if entry is None:
-                entry = self._capture_chunk(key, x[lo:hi])
-            graph, gx, gn = entry
+                entry = self._capture_chunk(key, x[lo:hi], None if src is None else src[lo:hi])
+            graph, gx, gn, gsrc = entry
             gx.copy_(x[lo:hi])
+            if gsrc is not None:
+                gsrc.copy_(src[lo:hi])
             graph.replay()
             noises[lo:hi].copy_(gn)
         return noises
@@ -353,23 +409,30 @@ class ChunkedDenoiser:
     @torch.no_grad()
     def step(self, x: torch.Tensor, i: int) -> torch.Tensor:
         t = self.timesteps[i]
+        src = None
+        if self.source_latents is not None:                                 # generate.py:226-231 (pre_iter)
+            pnp.register_time(self.unet, t, modules=self._pnp_targets)
+            src = self.source_latents(t)
         if self.chunk_graphs and self.merge_global and x.is_cuda and not self._stores:
             self._install_stores()
         if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.chunk_graphs:
-            noises = self._chunk_graph_noises(x, t)
+            noises = self._chunk_graph_noises(x, t, src)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.capture_global:
-            noises = self._slot_noises(x, t)
+            noises = self._slot_noises(x, t, src)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup:
-            if self._graph is None or self._graph[4] != tuple(x.shape):
-                self._capture(x, t)
+            if self._graph is None or self._graph[4] != self._graph_key(x, t):
+                self._capture(x, t, src)
             graph, gx, gt, gn = self._graph[:4]
+            gsrc = self._graph[5]
             gx.copy_(x, non_blocking=True)
+            if gsrc is not None:
+                gsrc.copy_(src, non_blocking=True)
             gt.fill_(int(t))
             graph.replay()
             noises = gn
         else:
             self._eager_steps += 1
-            noises = self._all_noises(x, t)
+            noises = self._all_noises(x, t, src)
         x = self.pred_next_x(x, noises, i)
         if self.merge_global:
             self._reset_global()

@@ -137,9 +137,9 @@ class SkeletonUNet(ModelMixin):
     def __init__(self, census: List[BlockSpec], in_channels: int = 4, cross_attention_dim: int = 768,
                  hot_path_only: bool = True, max_downsample: Optional[int] = None):
         super().__init__()
-        if max_downsample is not None:
-            census = [s for s in census if s.downsample <= max_downsample]
-        self.census = list(census)
+        keep = [i for i, s in enumerate(census) if max_downsample is None or s.downsample <= max_downsample]
+        self.census_index = keep                  # position of every block in the full census
+        self.census = [census[i] for i in keep]
         self.in_channels = in_channels
         self.blocks = nn.ModuleList(
             [BasicTransformerBlock(s.dim, s.heads, cross_attention_dim, hot_path_only) for s in self.census])
@@ -166,6 +166,18 @@ class SkeletonUNet(ModelMixin):
                 out = F.interpolate(out, scale_factor=ds, mode="nearest")
             eps = eps + out
         return SimpleNamespace(sample=eps)
+
+
+# Census positions of the reference's PnP targets (utils/pnp_utils.py:97, RES_DICT = {1: [1, 2], 2: [0, 1, 2], 3: [0, 1, 2]}):
+# up_blocks[1].attentions[1, 2], up_blocks[2].attentions[0..2] and up_blocks[3].attentions[0..2] are blocks 8 - 15 of
+# the 16-block SD census (down 6, mid 1, up 9).
+PNP_CENSUS_BLOCKS = range(8, 16)
+
+
+def pnp_attention_modules(net: SkeletonUNet) -> List[nn.Module]:
+    """The attn1 modules PnP controls (pnp.register_attention_control(modules=...)) for a skeleton built from the SD
+    census; blocks that max_downsample left out are skipped."""
+    return [b.attn1 for i, b in zip(net.census_index, net.blocks) if i in PNP_CENSUS_BLOCKS]
 
 
 def make_skeleton(name: str = "sd15", hot_path_only: bool = True, max_downsample: Optional[int] = None,
