@@ -234,9 +234,10 @@ def test_c4_full_size_with_global_stage_bit_exact(T, C, Lwant, monkeypatch):
 def test_zero_norm_rows_never_participate_in_matching(monkeypatch):
     """Reference: a zero token row gives NaN after `metric / metric.norm()` (merge.py:84, no epsilon); torch.max /
     argsort then propagate the NaN (App. C.5): a zero DST row makes EVERY src row's maximum NaN and the whole match
-    degenerates.  Waiver (DESIGN.md §6): here a row whose norm is zero or non-finite does not take part in matching —
-    as src it ranks last (stays unmerged while r < Ns), as dst it is never a merge target; every other row is matched
-    exactly as if the row's scores were -inf.  Indices stay in bounds.  This test pins that behaviour bit for bit."""
+    degenerates.  Waiver (DESIGN.md §1): here a zero row, and a row with a non-finite entry, does not take part in
+    matching — as src it ranks last (stays unmerged while r < Ns), as dst it is never a merge target; every other row is
+    matched exactly as if the row's scores were -inf.  Indices stay in bounds.  This test pins that behaviour bit for
+    bit.  A finite row whose fp16 norm overflows is not waived: it normalises to +-0 as in the reference."""
     from vidtome_b200 import merge
     rng = np.random.default_rng(77)
     B, F, T, C = 2, 4, 64, 128
