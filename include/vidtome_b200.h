@@ -145,12 +145,6 @@ int vtm_normalize_split_ln(const void* x_dev, int64_t x_batch_stride, const int3
 int vtm_sim_argmax(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd,
                    int32_t C, int32_t align_batch, uint64_t* keys_out_dev, void* stream);
 
-/* KA built on CTA pairs (clusters of two CTAs: each takes one 128-row src block, loads half of every dst tile and
- * multicasts it to both, so dst tiles leave L2 once per pair).  Same results bit for bit; kept for A/B measurements
- * and tests. */
-int vtm_sim_argmax_pair(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd,
-                        int32_t C, int32_t align_batch, uint64_t* keys_out_dev, void* stream);
-
 /* Debug/verification twin of KA on CUDA cores (one thread per src row, sequential fp32 FMA over K
  * in index order).  Same outputs; used by tests to cross-check KA at sizes the CPU oracle cannot
  * reach.  Not used by the product path. */
@@ -160,8 +154,8 @@ int vtm_sim_argmax_simt(const void* a_dev, const void* b_dev, int32_t B, int32_t
 /* KA with device counts (mode-2 splits): a_dev [B, ns_cap, C] and b_dev [B, nd_cap, C] as vtm_normalize_split writes
  * them for such a split; Ns = counts_dev[0] and Nd = counts_dev[1] are read on the device.  Src rows >= Ns publish
  * nothing and dst columns >= Nd take no part; keys_out_dev is [B', ns_cap] (row stride ns_cap), zeroed first.  The keys
- * of the first Ns rows equal those of vtm_sim_argmax called with the same counts as host values.  Only the default
- * one-CTA build has this path. */
+ * of the first Ns rows equal those of vtm_sim_argmax called with the same counts as host values.  The SIMT twin has
+ * no such path. */
 int vtm_sim_argmax_dev(const void* a_dev, const void* b_dev, int32_t B, int32_t ns_cap, int32_t nd_cap, int32_t C,
                        int32_t align_batch, const int32_t* counts_dev, uint64_t* keys_out_dev, void* stream);
 

@@ -257,7 +257,7 @@ def test_driver_chunk_graphs_full_size(monkeypatch):
 
 
 # --------------------------------------------------------------------------- 5. refusals
-def test_store_refuses_other_merge_and_exchange_modes(monkeypatch):
+def test_store_refuses_other_merge_exchange_and_simt_modes(monkeypatch):
     from vidtome_b200 import merge, ops, patch
     from vidtome_b200._lib import VtmSplit
     L, Lg, cap, C = 40, 30, 48, 64
@@ -269,12 +269,8 @@ def test_store_refuses_other_merge_and_exchange_modes(monkeypatch):
         ops.merge_reduce(cat, sp, 0, m.keys, m.edge, "mean")          # reductions have no device-count path
     with pytest.raises(RuntimeError, match="inconsistent vtm_split_t"):
         ops.compose_maps(sp, 0, m.keys, m.edge, m.rank, None, None, 0, L + cap)
-    monkeypatch.setattr(ops, "KA_VARIANT", "pair")
     a, b = ops.normalize_split(cat, None, sp)
-    with pytest.raises(RuntimeError, match="one-CTA"):
-        ops.sim_argmax(a, b, False, counts=m.counts)
-    monkeypatch.setattr(ops, "KA_VARIANT", "cta")
-    with pytest.raises(RuntimeError, match="one-CTA"):
+    with pytest.raises(RuntimeError, match="SIMT twin"):
         ops.sim_argmax(a, b, False, simt=True, counts=m.counts)
 
     info = {"size": (8, 8), "hooks": [], "args": dict(

@@ -1,7 +1,7 @@
 """KA (similarity + arg-max) at the shapes its tiling makes special: 256-wide dst tiles with every kind of ragged
 last tile, more work items than CTAs (the src block resident in shared memory is reloaded), and channel counts whose
 src block does not fit next to the dst ring (streamed src chunks).  Bit exact against the numpy oracle on
-exact-arithmetic tokens, for the default kernel and its CTA-pair build.  Needs an H100 (sm_90a)."""
+exact-arithmetic tokens.  Needs an H100 (sm_90a)."""
 import numpy as np
 import pytest
 import torch
@@ -22,25 +22,18 @@ def _exact_tokens(rng, shape, nnz=64, val=0.125):
     return x
 
 
-@pytest.fixture(params=["cta", "pair"])
-def ka_variant(request, monkeypatch):
-    from vidtome_b200 import ops
-    monkeypatch.setattr(ops, "KA_VARIANT", request.param)
-    return request.param
-
-
 @pytest.mark.parametrize("B,Ns,Nd,C,align", [
     (2, 300, 868, 320, False),     # Nd % 256 = 100: last dst tile at most half full
     (2, 300, 712, 320, True),      # Nd % 256 = 200: last dst tile more than half full
     (1, 257, 200, 320, False),     # Nd < 256: one partial dst tile
-    (2, 10240, 868, 320, False),   # 160 work items (80 in pairs) for at most 132 CTAs: src blocks are reloaded
+    (2, 10240, 868, 320, False),   # 160 work items for at most 132 CTAs: src blocks are reloaded
     (2, 10240, 712, 320, True),
     (2, 300, 712, 640, False),     # C = 640: src chunks streamed through the ring
     (2, 300, 868, 640, True),
     (2, 260, 868, 1280, False),    # C = 1280: streamed
     (1, 129, 300, 1280, True),
 ])
-def test_sim_argmax_tiles_bit_exact_on_exact_inputs(B, Ns, Nd, C, align, ka_variant):
+def test_sim_argmax_tiles_bit_exact_on_exact_inputs(B, Ns, Nd, C, align):
     from vidtome_b200 import ops
     rng = np.random.default_rng(B * 100003 + Ns * 31 + Nd + C)
     nnz = min(64, C // 2)

@@ -96,7 +96,7 @@ def test_normalize_split_rowmap():
     (2, 515, 5000, 320, False),    # many dst tiles -> split dst sweeps + atomic combine
     (1, 130, 257, 72, False),      # K tail (72 = 64 + 8), 1-row / 1-column tails
 ])
-def test_sim_argmax_bit_exact_on_exact_inputs(B, Ns, Nd, C, align, ka_variant):
+def test_sim_argmax_bit_exact_on_exact_inputs(B, Ns, Nd, C, align):
     ops = _ops()
     rng = np.random.default_rng(B * 1000 + Ns)
     nnz = min(64, C // 2)
@@ -109,17 +109,8 @@ def test_sim_argmax_bit_exact_on_exact_inputs(B, Ns, Nd, C, align, ka_variant):
     np.testing.assert_array_equal(arg.cpu().numpy(), idx)
 
 
-@pytest.fixture(params=["cta", "cta_pair"])
-def ka_variant(request, monkeypatch):
-    """KA's default kernel and its CTA-pair build (2-CTA cluster sharing every dst tile by TMA multicast;
-    vtm_sim_argmax / vtm_sim_argmax_pair)."""
-    from vidtome_b200 import ops
-    monkeypatch.setattr(ops, "KA_VARIANT", "pair" if request.param == "cta_pair" else "cta")
-    return request.param
-
-
 @pytest.mark.parametrize("align", [False, True])
-def test_sim_argmax_equal_maxima_across_dst_ranges(align, ka_variant):
+def test_sim_argmax_equal_maxima_across_dst_ranges(align):
     """The epilogue filters on the maximum other dst ranges have already published.  Every dst row here occurs
     many times across the whole sweep (and in both samples), so the winning score is tied across work items that
     run in arbitrary order: the smallest dst index must still win, bit for bit."""
@@ -139,7 +130,7 @@ def test_sim_argmax_equal_maxima_across_dst_ranges(align, ka_variant):
     np.testing.assert_array_equal(arg.cpu().numpy(), idx)
 
 
-def test_sim_argmax_nonpositive_and_zero_scores(ka_variant):
+def test_sim_argmax_nonpositive_and_zero_scores():
     """Rows whose best score is negative, +0 or -0 (threshold stepping around zero, merge.py:112 semantics)."""
     ops = _ops()
     rng = np.random.default_rng(12)
@@ -157,20 +148,6 @@ def test_sim_argmax_nonpositive_and_zero_scores(ka_variant):
         score, arg = ops.keys_to_score_arg(keys)
         assert np.array_equal(score.cpu().numpy().astype(np.float32), mx.astype(np.float32))     # -0 == +0
         np.testing.assert_array_equal(arg.cpu().numpy(), idx)
-
-
-def test_sim_argmax_cta_pair_equals_default(monkeypatch):
-    ops = _ops()
-    g = torch.Generator(device="cuda").manual_seed(5)
-    for (B, Ns, Nd, C, align) in [(2, 3072, 1024, 320, False), (2, 1000, 5000, 640, True), (3, 129, 257, 1280, False),
-                                  (1, 77, 33, 64, False)]:
-        a = torch.randn((B, Ns, C), generator=g, device="cuda").half()
-        b = torch.randn((B, Nd, C), generator=g, device="cuda").half()
-        monkeypatch.setattr(ops, "KA_VARIANT", "cta")
-        k1 = ops.sim_argmax(a, b, align)
-        monkeypatch.setattr(ops, "KA_VARIANT", "pair")
-        k2 = ops.sim_argmax(a, b, align)
-        assert torch.equal(k1, k2)
 
 
 @pytest.mark.parametrize("align", [False, True])

@@ -3,8 +3,8 @@
 Prints one JSON line per (kernel, shape): CUDA-event time (median of `--iters` after warm-up, L2 flushed
 between iterations by writing a 256 MiB buffer), achieved TFLOP/s or GB/s and the fraction of the measured
 peak in MEASURED_PEAKS.json (else the H100 SXM data-sheet figures).  `--quick` runs only the BASELINE config-2 shapes;
-`--ka-only` only the KA (similarity + arg-max) shapes, `--ka-variant pair` with KA's CTA-pair build; `--kd-only` only
-the two KD (merged-token self-attention) shapes.
+`--ka-only` only the KA (similarity + arg-max) shapes; `--kd-only` only the two KD (merged-token self-attention)
+shapes.
 
 The KA line also gives `l2_fill_MB`: the operand bytes the kernel's tiling loads into shared memory (computed from the
 shapes, the tile sizes and the work split of csrc/sim_argmax.cu), and `l2_fill_TBs`, those bytes over the kernel time.
@@ -88,23 +88,21 @@ def time_rotating_ms(fns, reps=12, warmup=3):
     return ts[len(ts) // 2]
 
 
-def ka_l2_fill_bytes(B, Ns, Nd, C, pair, sms):
+def ka_l2_fill_bytes(B, Ns, Nd, C, sms):
     """Operand bytes KA moves from L2 (or HBM) into shared memory, mirroring ka::Items / ka::Layout in sim_argmax.cu:
     128 x 256 tiles, 64-column K chunks, the src block loaded once per work item when it fits in shared memory next to
-    three 256 x 64 dst stages (else once per tile), each dst tile once per CTA (once per pair in the pair build)."""
+    three 256 x 64 dst stages (else once per tile), each dst tile once per CTA."""
     BM, BN, BK, target = 128, 256, 64, 8
     kp = -(-C // BK) * BK
     m_tiles, n_tiles = -(-Ns // BM), -(-Nd // BN)
-    units = (m_tiles + 1) // 2 if pair else m_tiles
     resident = kp // BK <= 8 and 1024 + 224 + BM * kp * 2 + 3 * BN * BK * 2 <= 227 * 1024
     s = 1
-    while units * B * s < target * (sms // 2 if pair else sms) and s * 2 <= n_tiles:
+    while m_tiles * B * s < target * sms and s * 2 <= n_tiles:
         s *= 2
     tps = -(-n_tiles // s)
     n_splits = -(-n_tiles // tps)
-    blocks = 2 * units if pair else m_tiles
-    a_loads = blocks * B * (n_splits if resident else n_tiles)
-    return 2.0 * kp * (a_loads * BM + units * B * n_tiles * BN)
+    a_loads = m_tiles * B * (n_splits if resident else n_tiles)
+    return 2.0 * kp * (a_loads * BM + m_tiles * B * n_tiles * BN)
 
 
 def bench_sim_argmax(B, Ns, Nd, C, align, iters):
@@ -115,9 +113,8 @@ def bench_sim_argmax(B, Ns, Nd, C, align, iters):
     med, best = time_ms(lambda: ops.sim_argmax(a, b, align), iters)
     flops = 2.0 * B * Ns * Nd * C
     byts = 2.0 * B * (Ns + Nd) * C + 8.0 * (1 if align else B) * Ns
-    fill = ka_l2_fill_bytes(B, Ns, Nd, C, ops.KA_VARIANT == "pair",
-                            torch.cuda.get_device_properties(0).multi_processor_count)
-    print(json.dumps({"kernel": "KA sim_argmax", "variant": ops.KA_VARIANT, "B": B, "Ns": Ns, "Nd": Nd, "C": C,
+    fill = ka_l2_fill_bytes(B, Ns, Nd, C, torch.cuda.get_device_properties(0).multi_processor_count)
+    print(json.dumps({"kernel": "KA sim_argmax", "B": B, "Ns": Ns, "Nd": Nd, "C": C,
                       "align": align, "ms": round(med, 4), "ms_best": round(best, 4),
                       "tflops": round(flops / med / 1e9, 1), "frac_tensor_peak": round(flops / med / 1e9 / tf, 3),
                       "eff_GBs": round(byts / med / 1e6, 1), "l2_fill_MB": round(fill / 1e6, 1),
@@ -230,11 +227,9 @@ def main():
     ap.add_argument("--quick", action="store_true")
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--ka-only", action="store_true")
-    ap.add_argument("--ka-variant", default="cta", choices=["cta", "pair"])
     ap.add_argument("--kd-only", action="store_true")
     args = ap.parse_args()
     torch.cuda.init()
-    ops.KA_VARIANT = args.ka_variant
     if args.kd_only:
         from vidtome_b200._lib import LIB_PATH
         print(json.dumps({"device": torch.cuda.get_device_name(0), "lib": LIB_PATH}), flush=True)

@@ -97,7 +97,6 @@ SIGNATURES = {
     "vtm_gather_rows_peers": (C.c_int, [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _vp, C.c_float, _vp, _i64,
                                         C.POINTER(C.c_void_p), _i32, _vp]),
     "vtm_sim_argmax": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
-    "vtm_sim_argmax_pair": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "vtm_sim_argmax_simt": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "vtm_key_score_half_bits": (C.c_uint16, [C.c_uint64]),
     "vtm_key_arg": (C.c_uint32, [C.c_uint64]),

@@ -203,19 +203,4 @@ inline int make_tmap_3d_f16(CUtensorMap* m, const void* base, uint64_t d0, uint6
   return r == CUDA_SUCCESS ? VTM_OK : 100000 + static_cast<int>(r);
 }
 
-// fp16 tensor of rank 4 with arbitrary (16-byte multiple) strides given in elements; box {b0, b1, 1, 1}.
-inline int make_tmap_4d_f16(CUtensorMap* m, const void* base, const uint64_t dims[4], const uint64_t strides_el[3],
-                            uint32_t b0, uint32_t b1) {
-  PFN_tmapEncodeTiled enc = get_tmap_encode();
-  if (!enc) return VTM_E_DRIVER;
-  cuuint64_t d[4] = {dims[0], dims[1], dims[2], dims[3]};
-  cuuint64_t st[3] = {strides_el[0] * 2, strides_el[1] * 2, strides_el[2] * 2};
-  cuuint32_t box[4] = {b0, b1, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), d, st, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? VTM_OK : 100000 + static_cast<int>(r);
-}
-
 }  // namespace vtm

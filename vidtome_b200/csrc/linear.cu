@@ -43,10 +43,8 @@ struct StoreEpi {
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const float2 bf = __half22float2(b2[e]);
-            float a, b;
-            f32x2_unpack(f32x2_add(f32x2_pack(__uint_as_float(r[8 * v8 + 2 * e]), __uint_as_float(r[8 * v8 + 2 * e + 1])),
-                                   f32x2_pack(bf.x, bf.y)), a, b);
-            pk[4 * v8 + e] = pack_f16x2(a, b);
+            pk[4 * v8 + e] = pack_f16x2(__fadd_rn(__uint_as_float(r[8 * v8 + 2 * e]), bf.x),
+                                        __fadd_rn(__uint_as_float(r[8 * v8 + 2 * e + 1]), bf.y));
           }
         }
       } else {
@@ -111,18 +109,22 @@ struct StoreEpi {
 // g h rounds to -0 in fp16 as gelu does, and ex2 flushes h to 0 once p < -126.  Holding h at its value at a clamp instead
 // would let g h grow with |g|.  Then gelu(g) = g (1 - h) for g >= 0 and g h for g < 0: over every finite fp16 gate the
 // fp16 result is within one ulp of the correctly rounded gelu, and zero wherever that is (+0 at g = -0).  Two values at
-// a time.
+// a time, their Horner steps interleaved.
 __device__ __forceinline__ void gelu_x2(float g0, float g1, float& y0, float& y1) {
-  const uint64_t t2 = f32x2_pack(fabsf(g0), fabsf(g1));
-  uint64_t p2 = f32x2_fma(f32x2_pack(-1.79155074e-06f, -1.79155074e-06f), t2, f32x2_pack(6.06881658e-05f, 6.06881658e-05f));
-  p2 = f32x2_fma(p2, t2, f32x2_pack(-0.000922937703f, -0.000922937703f));
-  p2 = f32x2_fma(p2, t2, f32x2_pack(0.00847607013f, 0.00847607013f));
-  p2 = f32x2_fma(p2, t2, f32x2_pack(-0.0538897403f, -0.0538897403f));
-  p2 = f32x2_fma(p2, t2, f32x2_pack(-0.458542407f, -0.458542407f));
-  p2 = f32x2_fma(p2, t2, f32x2_pack(-1.15121424f, -1.15121424f));
-  p2 = f32x2_fma(p2, t2, f32x2_pack(-1.f, -1.f));                      // p(t) - 1
-  float p0, p1;
-  f32x2_unpack(p2, p0, p1);
+  const float t0 = fabsf(g0), t1 = fabsf(g1);
+  const float lead = -1.79155074e-06f;
+  float p0 = lead, p1 = lead;
+  auto horner = [&](float c) {                    // p = p t + c
+    p0 = __fmaf_rn(p0, t0, c);
+    p1 = __fmaf_rn(p1, t1, c);
+  };
+  horner(6.06881658e-05f);
+  horner(-0.000922937703f);
+  horner(0.00847607013f);
+  horner(-0.0538897403f);
+  horner(-0.458542407f);
+  horner(-1.15121424f);
+  horner(-1.f);                                   // p(t) - 1
   const float h0 = ex2_approx(p0), h1 = ex2_approx(p1);                 // erfc(t / sqrt 2) / 2
   const float gh0 = g0 * h0, gh1 = g1 * h1;
   y0 = g0 >= 0.f ? g0 - gh0 : gh0;
@@ -170,11 +172,9 @@ struct GegluEpi {
             // fp16 roundings of the unfused pipeline: projection output, gelu output, product.  The product of the two
             // fp16 values is taken by HMUL2 (the fp32 product of two fp16 numbers is exact, so one rounding to fp16
             // either way).
-            float a0, a1, g0, g1;
-            f32x2_unpack(f32x2_add(f32x2_pack(__uint_as_float(r[i]), __uint_as_float(r[i + 1])), f32x2_pack(fa.x, fa.y)), a0, a1);
-            f32x2_unpack(f32x2_add(f32x2_pack(__uint_as_float(r[32 + i]), __uint_as_float(r[32 + i + 1])), f32x2_pack(fg.x, fg.y)), g0, g1);
-            const uint32_t a16 = pack_f16x2(a0, a1);
-            const uint32_t g16 = pack_f16x2(g0, g1);
+            const uint32_t a16 = pack_f16x2(__fadd_rn(__uint_as_float(r[i]), fa.x), __fadd_rn(__uint_as_float(r[i + 1]), fa.y));
+            const uint32_t g16 = pack_f16x2(__fadd_rn(__uint_as_float(r[32 + i]), fg.x),
+                                            __fadd_rn(__uint_as_float(r[32 + i + 1]), fg.y));
             const float2 gf = __half22float2(*reinterpret_cast<const __half2*>(&g16));
             float q0, q1;
             gelu_x2(gf.x, gf.y, q0, q1);

@@ -12,24 +12,10 @@ namespace vtm {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
-
 __device__ __forceinline__ uint64_t globaltimer_ns() {
   uint64_t t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
-}
-
-// One elected lane of a fully converged warp (the warp stays converged, so address/descriptor arithmetic
-// around single-thread instructions can live on the uniform datapath).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ---------------------------------------------------------------- mbarrier
@@ -38,9 +24,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -82,64 +65,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
       " [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-// ---------------------------------------------------------------- clusters (CTA pairs)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_id_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_count_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-  return r;
-}
-// every thread of every CTA of the cluster
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-}
-// shared::cluster address of `smem_addr` in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-// arrive on an mbarrier of another CTA of the cluster (release: this thread's prior reads of shared memory are done)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait whose acquire covers arrivals from the other CTAs of the cluster (bounded like mbar_wait)
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  const uint64_t t0 = globaltimer_ns();
-  uint32_t spins = 0;
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if ((++spins & 0x3FFu) == 0 && globaltimer_ns() - t0 > 4000000000ull) __trap();
-  }
-}
-// TMA load delivered to the same shared-memory offset in every CTA of `cta_mask`, each signalling its own mbarrier at
-// offset `bar`
-__device__ __forceinline__ void tma_load_3d_multicast(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar,
-                                                      int32_t c0, int32_t c1, int32_t c2, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4, %5}], [%2], %6;"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
       : "memory");
 }
 
@@ -382,40 +307,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-// ---------------------------------------------------------------- fp32 pairs
-// Two fp32 values in one 64-bit register pair {lo, hi}; the arithmetic is per lane with round-to-nearest (sm_90 has no
-// packed fp32 instructions), so every result equals the scalar fmaf / __fadd_rn / __fmul_rn / __fsub_rn of its lane.
-__device__ __forceinline__ uint64_t f32x2_pack(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void f32x2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f32x2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  float a0, a1, b0, b1, c0, c1;
-  f32x2_unpack(a, a0, a1); f32x2_unpack(b, b0, b1); f32x2_unpack(c, c0, c1);
-  return f32x2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
-__device__ __forceinline__ uint64_t f32x2_add(uint64_t a, uint64_t b) {
-  float a0, a1, b0, b1;
-  f32x2_unpack(a, a0, a1); f32x2_unpack(b, b0, b1);
-  return f32x2_pack(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
-}
-__device__ __forceinline__ uint64_t f32x2_mul(uint64_t a, uint64_t b) {
-  float a0, a1, b0, b1;
-  f32x2_unpack(a, a0, a1); f32x2_unpack(b, b0, b1);
-  return f32x2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
-}
-
 // ---------------------------------------------------------------- misc
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // Order-preserving 16-bit image of a (non-NaN) fp16 bit pattern; -0 is canonicalised to +0 so that
 // equal values always compare equal (IEEE: -0 == +0, as torch.max sees them).
 __host__ __device__ __forceinline__ uint32_t half_bits_to_ordered(uint32_t h) {

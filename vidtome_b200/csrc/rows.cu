@@ -25,7 +25,6 @@ __device__ __forceinline__ uint4 ld_nc_16(const void* p) {
                : "l"(p));
   return r;
 }
-__device__ __forceinline__ uint4 ld_16(const void* p) { return *reinterpret_cast<const uint4*>(p); }
 __device__ __forceinline__ void st_16(void* p, const uint4& v) {
   asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y),
                "r"(v.z), "r"(v.w)
@@ -47,10 +46,9 @@ struct LnParams {
 
 // In-register LayerNorm of one row held as P vectors per lane by a G-lane group (torch half semantics: fp32
 // statistics, y = gamma * (rstd * (x - mean)) + beta in fp32, rounded to fp16).  The kernels that fuse it are bound by
-// instruction issue, not by HBM (r01: 0.45-0.49 of the copy bandwidth; a first r02 attempt with fewer rows per warp was
-// slower still: 0.42), so the row is converted to fp32 ONCE, kept in registers as packed pairs through both statistics
-// passes and the affine step, all arithmetic is packed (f32x2), and gamma / beta are read as fp32 from shared memory
-// (staged once per CTA by stage_ln_params) instead of two 16-byte global loads + 16 conversions per data vector.
+// instruction issue, not by HBM, so the row is converted to fp32 ONCE and kept in registers through both statistics
+// passes and the affine step, and gamma / beta are read as fp32 from shared memory (staged once per CTA by
+// stage_ln_params) instead of two 16-byte global loads + 16 conversions per data vector.
 constexpr int LN_MAX_C = 2048;
 __device__ __forceinline__ void stage_ln_params(const LnParams& ln, int C, float* s_gamma, float* s_beta) {
   for (int i = threadIdx.x; i < C; i += blockDim.x) {
@@ -59,65 +57,57 @@ __device__ __forceinline__ void stage_ln_params(const LnParams& ln, int C, float
   }
   __syncthreads();
 }
-__device__ __forceinline__ float f32x2_hsum(uint64_t a) {
-  float lo, hi;
-  f32x2_unpack(a, lo, hi);
-  return lo + hi;
-}
-// fp16x2 -> packed fp32 pair
-__device__ __forceinline__ uint64_t h2_to_f32x2(__half2 h) {
-  const float2 t = __half22float2(h);
-  return f32x2_pack(t.x, t.y);
-}
-__device__ __forceinline__ __half2 f32x2_to_h2(uint64_t a) {
-  float lo, hi;
-  f32x2_unpack(a, lo, hi);
-  return __floats2half2_rn(lo, hi);
-}
-// All arithmetic on PACKED fp32 pairs (add / mul / fma .f32x2: the same IEEE operations per lane at half the issue
-// slots, tools/ubench/fma2_pipe.cu).  The row lives in registers as P x 4 pairs.
+// Sum of two pairs of partial sums (x, y): the lanes first, then the two lane totals.
+__device__ __forceinline__ float pair_sum(float2 a, float2 b) { return __fadd_rn(a.x, b.x) + __fadd_rn(a.y, b.y); }
+// The row lives in registers as P x 4 fp32 pairs, one per fp16 pair of a vector.
 // FULL: the row is exactly G x P vectors wide (C = 320 / 640 / 1280 with G = 8 / 16 / 32, P = 5), so the per-vector range
 // tests — a divergence scaffold of BSSY / BSYNC / BRA around every vector in SASS — are compiled out.
 template <int G, int P, bool FULL = false>
 __device__ __forceinline__ void layer_norm_row(uint4 (&v)[P], int sub, int vecs, int C, float eps,
                                                const float* __restrict__ s_gamma, const float* __restrict__ s_beta) {
-  uint64_t f[P][4];
-  uint64_t acc0 = 0, acc1 = 0;                         // (0.f, 0.f)
+  float2 f[P][4];
+  float2 acc[2] = {{0.f, 0.f}, {0.f, 0.f}};
 #pragma unroll
   for (int i = 0; i < P; ++i) {
     const __half2* h = reinterpret_cast<const __half2*>(&v[i]);   // vectors beyond the row were loaded as zeros
 #pragma unroll
-    for (int e = 0; e < 4; ++e) f[i][e] = h2_to_f32x2(h[e]);
-    acc0 = f32x2_add(acc0, f32x2_add(f[i][0], f[i][1]));
-    acc1 = f32x2_add(acc1, f32x2_add(f[i][2], f[i][3]));
+    for (int e = 0; e < 4; ++e) f[i][e] = __half22float2(h[e]);
+#pragma unroll
+    for (int e = 0; e < 4; e += 2) {
+      acc[e / 2].x = __fadd_rn(acc[e / 2].x, __fadd_rn(f[i][e].x, f[i][e + 1].x));
+      acc[e / 2].y = __fadd_rn(acc[e / 2].y, __fadd_rn(f[i][e].y, f[i][e + 1].y));
+    }
   }
-  const float mean = group_sum<G>(f32x2_hsum(f32x2_add(acc0, acc1))) / static_cast<float>(C);
-  const uint64_t nm2 = f32x2_pack(-mean, -mean);
-  uint64_t q0 = 0, q1 = 0;
+  const float mean = group_sum<G>(pair_sum(acc[0], acc[1])) / static_cast<float>(C);
+  float2 q[2] = {{0.f, 0.f}, {0.f, 0.f}};
 #pragma unroll
   for (int i = 0; i < P; ++i) {
     if (FULL || sub + G * i < vecs) {
 #pragma unroll
-      for (int e = 0; e < 4; ++e) f[i][e] = f32x2_add(f[i][e], nm2);
-      q0 = f32x2_fma(f[i][0], f[i][0], q0);
-      q1 = f32x2_fma(f[i][1], f[i][1], q1);
-      q0 = f32x2_fma(f[i][2], f[i][2], q0);
-      q1 = f32x2_fma(f[i][3], f[i][3], q1);
+      for (int e = 0; e < 4; ++e) {
+        f[i][e].x = __fadd_rn(f[i][e].x, -mean);
+        f[i][e].y = __fadd_rn(f[i][e].y, -mean);
+      }
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        q[e & 1].x = __fmaf_rn(f[i][e].x, f[i][e].x, q[e & 1].x);
+        q[e & 1].y = __fmaf_rn(f[i][e].y, f[i][e].y, q[e & 1].y);
+      }
     }
   }
-  const float rstd = rsqrtf(group_sum<G>(f32x2_hsum(f32x2_add(q0, q1))) / static_cast<float>(C) + eps);
-  const uint64_t r2 = f32x2_pack(rstd, rstd);
+  const float rstd = rsqrtf(group_sum<G>(pair_sum(q[0], q[1])) / static_cast<float>(C) + eps);
+  auto affine = [&](float x, float g, float b) { return __fmaf_rn(g, __fmul_rn(rstd, x), b); };
 #pragma unroll
   for (int i = 0; i < P; ++i) {
     const int vi = sub + G * i;
     if (FULL || vi < vecs) {
-      const ulonglong2 g0 = *reinterpret_cast<const ulonglong2*>(s_gamma + vi * 8), g1 = *reinterpret_cast<const ulonglong2*>(s_gamma + vi * 8 + 4);
-      const ulonglong2 b0 = *reinterpret_cast<const ulonglong2*>(s_beta + vi * 8), b1 = *reinterpret_cast<const ulonglong2*>(s_beta + vi * 8 + 4);
+      const float4 g0 = *reinterpret_cast<const float4*>(s_gamma + vi * 8), g1 = *reinterpret_cast<const float4*>(s_gamma + vi * 8 + 4);
+      const float4 b0 = *reinterpret_cast<const float4*>(s_beta + vi * 8), b1 = *reinterpret_cast<const float4*>(s_beta + vi * 8 + 4);
       __half2* h = reinterpret_cast<__half2*>(&v[i]);
-      h[0] = f32x2_to_h2(f32x2_fma(g0.x, f32x2_mul(r2, f[i][0]), b0.x));
-      h[1] = f32x2_to_h2(f32x2_fma(g0.y, f32x2_mul(r2, f[i][1]), b0.y));
-      h[2] = f32x2_to_h2(f32x2_fma(g1.x, f32x2_mul(r2, f[i][2]), b1.x));
-      h[3] = f32x2_to_h2(f32x2_fma(g1.y, f32x2_mul(r2, f[i][3]), b1.y));
+      h[0] = __floats2half2_rn(affine(f[i][0].x, g0.x, b0.x), affine(f[i][0].y, g0.y, b0.y));
+      h[1] = __floats2half2_rn(affine(f[i][1].x, g0.z, b0.z), affine(f[i][1].y, g0.w, b0.w));
+      h[2] = __floats2half2_rn(affine(f[i][2].x, g1.x, b1.x), affine(f[i][2].y, g1.y, b1.y));
+      h[3] = __floats2half2_rn(affine(f[i][3].x, g1.z, b1.z), affine(f[i][3].y, g1.w, b1.w));
     }
   }
 }
@@ -129,12 +119,9 @@ __device__ __forceinline__ void layer_norm_row(uint4 (&v)[P], int sub, int vecs,
 // K0 is bound by instruction issue, not by HBM (ncu: 866 warp instructions per two rows of 640 values, issue slots 54 %,
 // DRAM 19 %): FULL (see layer_norm_row) removes the per-vector range tests and the two division variants run as separate
 // loops instead of a test per value pair.
-#ifndef VTM_K0_PREFETCH
-#define VTM_K0_PREFETCH 0
-#endif
 // DC: device-count (mode 2) split, src / dst rows at the capacity's row stride (vtm_split_t mode 2)
 template <int G, int P, bool LN, bool FULL = false, bool DC = false>
-__global__ void __launch_bounds__(ROW_THREADS, VTM_K0_PREFETCH ? (LN ? 2 : 3) : (LN ? 3 : 4))
+__global__ void __launch_bounds__(ROW_THREADS, LN ? 3 : 4)
 normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* __restrict__ rowmap,
                        long long map_bs, Split sp, int B, int C, LnParams ln, __half* __restrict__ a_out,
                        __half* __restrict__ b_out) {
@@ -179,44 +166,26 @@ normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* 
       if (live && (FULL || sub + G * i < vecs)) w[i] = ld_nc_16(src + (sub + G * i) * 8);
     }
   };
-#if VTM_K0_PREFETCH
-  // The rows of the NEXT iteration are requested before the current ones are reduced: one warp iteration is a serial chain
-  // (load -> three shuffle reductions -> division -> store) and with six warps per scheduler the loads are exposed.
-  const __half* src_n;
-  __half* dst_n;
-  uint4 v[P], vn[P];
-  long long o0 = warp_id * RPW;
-  bool live_n = locate(o0, src_n, dst_n);
-  load_row(vn, src_n, live_n);
-  for (; o0 < total; o0 += n_warps * RPW) {
-    const bool live = live_n;
-    __half* dst = dst_n;
-#pragma unroll
-    for (int i = 0; i < P; ++i) v[i] = vn[i];
-    live_n = locate(o0 + n_warps * RPW, src_n, dst_n);
-    load_row(vn, src_n, live_n);
-#else
   for (long long o0 = warp_id * RPW; o0 < total; o0 += n_warps * RPW) {
     const __half* src;
     __half* dst;
     const bool live = locate(o0, src, dst);
     uint4 v[P];
     load_row(v, src, live);
-#endif
     if (LN) layer_norm_row<G, P, FULL>(v, sub, vecs, C, ln.eps, s_gamma, s_beta);
-    uint64_t ss0 = 0, ss1 = 0;
+    float2 ss[2] = {{0.f, 0.f}, {0.f, 0.f}};
 #pragma unroll
     for (int i = 0; i < P; ++i) {
       const __half2* h = reinterpret_cast<const __half2*>(&v[i]);
 #pragma unroll
-      for (int e = 0; e < 4; e += 2) {
-        const uint64_t a = h2_to_f32x2(h[e]), c = h2_to_f32x2(h[e + 1]);
-        ss0 = f32x2_fma(a, a, ss0);
-        ss1 = f32x2_fma(c, c, ss1);
+      for (int e = 0; e < 4; ++e) {
+        const float2 a = __half22float2(h[e]);
+        ss[e & 1].x = __fmaf_rn(a.x, a.x, ss[e & 1].x);
+        ss[e & 1].y = __fmaf_rn(a.y, a.y, ss[e & 1].y);
       }
     }
-    const float ss = group_sum<G>(f32x2_hsum(f32x2_add(ss0, ss1)));
-    const float nrm = __half2float(__float2half_rn(sqrtf(ss)));
+    const float ss_row = group_sum<G>(pair_sum(ss[0], ss[1]));
+    const float nrm = __half2float(__float2half_rn(sqrtf(ss_row)));
     // x / nrm, correctly rounded, with ONE IEEE division per row: r = RN(1/nrm), q0 = RN(x r),
     // rem = x - q0 nrm (exact, FMA), q = RN(q0 + rem r) is RN(x / nrm) (Markstein) — checked exhaustively over
     // all fp16 numerators x 3000 fp16 norms in tests/test_host_cpu.py.  Only finite normal norms take it: sub-normal
@@ -225,7 +194,10 @@ normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* 
     // (nrm >= +0; NaN fails it too), as cheap as the single bound it replaced.
     const bool fast = __float_as_uint(nrm) - 0x38800000u <= 0x477FE000u - 0x38800000u;
     const float rinv = 1.0f / nrm;
-    const uint64_t rinv2 = f32x2_pack(rinv, rinv), nnrm2 = f32x2_pack(-nrm, -nrm);
+    auto div = [&](float x) {
+      const float q0 = __fmul_rn(x, rinv);
+      return __fmaf_rn(__fmaf_rn(q0, -nrm, x), rinv, q0);
+    };
     if (fast) {
 #pragma unroll
       for (int i = 0; i < P; ++i) {
@@ -233,9 +205,8 @@ normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* 
           __half2* h = reinterpret_cast<__half2*>(&v[i]);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            const uint64_t f2 = h2_to_f32x2(h[e]);
-            const uint64_t q0 = f32x2_mul(f2, rinv2);
-            h[e] = f32x2_to_h2(f32x2_fma(f32x2_fma(q0, nnrm2, f2), rinv2, q0));
+            const float2 x = __half22float2(h[e]);
+            h[e] = __floats2half2_rn(div(x.x), div(x.y));
           }
           st_16(dst + (sub + G * i) * 8, v[i]);
         }
@@ -374,8 +345,6 @@ int grid_for_rows(K kernel, long long rows, int rows_per_warp, int sms) {
   else if ((vecs) <= 16 * 5) { CALL(16, 5) }        \
   else if ((vecs) <= 32 * 5) { CALL(32, 5) }        \
   else { CALL(32, 8) }
-// with the LayerNorm fused a lane also keeps its part of the row as packed fp32 (about 80 registers: 3 CTAs per SM)
-#define VTM_DISPATCH_GP_LN(vecs, CALL) VTM_DISPATCH_GP(vecs, CALL)
 
 }  // namespace
 }  // namespace vtm
@@ -415,7 +384,7 @@ extern "C" int vtm_normalize_split_ln(const void* x_dev, int64_t x_batch_stride,
   else { CALL_K0_(G, P, LN, false, false) }
   if (ln.w) {
 #define CALL(G, P) CALL_K0(G, P, true)
-    VTM_DISPATCH_GP_LN(vecs, CALL)
+    VTM_DISPATCH_GP(vecs, CALL)
 #undef CALL
   } else {
 #define CALL(G, P) CALL_K0(G, P, false)
@@ -463,7 +432,7 @@ extern "C" int vtm_gather_rows_peers(const void* x_dev, int64_t x_batch_stride, 
           static_cast<__half*>(y_dev), y_batch_stride, peers);
   if (ln.w) {
 #define CALL(G, P) CALL_KC(G, P, true)
-    VTM_DISPATCH_GP_LN(vecs, CALL)
+    VTM_DISPATCH_GP(vecs, CALL)
 #undef CALL
   } else {
 #define CALL(G, P) CALL_KC(G, P, false)

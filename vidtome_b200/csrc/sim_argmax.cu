@@ -19,10 +19,6 @@
 // running ahead across work items.  Per dst tile only the dst bytes come from L2: 128 FLOP per byte instead of 64 for
 // a ring that carries both operands.
 // Streaming-A form (larger C): every ring stage carries the src chunk too, as in a plain GEMM mainloop.
-//
-// CTA-pair build (PAIR, clusters of two): the two CTAs of a cluster take the two src blocks of one work item (m unit =
-// 2 blocks) and sweep the same dst tiles; each loads HALF of every dst tile and multicasts it to both, so every dst
-// byte leaves L2 once per pair.  A ring stage may be refilled only when the consumers of BOTH CTAs are done with it.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -69,19 +65,16 @@ struct Layout {
   __host__ size_t smem_bytes() const { return FIXED + a_bytes + static_cast<size_t>(stages) * stage_bytes; }
 };
 
-// Work item = (m unit, b, [nt0, nt1)), m unit fastest: the dst ranges of one src block run far apart in time, so a
-// later range starts from the maxima the earlier ones published.
+// Work item = (src block, b, [nt0, nt1)), src block fastest: the dst ranges of one src block run far apart in time, so
+// a later range starts from the maxima the earlier ones published.
 struct Items {
   int batches;
-  int m_tiles, m_tiles_real;   // m units (pairs of src blocks in the CTA-pair build) / src blocks of the problem
-  int n_tiles, tiles_per_split, n_splits;
+  int m_tiles, n_tiles, tiles_per_split, n_splits;
   int k_chunks;
   int total;
-  __host__ void plan(int M, int N, int K, int B, int sms, int target_items_per_sm, bool pair) {
+  __host__ void plan(int M, int N, int K, int B, int sms, int target_items_per_sm) {
     batches = B;
-    m_tiles_real = (M + BM - 1) / BM;
-    m_tiles = pair ? (m_tiles_real + 1) / 2 : m_tiles_real;
-    if (pair) sms /= 2;   // work items are shared by the two CTAs of a cluster
+    m_tiles = (M + BM - 1) / BM;
     n_tiles = (N + BN - 1) / BN;
     k_chunks = (K + BK - 1) / BK;
     const long long base = static_cast<long long>(m_tiles) * B;
@@ -212,7 +205,6 @@ __device__ __forceinline__ void tile_argmax(const float (&d)[128], RowBest (&rb)
   }
 }
 
-template <bool PAIR>
 __global__ void __launch_bounds__(THREADS, 1)
 sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const Items wk, const Layout lay, const Args p_in) {
@@ -242,28 +234,26 @@ sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = warp >> 2;
-  // work-item stride: CTAs, or clusters of two in the pair build
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const int w_first = PAIR ? static_cast<int>(cluster_id_x()) : static_cast<int>(blockIdx.x);
-  const int w_step = PAIR ? static_cast<int>(cluster_count_x()) : static_cast<int>(gridDim.x);
+  // this CTA's work items: w_first, w_first + w_step, ...
+  const int w_first = static_cast<int>(blockIdx.x);
+  const int w_step = static_cast<int>(gridDim.x);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), PAIR ? 2 * CONSUMER_WARPS : CONSUMER_WARPS);
+      mbar_init(empty_bar(s), CONSUMER_WARPS);
     }
     if (resident) {
       for (int kc = 0; kc < wk.k_chunks; ++kc) {
         mbar_init(a_full_bar(kc), 1);
-        mbar_init(a_empty_bar(kc), CONSUMER_WARPS);   // the src block is this CTA's own: local consumers only
+        mbar_init(a_empty_bar(kc), CONSUMER_WARPS);
       }
     }
     fence_mbar_init();
   }
-  if constexpr (PAIR) cluster_sync_all();   // the peer's barriers are initialised before anything signals them
-  else __syncthreads();
+  __syncthreads();
 
   if (wg == 0) {
     // ===================== TMA producer =====================
@@ -271,17 +261,12 @@ sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0, a_phase = 0;
-      const uint32_t stage_tx = lay.stage_bytes;   // own src chunk (streaming) + both halves of the dst chunk
+      const uint32_t stage_tx = lay.stage_bytes;   // src chunk (streaming) + dst chunk
       for (int w = w_first; w < wk.total; w += w_step) {
         int m_tile, b, nt0, nt1;
         wk.decode(w, &m_tile, &b, &nt0, &nt1);
         if (nt1 > nt_end) nt1 = nt_end;
         if (nt0 >= nt1 || m_tile * BM >= p.Ns) continue;
-        if (PAIR) {
-          m_tile = 2 * m_tile + static_cast<int>(rank);
-          // the second block of an odd last pair lies past M: load a real block (its rows are never published)
-          if (m_tile >= wk.m_tiles_real) m_tile = wk.m_tiles_real - 1;
-        }
         for (int nt = nt0; nt < nt1; ++nt) {
           for (int kc = 0; kc < wk.k_chunks; ++kc) {
             if (resident && nt == nt0) {
@@ -291,15 +276,10 @@ sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
               tma_load_3d(a_base + kc * A_BYTES, &tmap_a, a_full_bar(kc), kc * BK, m_tile * BM, b);
             }
             const uint32_t sa = ring_base + stage * lay.stage_bytes;
-            if constexpr (PAIR) mbar_wait_cluster(empty_bar(stage), phase ^ 1u);   // both CTAs released the slot
-            else mbar_wait(empty_bar(stage), phase ^ 1u);
+            mbar_wait(empty_bar(stage), phase ^ 1u);
             mbar_arrive_expect_tx(full_bar(stage), stage_tx);
             if (!resident) tma_load_3d(sa, &tmap_a, full_bar(stage), kc * BK, m_tile * BM, b);
-            if constexpr (PAIR)
-              tma_load_3d_multicast(sa + b_off + rank * (B_BYTES / 2), &tmap_b, full_bar(stage), kc * BK,
-                                    nt * BN + static_cast<int>(rank) * (BN / 2), b, 0x3);
-            else
-              tma_load_3d(sa + b_off, &tmap_b, full_bar(stage), kc * BK, nt * BN, b);
+            tma_load_3d(sa + b_off, &tmap_b, full_bar(stage), kc * BK, nt * BN, b);
             if (++stage == stages) { stage = 0; phase ^= 1u; }
           }
         }
@@ -315,13 +295,10 @@ sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     int stage = 0;
     uint32_t phase = 0, a_phase = 0;
     float d[128];
-    // smem slot reusable: this warp's MMAs reading it have retired (both CTAs' consumers gate a slot in the pair build)
+    // smem slot reusable: this warp's MMAs reading it have retired
     auto release = [&](int st) {
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(empty_bar(st));
-        if constexpr (PAIR) mbar_arrive_cluster(mapa_shared(empty_bar(st), rank ^ 1u));
-      }
+      if (lane == 0) mbar_arrive(empty_bar(st));
     };
     auto release_a = [&](int kc) {
       __syncwarp();
@@ -332,7 +309,6 @@ sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       wk.decode(w, &m_tile, &b, &nt0, &nt1);
       if (nt1 > nt_end) nt1 = nt_end;
       if (nt0 >= nt1 || m_tile * BM >= p.Ns) continue;
-      if (PAIR) m_tile = 2 * m_tile + static_cast<int>(rank);   // may lie past M: rows >= Ns are never published
       const int row = m_tile * BM + r0;
       RowBest rb[2];
       rb[0].begin(p, row, b);
@@ -375,45 +351,25 @@ sim_argmax_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       a_phase ^= 1u;
     }
   }
-  // the peer may still multicast into this CTA's shared memory or arrive on its barriers until it is done too
-  if constexpr (PAIR) cluster_sync_all();
 }
 
-template <bool PAIR>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Items& wk, const Layout& lay, const Args& p, int sms,
            cudaStream_t stream) {
   const size_t smem = lay.smem_bytes();
-  // shared-memory opt-in: once per instantiation and device, at the limit (a per-function, per-device attribute)
+  // shared-memory opt-in: once per device, at the limit (a per-function, per-device attribute)
   static bool opted[64];
   int dev = 0;
   int rc = cuda_rc(cudaGetDevice(&dev));
   if (rc) return rc;
   if (dev < 0 || dev >= 64 || !opted[dev]) {
-    rc = cuda_rc(cudaFuncSetAttribute(sim_argmax_kernel<PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    rc = cuda_rc(cudaFuncSetAttribute(sim_argmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       static_cast<int>(SMEM_LIMIT)));
     if (rc) return rc;
     if (dev >= 0 && dev < 64) opted[dev] = true;
   }
-  if constexpr (!PAIR) {
-    const int grid = wk.total < sms ? wk.total : sms;
-    sim_argmax_kernel<false><<<grid, THREADS, smem, stream>>>(ta, tb, wk, lay, p);
-    return launch_rc();
-  } else {
-    const int pairs = wk.total < sms / 2 ? wk.total : sms / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(static_cast<unsigned>(2 * (pairs > 0 ? pairs : 1)));
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cuda_rc(cudaLaunchKernelEx(&cfg, sim_argmax_kernel<true>, ta, tb, wk, lay, p));
-  }
+  const int grid = wk.total < sms ? wk.total : sms;
+  sim_argmax_kernel<<<grid, THREADS, smem, stream>>>(ta, tb, wk, lay, p);
+  return launch_rc();
 }
 }  // namespace ka
 
@@ -466,11 +422,10 @@ namespace vtm {
 namespace {
 // Ns, Nd: the counts, or with counts_dev (device counts) the capacities the buffers and the grid are sized for
 int sim_argmax_impl(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd, int32_t C,
-                    int32_t align_batch, uint64_t* keys_out_dev, void* stream_, bool use_pair,
+                    int32_t align_batch, uint64_t* keys_out_dev, void* stream_,
                     const int32_t* counts_dev = nullptr) {
   int rc = check_args(a_dev, b_dev, B, Ns, Nd, C, keys_out_dev);
   if (rc) return rc;
-  if (counts_dev && use_pair) return VTM_E_SPLIT;   // only the one-CTA build reads device counts
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int Bp = align_batch ? 1 : B;
   rc = cuda_rc(cudaMemsetAsync(keys_out_dev, 0, sizeof(uint64_t) * static_cast<size_t>(Bp) * Ns, stream));
@@ -479,42 +434,35 @@ int sim_argmax_impl(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns,
   CUtensorMap ta, tb;
   rc = make_tmap_3d_f16(&ta, a_dev, C, Ns, B, C, static_cast<uint64_t>(Ns) * C, ka::BK, ka::BM);
   if (rc) return rc;
-  // the pair build loads half of every dst tile per CTA (multicast to both CTAs of the cluster)
-  rc = make_tmap_3d_f16(&tb, b_dev, C, Nd, B, C, static_cast<uint64_t>(Nd) * C, ka::BK, use_pair ? ka::BN / 2 : ka::BN);
+  rc = make_tmap_3d_f16(&tb, b_dev, C, Nd, B, C, static_cast<uint64_t>(Nd) * C, ka::BK, ka::BN);
   if (rc) return rc;
   int sms = 0;
   rc = cached_sm_count(&sms);
   if (rc) return rc;
 
   ka::Items wk;
-  wk.plan(Ns, Nd, C, B, sms, ka::TARGET_ITEMS_PER_SM, use_pair);
+  wk.plan(Ns, Nd, C, B, sms, ka::TARGET_ITEMS_PER_SM);
   ka::Layout lay;
   lay.plan(wk.k_chunks);
   ka::Args p;
   p.keys = reinterpret_cast<unsigned long long*>(keys_out_dev);
   p.Ns = Ns; p.Nd = Nd; p.align_batch = align_batch ? 1 : 0;
   p.ld = Ns; p.counts = counts_dev;
-  if (use_pair) return ka::launch<true>(ta, tb, wk, lay, p, sms, stream);
-  return ka::launch<false>(ta, tb, wk, lay, p, sms, stream);
+  return ka::launch(ta, tb, wk, lay, p, sms, stream);
 }
 }  // namespace
 }  // namespace vtm
 
 extern "C" int vtm_sim_argmax(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd,
                               int32_t C, int32_t align_batch, uint64_t* keys_out_dev, void* stream_) {
-  return vtm::sim_argmax_impl(a_dev, b_dev, B, Ns, Nd, C, align_batch, keys_out_dev, stream_, false);
+  return vtm::sim_argmax_impl(a_dev, b_dev, B, Ns, Nd, C, align_batch, keys_out_dev, stream_);
 }
 
 extern "C" int vtm_sim_argmax_dev(const void* a_dev, const void* b_dev, int32_t B, int32_t ns_cap, int32_t nd_cap,
                                   int32_t C, int32_t align_batch, const int32_t* counts_dev, uint64_t* keys_out_dev,
                                   void* stream_) {
   if (!counts_dev) return VTM_E_NULL;
-  return vtm::sim_argmax_impl(a_dev, b_dev, B, ns_cap, nd_cap, C, align_batch, keys_out_dev, stream_, false, counts_dev);
-}
-
-extern "C" int vtm_sim_argmax_pair(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd,
-                                   int32_t C, int32_t align_batch, uint64_t* keys_out_dev, void* stream_) {
-  return vtm::sim_argmax_impl(a_dev, b_dev, B, Ns, Nd, C, align_batch, keys_out_dev, stream_, true);
+  return vtm::sim_argmax_impl(a_dev, b_dev, B, ns_cap, nd_cap, C, align_batch, keys_out_dev, stream_, counts_dev);
 }
 
 extern "C" int vtm_sim_argmax_simt(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns,

@@ -122,9 +122,6 @@ def normalize_split(x: torch.Tensor, rowmap: Optional[torch.Tensor], split: VtmS
     return a, b
 
 
-KA_VARIANT = "cta"     # "cta" (default) | "pair" (2-CTA cluster build, A/B measurements and tests)
-
-
 def sim_argmax(a: torch.Tensor, b: torch.Tensor, align_batch: bool, simt: bool = False,
                counts: Optional[torch.Tensor] = None) -> torch.Tensor:
     """KA.  Returns the packed keys [B'|Ns] as an int64 tensor (bit pattern of the uint64 keys).  With `counts` (the
@@ -137,14 +134,14 @@ def sim_argmax(a: torch.Tensor, b: torch.Tensor, align_batch: bool, simt: bool =
     lib = _lib.load()
     if counts is not None:
         _require(counts, torch.int32, "counts")
-        if simt or KA_VARIANT != "cta":
-            check(-3, "KA with device counts (only the default one-CTA build reads them)")
+        if simt:
+            check(-3, "KA with device counts (the SIMT twin does not read them)")
         with _Timed("KA", 2.0 * B * Ns * Nd * Cc, 2.0 * B * (Ns + Nd) * Cc + 8.0 * keys.shape[0] * Ns):
             check(lib.vtm_sim_argmax_dev(a.data_ptr(), b.data_ptr(), B, Ns, Nd, Cc, int(bool(align_batch)),
                                          counts.data_ptr(), keys.data_ptr(), _stream()), "vtm_sim_argmax_dev")
         STATS.launches += 1
         return keys
-    fn = lib.vtm_sim_argmax_simt if simt else (lib.vtm_sim_argmax_pair if KA_VARIANT == "pair" else lib.vtm_sim_argmax)
+    fn = lib.vtm_sim_argmax_simt if simt else lib.vtm_sim_argmax
     with _Timed("KA", 2.0 * B * Ns * Nd * Cc, 2.0 * B * (Ns + Nd) * Cc + 8.0 * keys.shape[0] * Ns):
         check(fn(a.data_ptr(), b.data_ptr(), B, Ns, Nd, Cc, int(bool(align_batch)), keys.data_ptr(), _stream()),
               "vtm_sim_argmax")
