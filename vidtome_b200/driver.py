@@ -8,7 +8,9 @@ Restates, on synthetic latents, the parts of the reference's Generator that sit 
   post_iter       generate.py:233-236   (reset global tokens after each step)
   init_pnp        generate.py:313-319   (PnP self-attention injection schedule; with `source_latents`)
   pre_iter        generate.py:226-231   (PnP: set the timestep, fetch the source latents of the step)
-Text conditioning, VAE, ControlNet, PnP's conv-feature injection and file IO are outside the hot path and not restated.
+  ControlNet      generate.py:56-63,264-275, utils/utils.py:280-295 (residuals of `controlnet`, with `control_images`)
+Text conditioning, VAE, ControlNet preprocessing, PnP's conv-feature injection and file IO are outside the hot path and
+not restated.
 """
 from __future__ import annotations
 
@@ -41,7 +43,9 @@ class ChunkedDenoiser:
                  perm_div: float = 3.0, randomize_chunks: bool = False, cond: Optional[torch.Tensor] = None,
                  cuda_graph: bool = False, graph_warmup: int = 2, shard: bool = False, capture_global: bool = False,
                  chunk_graphs: bool = False, source_latents: Optional[Callable[[int], torch.Tensor]] = None,
-                 pnp_attn_t: float = 0.5, pnp_modules: Optional[Iterable[torch.nn.Module]] = None):
+                 pnp_attn_t: float = 0.5, pnp_modules: Optional[Iterable[torch.nn.Module]] = None,
+                 controlnet: Optional[torch.nn.Module] = None, control_images: Optional[torch.Tensor] = None,
+                 control_scale: float = 1.0):
         """`cuda_graph=True`: after `graph_warmup` eager steps, the noise prediction of a whole step (every chunk:
         CFG batch, UNet forward with the merge path, guidance combine) is captured once into a CUDA graph and
         replayed; per step the host then issues one graph launch plus the DDIM update instead of ~250 kernel
@@ -75,7 +79,26 @@ class ChunkedDenoiser:
         the decoder self-attention modules from the source sample (pnp.register_attention_control; `pnp_modules` names
         those modules for a model without the diffusers up_blocks hierarchy).  The model must be patched with
         batch_size=3 and align_batch=True.  In every graph mode the injection is decided on the host when a graph is
-        captured, so graphs are keyed by it as well; the injected ones are released once the schedule has passed."""
+        captured, so graphs are keyed by it as well; the injected ones are released once the schedule has passed.
+
+        `controlnet` with `control_images` ([flen, 3, H, W], the reference's prepare_control output) switches on
+        ControlNet control (generate.py:56-63, `control: "depth"`, `"softedge"`, ...): every UNet call first runs the
+        ControlNet on the same batch and text with the chunk's control images repeated over the CFG batch, scales its
+        residuals by `control_scale` and passes them to the UNet (utils/utils.py:280-295).  The ControlNet may be
+        patched too (apply_patch(include_control=True) on a StableDiffusionControlNetPipeline); its blocks then draw
+        from their own generators and keep their own global tokens, which every graph mode registers and resets like
+        the UNet's.  The control images are a static input of every graph.  One control mode at a time: ControlNet
+        and PnP (`source_latents`) are refused together, as the reference takes one (generate.py:61-68)."""
+        if controlnet is not None and source_latents is not None:
+            raise ValueError("controlnet and source_latents (PnP) are exclusive: the reference runs one control mode "
+                             "(generate.py:61-68)")
+        if (controlnet is None) != (control_images is None):
+            raise ValueError("controlnet and control_images go together")
+        if control_images is not None and (control_images.dim() != 4 or control_images.shape[1] != 3):
+            raise ValueError(f"control_images must be [flen, 3, H, W] (got {tuple(control_images.shape)})")
+        self.controlnet = controlnet
+        self.control_images = control_images
+        self.control_scale = control_scale
         self.unet = unet
         # shard=True: this process is one rank of a torch.distributed job and takes chunks i % world == rank of every
         # step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
@@ -100,7 +123,8 @@ class ChunkedDenoiser:
             raise ValueError("cuda_graph=True needs merge_global=False and randomize_chunks=False (static work)")
         if self.capture_global and self.shard:
             raise ValueError("capture_global=True does not capture the cross-rank exchange of shard=True")
-        # (chunk length, first in step, frame shape, PnP injection) -> (CUDAGraph, static x, static noise, static source)
+        # (chunk length, first in step, frame shape, PnP injection)
+        #   -> (CUDAGraph, static x, static noise, static source, static control images)
         self._chunk_graphs = {}
         self._chunk_t = None        # the UNet's timestep input shared by the chunk graphs
         self._stores = []           # patch.GlobalTokenStore of every block (chunk_graphs with merge_global)
@@ -171,15 +195,27 @@ class ChunkedDenoiser:
 
     # generate.py:238-279
     @torch.no_grad()
-    def pred_noise(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """`src`: the source latents of the chunk (PnP), prepended to the batch."""
+    def pred_noise(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None,
+                   ctrl: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`src`: the source latents of the chunk (PnP), prepended to the batch.  `ctrl`: the control images of the
+        chunk (ControlNet)."""
         flen = len(x)
         text = None if self.cond is None else self.cond.repeat_interleave(flen, dim=0)
         latent_model_input = torch.cat([x, x])                                # classifier-free guidance
+        batch_size = 2
         if src is not None:
             latent_model_input = torch.cat([src.to(x), latent_model_input])
-        eps = self.unet(latent_model_input, t, encoder_hidden_states=text).sample
-        noise_pred_uncond, noise_pred_cond = eps.chunk(2 if src is None else 3)[-2:]
+            batch_size += 1
+        kwargs = {}
+        if ctrl is not None:                                                  # generate.py:264-273
+            controlnet_cond = ctrl.repeat(batch_size, 1, 1, 1)
+            down, mid = self.controlnet(latent_model_input, t, encoder_hidden_states=text,
+                                        controlnet_cond=controlnet_cond, return_dict=False)
+            down = [d * self.control_scale for d in down]                    # utils/utils.py:288-292
+            mid *= self.control_scale
+            kwargs = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
+        eps = self.unet(latent_model_input, t, encoder_hidden_states=text, **kwargs).sample
+        noise_pred_uncond, noise_pred_cond = eps.chunk(batch_size)[-2:]
         return noise_pred_uncond + self.guidance_scale * (noise_pred_cond - noise_pred_uncond)
 
     # generate.py:281-311 (inversion=False branch)
@@ -206,42 +242,50 @@ class ChunkedDenoiser:
                                    "use 'allgather' for ragged chunks")
         return chunks
 
-    def _all_noises(self, x: torch.Tensor, t, src: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _all_noises(self, x: torch.Tensor, t, src: Optional[torch.Tensor] = None,
+                    ctrl: Optional[torch.Tensor] = None) -> torch.Tensor:
         noises = torch.zeros_like(x)
         for chunk in self._step_chunks(len(x)):
             # chunks are contiguous frame ranges (possibly visited in another order): slice instead of indexing with
             # a host tensor, which would cost a synchronous host->device copy per chunk per step
             lo, hi = int(chunk[0]), int(chunk[-1]) + 1
-            noises[lo:hi] = self.pred_noise(x[lo:hi], t, None if src is None else src[lo:hi])
+            noises[lo:hi] = self.pred_noise(x[lo:hi], t, None if src is None else src[lo:hi],
+                                            None if ctrl is None else ctrl[lo:hi])
         return noises
+
+    def _models(self) -> List[torch.nn.Module]:
+        """The UNet and, with ControlNet control, the ControlNet: the models whose blocks the driver serves."""
+        return [self.unet] + ([self.controlnet] if self.controlnet is not None else [])
 
     def _block_generators(self) -> List[torch.Generator]:
         seen, gens = set(), []
-        for m in self.unet.modules():
-            g = getattr(m, "generator", None)
-            if isinstance(g, torch.Generator) and g.device.type == "cuda" and id(g) not in seen:
-                seen.add(id(g))
-                gens.append(g)
+        for model in self._models():
+            for m in model.modules():
+                g = getattr(m, "generator", None)
+                if isinstance(g, torch.Generator) and g.device.type == "cuda" and id(g) not in seen:
+                    seen.add(id(g))
+                    gens.append(g)
         return gens
 
     def _graph_key(self, x: torch.Tensor, t: int):
         return tuple(x.shape), self.injecting(t)
 
-    def _capture(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor]):
+    def _capture(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor], ctrl: Optional[torch.Tensor]):
         """Capture `_all_noises` for inputs shaped like `x` (called after the eager warm-up steps, so that every
         lazily created piece of state — generators forked by the hook, cached packed weights, the library handle,
         allocator pools — already exists)."""
         self._graph = None                                                   # release the previous graph first
         gx = x.clone()
         gsrc = None if src is None else src.to(x).clone()                    # the source latents, set per replay
+        gctrl = None if ctrl is None else ctrl.clone()                       # the control images, set per replay
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)      # the UNet's timestep input, set per replay
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = self._all_noises(gx, gt, gsrc)
-        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gsrc)
+            gn = self._all_noises(gx, gt, gsrc, gctrl)
+        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gsrc, gctrl)
 
     @staticmethod
     def slot_index(chunks: List[torch.Tensor], flen: int) -> torch.Tensor:
@@ -257,7 +301,7 @@ class ChunkedDenoiser:
             raise RuntimeError("slot_index: the chunks must cover every frame exactly once")
         return torch.stack([fwd, inv])
 
-    def _capture_slots(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor]):
+    def _capture_slots(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor], ctrl: Optional[torch.Tensor]):
         """Capture the noise prediction of one step over chunk slots (capture_global=True): slot k runs chunk k of the
         step's visiting order on gx[k * chunk_size:(k + 1) * chunk_size].  get_chunks is not called here, so capturing
         consumes no draw of the host RNG that eager stepping would not."""
@@ -268,31 +312,35 @@ class ChunkedDenoiser:
         self._graph = None                                                   # release the previous graph first
         gx = x.clone()
         gsrc = None if src is None else src.to(x).clone()                   # source latents in slot order
+        gctrl = None if ctrl is None else ctrl.clone()                      # control images in slot order
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
-        patch.update_patch(self.unet, global_tokens=None)                # slot 0 starts the recurrence afresh
+        for model in self._models():                                        # slot 0 starts the recurrence afresh
+            patch.update_patch(model, global_tokens=None)
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
             gn = torch.zeros_like(gx)
             for k in range(flen // cs):
-                gn[k * cs:(k + 1) * cs] = self.pred_noise(gx[k * cs:(k + 1) * cs], gt,
-                                                          None if gsrc is None else gsrc[k * cs:(k + 1) * cs])
+                s = slice(k * cs, (k + 1) * cs)
+                gn[s] = self.pred_noise(gx[s], gt, None if gsrc is None else gsrc[s],
+                                        None if gctrl is None else gctrl[s])
         idx_dev = torch.empty((2, flen), dtype=torch.int64, device=x.device)
         idx_host = torch.empty((2, flen), dtype=torch.int64).pin_memory()
         copied = torch.cuda.Event()          # the pinned buffer is rewritten only after its last upload has run
-        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), idx_dev, idx_host, copied, gsrc)
+        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), idx_dev, idx_host, copied, gsrc, gctrl)
 
-    def _slot_noises(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _slot_noises(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None,
+                     ctrl: Optional[torch.Tensor] = None) -> torch.Tensor:
         flen = len(x)
         if flen % self.chunk_size != 0:
             raise RuntimeError(f"capture_global=True needs a frame count divisible by chunk_size (got {flen} frames, "
                                f"chunk_size {self.chunk_size}): chunks of unequal length cannot share one graph")
         order = self.slot_index(self.get_chunks(flen), flen)        # the same host draws as eager stepping
         if self._graph is None or self._graph[4] != self._graph_key(x, t):
-            self._capture_slots(x, t, src)
-        graph, gx, gt, gn, _, idx_dev, idx_host, copied, gsrc = self._graph
+            self._capture_slots(x, t, src, ctrl)
+        graph, gx, gt, gn, _, idx_dev, idx_host, copied, gsrc, gctrl = self._graph
         copied.synchronize()
         idx_host.copy_(order)
         idx_dev.copy_(idx_host, non_blocking=True)
@@ -300,6 +348,8 @@ class ChunkedDenoiser:
         torch.index_select(x, 0, idx_dev[0], out=gx)                # latents -> slots
         if gsrc is not None:
             torch.index_select(src.to(x), 0, idx_dev[0], out=gsrc)
+        if gctrl is not None:
+            torch.index_select(ctrl, 0, idx_dev[0], out=gctrl)
         gt.fill_(int(t))
         graph.replay()
         return torch.index_select(gn, 0, idx_dev[1])                # slots -> frames
@@ -350,23 +400,27 @@ class ChunkedDenoiser:
 
     def _install_stores(self):
         self._stores = []
-        for m in self.unet.modules():
-            if type(m).__name__ == "ToMeBlock":
-                m.global_tokens = patch.GlobalTokenStore(self.chunk_size)
-                self._stores.append(m.global_tokens)
+        for model in self._models():
+            for m in model.modules():
+                if type(m).__name__ == "ToMeBlock":
+                    m.global_tokens = patch.GlobalTokenStore(self.chunk_size)
+                    self._stores.append(m.global_tokens)
 
     def _reset_global(self):
         if self._stores:
             for st in self._stores:                                         # generate.py:233-236 on the stores
                 st.reset()
         else:
-            patch.update_patch(self.unet, global_tokens=None)               # generate.py:233-236
+            # generate.py:233-236: update_patch(pipe, ...) reaches the UNet and pipe.controlnet
+            for model in self._models():
+                patch.update_patch(model, global_tokens=None)
 
-    def _capture_chunk(self, key, x: torch.Tensor, src: Optional[torch.Tensor]):
+    def _capture_chunk(self, key, x: torch.Tensor, src: Optional[torch.Tensor], ctrl: Optional[torch.Tensor]):
         """Capture the noise prediction of one chunk shaped like `x`; `key[1]` says whether it is the first chunk of a
         step, i.e. whether the blocks' stores are empty when it runs."""
         gx = x.clone()
         gsrc = None if src is None else src.to(x).clone()
+        gctrl = None if ctrl is None else ctrl.clone()
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
@@ -374,11 +428,12 @@ class ChunkedDenoiser:
             st.filled = not key[1]
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = self.pred_noise(gx, self._chunk_t, gsrc)
-        self._chunk_graphs[key] = (graph, gx, gn, gsrc)
+            gn = self.pred_noise(gx, self._chunk_t, gsrc, gctrl)
+        self._chunk_graphs[key] = (graph, gx, gn, gsrc, gctrl)
         return self._chunk_graphs[key]
 
-    def _chunk_graph_noises(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _chunk_graph_noises(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None,
+                            ctrl: Optional[torch.Tensor] = None) -> torch.Tensor:
         flen = len(x)
         chunks = self.get_chunks(flen)                                      # the same host draws as eager stepping
         if not self._chunk_graphs:
@@ -396,11 +451,14 @@ class ChunkedDenoiser:
             key = (hi - lo, self.merge_global and k == 0, tuple(x.shape[1:]), inject)
             entry = self._chunk_graphs.get(key)
             if entry is None:
-                entry = self._capture_chunk(key, x[lo:hi], None if src is None else src[lo:hi])
-            graph, gx, gn, gsrc = entry
+                entry = self._capture_chunk(key, x[lo:hi], None if src is None else src[lo:hi],
+                                            None if ctrl is None else ctrl[lo:hi])
+            graph, gx, gn, gsrc, gctrl = entry
             gx.copy_(x[lo:hi])
             if gsrc is not None:
                 gsrc.copy_(src[lo:hi])
+            if gctrl is not None:
+                gctrl.copy_(ctrl[lo:hi])
             graph.replay()
             noises[lo:hi].copy_(gn)
         return noises
@@ -413,26 +471,33 @@ class ChunkedDenoiser:
         if self.source_latents is not None:                                 # generate.py:226-231 (pre_iter)
             pnp.register_time(self.unet, t, modules=self._pnp_targets)
             src = self.source_latents(t)
+        ctrl = None
+        if self.controlnet is not None:
+            if len(self.control_images) != len(x):
+                raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
+            ctrl = self.control_images.to(x)                                # prepare_data's .to(self.init_noise)
         if self.chunk_graphs and self.merge_global and x.is_cuda and not self._stores:
             self._install_stores()
         if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.chunk_graphs:
-            noises = self._chunk_graph_noises(x, t, src)
+            noises = self._chunk_graph_noises(x, t, src, ctrl)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.capture_global:
-            noises = self._slot_noises(x, t, src)
+            noises = self._slot_noises(x, t, src, ctrl)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup:
             if self._graph is None or self._graph[4] != self._graph_key(x, t):
-                self._capture(x, t, src)
+                self._capture(x, t, src, ctrl)
             graph, gx, gt, gn = self._graph[:4]
-            gsrc = self._graph[5]
+            gsrc, gctrl = self._graph[5:7]
             gx.copy_(x, non_blocking=True)
             if gsrc is not None:
                 gsrc.copy_(src, non_blocking=True)
+            if gctrl is not None:
+                gctrl.copy_(ctrl, non_blocking=True)
             gt.fill_(int(t))
             graph.replay()
             noises = gn
         else:
             self._eager_steps += 1
-            noises = self._all_noises(x, t, src)
+            noises = self._all_noises(x, t, src, ctrl)
         x = self.pred_next_x(x, noises, i)
         if self.merge_global:
             self._reset_global()
