@@ -141,6 +141,10 @@ int vtm_normalize_split_ln(const void* x_dev, int64_t x_batch_stride, const int3
  *       bits 32..47  order-preserving image of the fp16 row maximum (vtm_key_score())
  *       bits  0..31  0xFFFFFFFF - arg, arg = dst index j, or b*Nd + j when align_batch
  *   The buffer is zeroed by this call (cudaMemsetAsync on `stream`) before the kernel runs.
+ * Non-finite scores: a NaN score never wins, so a src row with a NaN entry publishes nothing (its key stays 0) and a
+ * NaN dst column is never the arg; a score that rounds to +inf competes as +inf.  A row whose every score is -inf
+ * publishes nothing either (key 0), where torch's max gives (-inf, index 0).  Neither happens for the unit rows K0
+ * writes: their scores are finite and at most about 1 in magnitude.
  */
 int vtm_sim_argmax(const void* a_dev, const void* b_dev, int32_t B, int32_t Ns, int32_t Nd,
                    int32_t C, int32_t align_batch, uint64_t* keys_out_dev, void* stream);

@@ -12,8 +12,8 @@
 // Kernel layout (persistent grid, 384 threads = three warpgroups):
 //   warpgroup 0      TMA producer (one lane issues);
 //   warpgroups 1, 2  wgmma m64n256k16 consumers, each owning 64 src rows of the tile (128 fp32 accumulators/thread).
-// Shared memory, resident-A form (the work item's whole 128 x C src block fits next to >= 3 ring stages; C <= 320 at
-// the limit of 227 KB): the src block stays in shared memory for the whole work item, one 128B-swizzled 64-column chunk
+// Shared memory, resident-A form (the work item's whole 128 x C src block fits next to >= 3 ring stages within 227 KB:
+// C <= 512, with 6 dst stages up to C = 128, 5 up to 256, 4 up to 384 and 3 up to 512): the src block stays in shared memory for the whole work item, one 128B-swizzled 64-column chunk
 // per K step, each guarded by its own full/empty mbarrier pair, and the ring carries only dst tiles (256 x 64).  A
 // chunk is refilled for the next work item as soon as the last tile's wgmma on it has retired, so the producer keeps
 // running ahead across work items.  Per dst tile only the dst bytes come from L2: 128 FLOP per byte instead of 64 for
