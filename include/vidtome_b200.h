@@ -280,9 +280,10 @@ int vtm_unmerge_add(const void* y_dev, int64_t y_batch_stride, const int32_t* ma
  * math restated in the reference at utils/pnp_utils.py:47-95): q,k,v = x Wq^T, x Wk^T, x Wv^T (no bias),
  * per-head softmax(q k^T * scale) v, heads re-joined, y = o Wo^T + bo.
  *   x_dev [B, L, C] fp16; w_qkv_dev [3C, C] fp16 (rows: Wq | Wk | Wv, torch Linear layout);
- *   w_o_dev [C, C] fp16; b_o_dev [C] fp16 (may be NULL); heads * head_dim == C; head_dim % 8 == 0 and head_dim <= 128 (else VTM_E_SHAPE / VTM_E_UNSUPPORTED)
+ *   w_o_dev [C, C] fp16; b_o_dev [C] fp16 (may be NULL); heads * head_dim == C; head_dim % 8 == 0 and head_dim <= 160 (else VTM_E_SHAPE / VTM_E_UNSUPPORTED)
  *   y_dev [B, L, C] fp16; ws_dev workspace of vtm_attention_workspace_bytes(B, L, C, heads) bytes (q/k/v head-major
- *   with rows padded to 64 or 128 halfs, plus the attention output before the out projection).
+ *   with rows padded to 64, 128 or 192 halfs for head_dim <= 64, <= 128, <= 160, plus the attention output before the
+ *   out projection).
  */
 size_t vtm_attention_workspace_bytes(int32_t B, int32_t L, int32_t C, int32_t heads);
 int vtm_attention(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
@@ -320,7 +321,7 @@ int vtm_linear_f16(const void* a_dev, const void* w_dev, const void* bias_dev, i
  *   q = x Wq^T, [k | v] = ctx [Wk; Wv]^T (no bias), per-head softmax(q k^T * scale) v, y = o Wo^T + bo (+ resid).
  *   x_dev [B, Lq, C] fp16 (norm2 output); ctx_dev [B, Lk, Cctx] fp16; w_q_dev [C, C]; w_kv_dev [2C, Cctx] (rows Wk | Wv);
  *   w_o_dev [C, C]; b_o_dev [C] or NULL; resid_dev [B, Lq, C] or NULL; y_dev [B, Lq, C].
- *   B counts (sample x frame) items: every item attends to its own Lk context rows.  head_dim % 8 == 0, <= 128.
+ *   B counts (sample x frame) items: every item attends to its own Lk context rows.  head_dim % 8 == 0, <= 160.
  */
 size_t vtm_cross_attention_workspace_bytes(int32_t B, int32_t Lq, int32_t Lk, int32_t C, int32_t heads);
 int vtm_cross_attention(const void* x_dev, const void* ctx_dev, const void* w_q_dev, const void* w_kv_dev,

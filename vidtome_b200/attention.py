@@ -16,6 +16,21 @@ from . import _lib, ops
 # Switched on once the attention kernel is built into the library.
 ENABLED = True
 
+# Largest head_dim that runs in the library (self-attention of merged blocks and cross-attention); wider modules run
+# their own forward.  The flash kernel is built up to 160 (KERNEL_MAX_HEAD_DIM): setting 160 here also routes SD1.5's
+# 1280-channel blocks (8 heads of 160) through it.  Read on every dispatch, so it may be changed at any time.
+MAX_HEAD_DIM = 128
+KERNEL_MAX_HEAD_DIM = 160
+
+
+def max_head_dim() -> int:
+    """MAX_HEAD_DIM, checked: a positive multiple of 8 no larger than KERNEL_MAX_HEAD_DIM."""
+    v = MAX_HEAD_DIM
+    if isinstance(v, bool) or not isinstance(v, int) or v <= 0 or v % 8 != 0 or v > KERNEL_MAX_HEAD_DIM:
+        raise ValueError(f"vidtome_b200.attention.MAX_HEAD_DIM = {v!r}: must be a positive multiple of 8 and at most "
+                         f"{KERNEL_MAX_HEAD_DIM}, the widest head the flash-attention kernel is built for")
+    return v
+
 
 def _packed_weights(attn: torch.nn.Module, like: torch.Tensor):
     """[3C, C] fp16 (Wq | Wk | Wv), Wo [C, C], bo [C] — cached on the module, refreshed when a weight
@@ -81,7 +96,7 @@ def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:
     if attn.to_q.weight.dtype != torch.float16 or not attn.to_q.weight.is_cuda or ctx.dtype != torch.float16:
         return False
     d = C // int(attn.heads)
-    return d * int(attn.heads) == C and d % 8 == 0 and d <= 128
+    return d * int(attn.heads) == C and d % 8 == 0 and d <= max_head_dim()
 
 
 def cross_attention_residual(attn: torch.nn.Module, x: torch.Tensor, ctx: torch.Tensor, resid: torch.Tensor) -> torch.Tensor:

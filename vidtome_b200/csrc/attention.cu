@@ -22,7 +22,7 @@ namespace vtm {
 namespace {
 
 // ---------------------------------------------------------------------------------------------------------
-// QKV projection epilogue: writes q, k, v HEAD-MAJOR with rows padded to DP = 64 or 128 halfs (128 / 256 bytes):
+// QKV projection epilogue: writes q, k, v HEAD-MAJOR with rows padded to DP = 64, 128 or 192 halfs (fa_padded_row):
 //   qkvh[which][b][head][l][0..DP)   (which = 0 q, 1 k, 2 v; columns >= head_dim are written as zeros)
 // so that a K or V tile of consecutive keys of one head is one contiguous run of full cache lines (read in place
 // from the [B*L, 3C] GEMM output, every key row would be an 80-byte slice at a 1920-byte pitch: many partial-sector
@@ -117,6 +117,12 @@ struct HeadSplitEpi {
 // Columns of a head-major padded row that the flash kernel reads for head_dim d: 16 x its k-step count.
 inline int fa_columns_read(int d) { return 16 * ((d + 15) / 16); }
 
+// Largest head_dim the flash kernel is built for (KS = 10 k-steps).
+constexpr int FA_MAX_HEAD_DIM = 160;
+
+// Padded row of the head-major q / k / v buffers: the 64-column TMA boxes the flash kernel loads (64, 128 or 192 halfs).
+inline int fa_padded_row(int d) { return 64 * ((fa_columns_read(d) + 63) / 64); }
+
 // x [nb * L, K] -> projections which0 .. which0 + n_proj - 1 of (q, k, v), head-major padded, at `out`
 // ([n_proj][nb][H][L][DP], or projections `which_stride` halfs apart when it is > 0); w [n_proj * C, K].
 int launch_head_proj(const void* x, const void* w, __half* out, int nb, int L, int K, int C, int H, int DP, int which0,
@@ -158,7 +164,8 @@ template <int KS, int G = 1>
 struct FaCfg {
   // Consumer warpgroups, 64 query rows each.  Three (512 threads, at most 128 registers each) hide more of the softmax's
   // latency than two; from head_dim 96 on, O no longer fits next to S and P in 128 registers, so those keep two.  A
-  // CTA that serves G > 1 samples holds G accumulators O and keeps two (up to 168 registers each).
+  // CTA that serves G > 1 samples holds G accumulators O and keeps two (up to 168 registers each, or 232 with the
+  // producer's registers from head_dim 136 on: fa_moves_registers).
   static constexpr int CW = G == 1 && KS <= 5 ? 3 : 2;
   static constexpr int BQ = 64 * CW;                      // query rows per CTA
   static constexpr int THREADS = 128 * (CW + 1);          // producer warpgroup + consumers
@@ -181,6 +188,12 @@ struct FaCfg {
 // Largest number of samples one CTA serves in a shared (PnP) call at KS k-steps: G accumulators O of DV / 2 registers
 // each next to S and P without spills (ptxas -v; DESIGN §4).
 constexpr int fa_group_max(int KS) { return KS <= 2 ? 4 : KS == 3 ? 3 : KS <= 5 ? 2 : 1; }
+
+// From head_dim 136 on (KS >= 9) O takes 72 or 80 registers next to S and P, which leaves KS = 10 at 167 of the 168
+// that 384 threads get at launch: the producer warpgroup, one lane of which only issues TMA loads, gives its registers
+// to the two consumer warpgroups (128 x 40 + 256 x 232 <= 64K), as the GEMM mainloop does.  Below that the kernels are
+// built without setmaxnreg (DESIGN §4).
+constexpr bool fa_moves_registers(int KS) { return KS >= 9; }
 
 // Online softmax of one 64-key tile of S in the log2 domain.  The thread holds rows r0 = lane/4 (s[4n], s[4n+1]) and
 // r0 + 8 (s[4n+2], s[4n+3]), columns 8n + 2(lane%4).  On return s holds P = ex2(s * scale - m_new), m_r the new row
@@ -286,6 +299,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
 
   if (wg == 0) {
     // ===================== TMA producer =====================
+    if constexpr (fa_moves_registers(KS)) setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(q_full, Cf::Q_BYTES);
       for (int a = 0; a < Cf::ATOMS; ++a) tma_load_3d(sq + a * Cf::Q_ATOM, &tm_q, q_full, 64 * a, q0, sqk);
@@ -309,6 +323,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
   }
 
   // ===================== consumers: 64 query rows per warpgroup =====================
+  if constexpr (fa_moves_registers(KS)) setmaxnreg_inc<232>();
   const int cg = wg - 1, wq = warp & 3;
   float o[G][DV / 2];
 #pragma unroll
@@ -512,6 +527,7 @@ int launch_fa_any(const __half* qh, const __half* kh, const __half* vh, __half* 
                                                                  qk_shared, stream, len_dev)                         \
                    : launch_fa_group<KS, fa_group_max(KS), false>(g, qh, kh, vh, o, B, Lq, L, C, H, DP, scale,        \
                                                                   qk_shared, stream, nullptr);
+  if (C / H > FA_MAX_HEAD_DIM) return VTM_E_UNSUPPORTED;
   switch (ks) {
     VTM_FA_CASE(1)
     VTM_FA_CASE(2)
@@ -520,8 +536,11 @@ int launch_fa_any(const __half* qh, const __half* kh, const __half* vh, __half* 
     VTM_FA_CASE(5)
     VTM_FA_CASE(6)
     VTM_FA_CASE(7)
-    default:
     VTM_FA_CASE(8)
+    VTM_FA_CASE(9)
+    VTM_FA_CASE(10)
+    default:
+      return VTM_E_UNSUPPORTED;
   }
 #undef VTM_FA_CASE
 }
@@ -533,8 +552,7 @@ extern "C" size_t vtm_attention_workspace_bytes(int32_t B, int32_t L, int32_t C,
   (void)heads;
   if (B <= 0 || L <= 0 || C <= 0) return 0;
   if (heads <= 0 || C % heads != 0) return 0;
-  const int d = C / heads;
-  const size_t DP = d <= 64 ? 64 : 128;
+  const size_t DP = vtm::fa_padded_row(C / heads);
   // q/k/v head-major [3][B][H][L][DP] + o [B*L, C], fp16
   return (static_cast<size_t>(3) * B * heads * L * DP + static_cast<size_t>(B) * L * C) * 2 + 256;
 }
@@ -549,10 +567,10 @@ int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev
   if (B <= 0 || L <= 0 || C <= 0 || heads <= 0 || C % heads != 0) return VTM_E_SHAPE;
   const int d = C / heads;
   if (d % 8 != 0 || C % 8 != 0) return VTM_E_SHAPE;
-  if (d > 128 || (flags & ~1) != 0) return VTM_E_UNSUPPORTED;
+  if (d > FA_MAX_HEAD_DIM || (flags & ~1) != 0) return VTM_E_UNSUPPORTED;
   if (ws_bytes < vtm_attention_workspace_bytes(B, L, C, heads)) return VTM_E_WS;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const int DP = d <= 64 ? 64 : 128;
+  const int DP = fa_padded_row(d);
   __half* qkv = static_cast<__half*>(ws_dev);
   __half* o = qkv + static_cast<size_t>(3) * B * heads * L * DP;
   const int M = B * L;
@@ -603,8 +621,7 @@ extern "C" int vtm_attention(const void* x_dev, const void* w_qkv_dev, const voi
 // the residual add) — diffusers Attention with K/V from the text context.
 extern "C" size_t vtm_cross_attention_workspace_bytes(int32_t B, int32_t Lq, int32_t Lk, int32_t C, int32_t heads) {
   if (B <= 0 || Lq <= 0 || Lk <= 0 || C <= 0 || heads <= 0 || C % heads != 0) return 0;
-  const int d = C / heads;
-  const size_t DP = d <= 64 ? 64 : 128;
+  const size_t DP = vtm::fa_padded_row(C / heads);
   return (static_cast<size_t>(B) * heads * (static_cast<size_t>(Lq) + 2 * static_cast<size_t>(Lk)) * DP +
           static_cast<size_t>(B) * Lq * C) * 2 + 512;
 }
@@ -618,10 +635,10 @@ extern "C" int vtm_cross_attention(const void* x_dev, const void* ctx_dev, const
   if (B <= 0 || Lq <= 0 || Lk <= 0 || C <= 0 || Cctx <= 0 || heads <= 0 || C % heads != 0) return VTM_E_SHAPE;
   const int d = C / heads;
   if (d % 8 != 0 || C % 8 != 0 || Cctx % 8 != 0) return VTM_E_SHAPE;
-  if (d > 128) return VTM_E_UNSUPPORTED;
+  if (d > FA_MAX_HEAD_DIM) return VTM_E_UNSUPPORTED;
   if (ws_bytes < vtm_cross_attention_workspace_bytes(B, Lq, Lk, C, heads)) return VTM_E_WS;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const int DP = d <= 64 ? 64 : 128;
+  const int DP = fa_padded_row(d);
   __half* qh = static_cast<__half*>(ws_dev);
   __half* kh = qh + static_cast<size_t>(B) * heads * Lq * DP;
   __half* vh = kh + static_cast<size_t>(B) * heads * Lk * DP;

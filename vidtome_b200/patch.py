@@ -403,8 +403,9 @@ def _plain_attention_module(attn: torch.nn.Module) -> bool:
         return False                       # inner dim != query dim or cross-attention shaped K/V
     if attn.to_v.weight.shape != attn.to_q.weight.shape or to_out[0].weight.shape != (C, C):
         return False
+    from .attention import max_head_dim
     head_dim = C // int(attn.heads)
-    return head_dim * int(attn.heads) == C and head_dim % 8 == 0 and head_dim <= 128   # KD's supported range
+    return head_dim * int(attn.heads) == C and head_dim % 8 == 0 and head_dim <= max_head_dim()   # KD's enabled range
 
 
 def make_tome_block(block_class: Type[torch.nn.Module]) -> Type[torch.nn.Module]:
