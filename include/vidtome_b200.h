@@ -345,6 +345,60 @@ int vtm_linear_geglu_f16(const void* a_dev, const void* w_il_dev, const void* bi
 int vtm_linear_residual_f16(const void* a_dev, const void* w_dev, const void* bias_dev, const void* resid_dev,
                             int64_t ldr, int32_t M, int32_t N, int32_t K, void* d_dev, int64_t ldd, void* stream);
 
+/*
+ * LoRA-adapted projections.  A LoRA layer computes y = x W^T + b + sum_a s_a (x A_a^T) B_a^T (diffusers'
+ * LoRACompatibleLinear and peft's lora.Linear, which the reference loads with `pipe.load_lora_weights`, generate.py:93-94).
+ * The adapters of a GEMM are stacked into one "down" matrix D [R, K] (the A_a rows) and one "up" matrix U [N, R] (the
+ * s_a B_a columns, zero where an adapter does not feed an output), and the library computes
+ *     y = fp16([x | T] [W | U]^T + b),   T = fp16(x D^T)
+ * i.e. the projection GEMM with R more K steps taken from (T, U): one fp32 accumulation and one final rounding, every
+ * epilogue (head split, bias, residual, GEGLU) unchanged.  T is computed into the caller's workspace by one extra launch
+ * of the store GEMM (N = R) per adapted GEMM.  A NULL descriptor or R == 0 gives bit for bit the result of the entry
+ * point without LoRA.  Nothing allocates or synchronises; every call can be captured in a CUDA graph.
+ */
+typedef struct vtm_lora_t {
+  const void* down_dev;  /* [R, K] fp16: lora_A rows of every active adapter of the GEMM's projections, stacked   */
+  const void* up_dev;    /* [N, R] fp16: matching lora_B columns with each adapter's scale folded in, 0 elsewhere */
+  int32_t R;             /* total rank, a multiple of 8 (pad with zero rows / columns); 0 = no LoRA               */
+} vtm_lora_t;
+
+/* vtm_linear_f16 / vtm_linear_residual_f16 with a LoRA: D[M, N] = fp16(A W^T + T U^T + bias) (resid_dev == NULL), or
+ * fp16(fp16(A W^T + T U^T + bias) + resid) with resid [M, ldr].  Workspace: vtm_linear_lora_workspace_bytes(M, R)
+ * (T [M, R]; 0 for R == 0, and ws_dev may then be NULL). */
+size_t vtm_linear_lora_workspace_bytes(int32_t M, int32_t R);
+int vtm_linear_lora_f16(const void* a_dev, const void* w_dev, const void* bias_dev, const void* resid_dev, int64_t ldr,
+                        const vtm_lora_t* lora, int32_t M, int32_t N, int32_t K, void* d_dev, int64_t ldd, void* ws_dev,
+                        size_t ws_bytes, void* stream);
+
+/* vtm_linear_geglu_f16 with a LoRA on the GEGLU projection: lora->up_dev [N, R] has its rows interleaved in groups of
+ * 32 exactly as w_il_dev.  Workspace: vtm_linear_lora_workspace_bytes(M, R). */
+int vtm_linear_geglu_lora_f16(const void* a_dev, const void* w_il_dev, const void* bias_il_dev, const vtm_lora_t* lora,
+                              int32_t M, int32_t N, int32_t K, void* d_dev, int64_t ldd, void* ws_dev, size_t ws_bytes,
+                              void* stream);
+
+/* KD with LoRAs: vtm_attention_ex (len_dev == NULL) or vtm_attention_dev (len_dev != NULL, L = L_cap) with
+ *   lora_qkv: the QKV GEMM, D [R, C], U [3C, R] (block-diagonal over the q / k / v row blocks);
+ *   lora_o:   to_out[0], D [R, C], U [C, R]; T is computed from the attention output between the flash kernel and the
+ *             output projection.
+ * Under VTM_ATTN_SHARED_QK q and k take the tail rows of sample 0 and v rows [2C, 3C) of U, as their weights do.
+ * Workspace: vtm_attention_lora_workspace_bytes(B, L, C, heads, R_qkv, R_o). */
+size_t vtm_attention_lora_workspace_bytes(int32_t B, int32_t L, int32_t C, int32_t heads, int32_t R_qkv, int32_t R_o);
+int vtm_attention_lora(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
+                       const vtm_lora_t* lora_qkv, const vtm_lora_t* lora_o, int32_t B, int32_t L, int32_t C,
+                       int32_t heads, float scale, int32_t flags, const int32_t* len_dev, void* y_dev, void* ws_dev,
+                       size_t ws_bytes, void* stream);
+
+/* vtm_cross_attention with LoRAs: lora_q on to_q (D [Rq, C], U [C, Rq], applied to x), lora_kv on to_k / to_v
+ * (D [Rkv, Cctx], U [2C, Rkv], applied to the context), lora_o on to_out[0] (D [Ro, C], U [C, Ro]; the residual is
+ * added after it as without LoRA).  Workspace: vtm_cross_attention_lora_workspace_bytes(B, Lq, Lk, C, heads, Rq, Rkv, Ro). */
+size_t vtm_cross_attention_lora_workspace_bytes(int32_t B, int32_t Lq, int32_t Lk, int32_t C, int32_t heads, int32_t R_q,
+                                                int32_t R_kv, int32_t R_o);
+int vtm_cross_attention_lora(const void* x_dev, const void* ctx_dev, const void* w_q_dev, const void* w_kv_dev,
+                             const void* w_o_dev, const void* b_o_dev, const void* resid_dev, const vtm_lora_t* lora_q,
+                             const vtm_lora_t* lora_kv, const vtm_lora_t* lora_o, int32_t B, int32_t Lq, int32_t Lk,
+                             int32_t C, int32_t Cctx, int32_t heads, float scale, void* y_dev, void* ws_dev,
+                             size_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -82,8 +82,14 @@ class VtmSplitDev(VtmSplit):
     _fields_ = [("glob_len_dev", C.c_void_p), ("glob_cap", C.c_int32)]
 
 
+class VtmLora(C.Structure):
+    """struct vtm_lora_t (include/vidtome_b200.h): a GEMM's stacked LoRA adapters, down D [R, K] and up U [N, R]."""
+    _fields_ = [("down_dev", C.c_void_p), ("up_dev", C.c_void_p), ("R", C.c_int32)]
+
+
 _vp, _i32, _i64, _sz = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
 _SPL = C.POINTER(VtmSplit)
+_LORA = C.POINTER(VtmLora)
 
 # name -> (restype, argtypes); mirrors include/vidtome_b200.h one to one
 SIGNATURES = {
@@ -125,6 +131,15 @@ SIGNATURES = {
     "vtm_linear_f16": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _i64, _vp]),
     "vtm_linear_geglu_f16": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _i64, _vp]),
     "vtm_linear_residual_f16": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp]),
+    "vtm_linear_lora_workspace_bytes": (_sz, [_i32, _i32]),
+    "vtm_linear_lora_f16": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _LORA, _i32, _i32, _i32, _vp, _i64, _vp, _sz, _vp]),
+    "vtm_linear_geglu_lora_f16": (C.c_int, [_vp, _vp, _vp, _LORA, _i32, _i32, _i32, _vp, _i64, _vp, _sz, _vp]),
+    "vtm_attention_lora_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32, _i32]),
+    "vtm_attention_lora": (C.c_int, [_vp, _vp, _vp, _vp, _LORA, _LORA, _i32, _i32, _i32, _i32, C.c_float, _i32, _vp,
+                                     _vp, _vp, _sz, _vp]),
+    "vtm_cross_attention_lora_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32]),
+    "vtm_cross_attention_lora": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _LORA, _LORA, _LORA, _i32, _i32, _i32,
+                                           _i32, _i32, _i32, C.c_float, _vp, _vp, _sz, _vp]),
 }
 
 _lib: Optional[C.CDLL] = None

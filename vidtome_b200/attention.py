@@ -11,7 +11,7 @@ from typing import Optional
 
 import torch
 
-from . import _lib, ops
+from . import _lib, lora, ops
 
 # Switched on once the attention kernel is built into the library.
 ENABLED = True
@@ -32,19 +32,33 @@ def max_head_dim() -> int:
     return v
 
 
-def _packed_weights(attn: torch.nn.Module, like: torch.Tensor):
-    """[3C, C] fp16 (Wq | Wk | Wv), Wo [C, C], bo [C] — cached on the module, refreshed when a weight
-    tensor is replaced or modified in place."""
-    ws = (attn.to_q.weight, attn.to_k.weight, attn.to_v.weight, attn.to_out[0].weight, attn.to_out[0].bias)
-    tag = tuple((w.data_ptr(), w._version) for w in ws if w is not None) + (like.device,)
+def _packed(attn: torch.nn.Module, like: torch.Tensor):
+    """(w_qkv, w_o, b_o, lora_qkv, lora_o): the tensors of _packed_weights and the LoRA packs (lora.pack) of the QKV GEMM
+    and of to_out[0] (None without adapters) — cached on the module, refreshed when a weight or adapter tensor is replaced
+    or modified in place, a scale changes or another set of adapters becomes active (lora.tag).  Under CUDA-graph replay
+    nothing is re-read: LoRA changes after capture are as static as weight changes."""
+    parts = [lora.linear_parts(m) for m in (attn.to_q, attn.to_k, attn.to_v, attn.to_out[0])]
+    tag = lora.tag(parts) + (like.device,)
     cache = getattr(attn, "_vtm_packed", None)
     if cache is None or cache[0] != tag:
-        w_qkv = torch.cat([ws[0], ws[1], ws[2]], dim=0).to(device=like.device, dtype=torch.float16).contiguous()
-        w_o = ws[3].to(device=like.device, dtype=torch.float16).contiguous()
-        b_o = None if ws[4] is None else ws[4].to(device=like.device, dtype=torch.float16).contiguous()
-        cache = (tag, w_qkv, w_o, b_o)
+        dev = like.device
+        w_qkv = torch.cat([p[0] for p in parts[:3]], dim=0).detach().to(device=dev, dtype=torch.float16).contiguous()
+        w_o = parts[3][0].detach().to(device=dev, dtype=torch.float16).contiguous()
+        b_o = None if parts[3][1] is None else parts[3][1].detach().to(device=dev, dtype=torch.float16).contiguous()
+        cache = (tag, w_qkv, w_o, b_o, lora.pack(parts[:3], dev), lora.pack(parts[3:], dev))
         attn._vtm_packed = cache
     return cache[1:]
+
+
+def _packed_weights(attn: torch.nn.Module, like: torch.Tensor):
+    """[3C, C] fp16 (Wq | Wk | Wv), Wo [C, C], bo [C] — cached on the module, refreshed when a weight tensor is replaced
+    or modified in place."""
+    return _packed(attn, like)[:3]
+
+
+def _packed_lora(attn: torch.nn.Module, like: torch.Tensor):
+    """(lora_qkv, lora_o): the LoRA packs of the QKV GEMM and of to_out[0], None where there is no adapter."""
+    return _packed(attn, like)[3:]
 
 
 def self_attention(attn: torch.nn.Module, x: torch.Tensor, shared_qk: bool = False,
@@ -52,15 +66,17 @@ def self_attention(attn: torch.nn.Module, x: torch.Tensor, shared_qk: bool = Fal
     """softmax(q k^T * scale) v with q,k,v = to_q/to_k/to_v(x), then to_out[0] (utils/pnp_utils.py:47-95).
     shared_qk: PnP injection — q and k of sample 0 for every sample (utils/pnp_utils.py:57-68,87-91).
     seq_len: the sequence is the first seq_len (a 1-element int32 CUDA tensor) rows of x (GlobalTokenStore stage)."""
-    w_qkv, w_o, b_o = _packed_weights(attn, x)
+    w_qkv, w_o, b_o, lora_qkv, lora_o = _packed(attn, x)
     heads = int(attn.heads)
     scale = float(getattr(attn, "scale", (x.shape[-1] // heads) ** -0.5))
-    return ops.attention(x, w_qkv, w_o, b_o, heads, scale, shared_qk=shared_qk, seq_len=seq_len)
+    return ops.attention(x, w_qkv, w_o, b_o, heads, scale, shared_qk=shared_qk, seq_len=seq_len, lora_qkv=lora_qkv,
+                         lora_o=lora_o)
 
 
 def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:
     """True if `attn` is a stock diffusers-style cross-attention (to_q [C, C], to_k / to_v [C, Cctx] without bias,
-    to_out = [Linear, Dropout], default processor, no hooks / overrides / options that alter the math)."""
+    to_out = [Linear, Dropout], default processor, no hooks / overrides / options that alter the math).  The projections
+    may be LoRA-adapted in any form lora.linear_parts reads."""
     from .patch import _PLAIN_PROCESSORS
     if attn is None or "forward" in vars(attn) or not isinstance(ctx, torch.Tensor) or ctx.dim() != 3:
         return False
@@ -71,7 +87,8 @@ def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:
     if not isinstance(to_out, (torch.nn.ModuleList, torch.nn.Sequential)) or len(to_out) < 1:
         return False
     linears = (attn.to_q, attn.to_k, attn.to_v, to_out[0])
-    if any(type(m) is not torch.nn.Linear for m in linears) or any(m.bias is not None for m in linears[:3]):
+    parts = [lora.linear_parts(m) for m in linears]
+    if any(p is None for p in parts) or any(p[1] is not None for p in parts[:3]):
         return False
     for m in (attn,) + linears + tuple(to_out[1:]):
         if m._forward_hooks or m._forward_pre_hooks:
@@ -87,13 +104,14 @@ def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:
             return False
     if getattr(attn, "residual_connection", False) or getattr(attn, "rescale_output_factor", 1.0) != 1.0:
         return False
-    C = attn.to_q.weight.shape[1]
-    Cctx = attn.to_k.weight.shape[1]
-    if attn.to_q.weight.shape != (C, C) or attn.to_k.weight.shape != (C, Cctx) or attn.to_v.weight.shape != (C, Cctx):
+    wq, wk, wv, wo = (p[0] for p in parts)
+    C = wq.shape[1]
+    Cctx = wk.shape[1]
+    if wq.shape != (C, C) or wk.shape != (C, Cctx) or wv.shape != (C, Cctx):
         return False
-    if to_out[0].weight.shape != (C, C) or ctx.shape[-1] != Cctx or Cctx % 8 != 0:
+    if wo.shape != (C, C) or ctx.shape[-1] != Cctx or Cctx % 8 != 0:
         return False
-    if attn.to_q.weight.dtype != torch.float16 or not attn.to_q.weight.is_cuda or ctx.dtype != torch.float16:
+    if wq.dtype != torch.float16 or not wq.is_cuda or ctx.dtype != torch.float16:
         return False
     d = C // int(attn.heads)
     return d * int(attn.heads) == C and d % 8 == 0 and d <= max_head_dim()
@@ -101,15 +119,19 @@ def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:
 
 def cross_attention_residual(attn: torch.nn.Module, x: torch.Tensor, ctx: torch.Tensor, resid: torch.Tensor) -> torch.Tensor:
     """attn2(x, encoder_hidden_states=ctx) + resid (vidtome/patch.py:171-185) through vtm_cross_attention."""
-    ws = (attn.to_q.weight, attn.to_k.weight, attn.to_v.weight, attn.to_out[0].weight, attn.to_out[0].bias)
-    tag = tuple((w.data_ptr(), w._version) for w in ws if w is not None)
+    parts = [lora.linear_parts(m) for m in (attn.to_q, attn.to_k, attn.to_v, attn.to_out[0])]
+    tag = lora.tag(parts)
     cache = getattr(attn, "_vtm_packed_x", None)
     if cache is None or cache[0] != tag:
-        w_kv = torch.cat([ws[1], ws[2]], dim=0).detach().contiguous()
-        cache = (tag, ws[0].detach().contiguous(), w_kv, ws[3].detach().contiguous(),
-                 None if ws[4] is None else ws[4].detach().contiguous())
+        (wq, _, _), (wk, _, _), (wv, _, _), (wo, bo, _) = parts
+        w_kv = torch.cat([wk, wv], dim=0).detach().contiguous()
+        dev = wq.device
+        cache = (tag, wq.detach().contiguous(), w_kv, wo.detach().contiguous(),
+                 None if bo is None else bo.detach().contiguous(),
+                 lora.pack(parts[:1], dev), lora.pack(parts[1:3], dev), lora.pack(parts[3:], dev))
         attn._vtm_packed_x = cache
-    _, w_q, w_kv, w_o, b_o = cache
+    _, w_q, w_kv, w_o, b_o, lora_q, lora_kv, lora_o = cache
     heads = int(attn.heads)
     scale = float(getattr(attn, "scale", (x.shape[-1] // heads) ** -0.5))
-    return ops.cross_attention(x.contiguous(), ctx.contiguous(), w_q, w_kv, w_o, b_o, heads, scale, resid=resid.contiguous())
+    return ops.cross_attention(x.contiguous(), ctx.contiguous(), w_q, w_kv, w_o, b_o, heads, scale, resid=resid.contiguous(),
+                               lora_q=lora_q, lora_kv=lora_kv, lora_o=lora_o)

@@ -17,6 +17,8 @@ extern "C" int vtm_linear_f16(const void*, const void*, const void*, int32_t, in
                               void*);
 extern "C" int vtm_linear_residual_f16(const void*, const void*, const void*, const void*, int64_t, int32_t, int32_t,
                                        int32_t, void*, int64_t, void*);
+extern "C" int vtm_linear_lora_f16(const void*, const void*, const void*, const void*, int64_t, const vtm_lora_t*,
+                                   int32_t, int32_t, int32_t, void*, int64_t, void*, size_t, void*);
 
 namespace vtm {
 namespace {
@@ -125,8 +127,10 @@ inline int fa_padded_row(int d) { return 64 * ((fa_columns_read(d) + 63) / 64); 
 
 // x [nb * L, K] -> projections which0 .. which0 + n_proj - 1 of (q, k, v), head-major padded, at `out`
 // ([n_proj][nb][H][L][DP], or projections `which_stride` halfs apart when it is > 0); w [n_proj * C, K].
+// t / u / R: a LoRA's K tail, T [nb * L, R] and U [n_proj * C, R] (R == 0: none).
 int launch_head_proj(const void* x, const void* w, __half* out, int nb, int L, int K, int C, int H, int DP, int which0,
-                     int n_proj, cudaStream_t stream, long long which_stride = 0) {
+                     int n_proj, cudaStream_t stream, long long which_stride = 0, const void* t = nullptr,
+                     const void* u = nullptr, int R = 0) {
   int sms = 0;
   int rc = gemm::device_sms(&sms);
   if (rc) return rc;
@@ -145,7 +149,21 @@ int launch_head_proj(const void* x, const void* w, __half* out, int nb, int L, i
   gemm::Work wk;
   wk.plan(M, N, K, 1, sms, 16, 1);
   wk.n_fastest = 1;
-  return gemm::launch<HeadSplitEpi>(ta, tb, wk, epi, sms, stream);
+  if (R == 0) return gemm::launch<HeadSplitEpi>(ta, tb, wk, epi, sms, stream);
+  CUtensorMap tt, tu;
+  rc = gemm::make_tail(t, u, R, M, N, &tt, &tu, &wk);
+  if (rc) return rc;
+  return gemm::launch_tail<HeadSplitEpi>(ta, tb, tt, tu, wk, epi, sms, stream);
+}
+
+// Rank of a LoRA descriptor (0 for NULL), checked.
+int lora_rank(const vtm_lora_t* l, int* R) {
+  *R = 0;
+  if (!l || l->R == 0) return VTM_OK;
+  if (l->R < 0 || l->R % 8 != 0) return VTM_E_SHAPE;
+  if (!l->down_dev || !l->up_dev) return VTM_E_NULL;
+  *R = l->R;
+  return VTM_OK;
 }
 
 constexpr int FA_BKV = 64;       // keys per K/V tile
@@ -557,18 +575,32 @@ extern "C" size_t vtm_attention_workspace_bytes(int32_t B, int32_t L, int32_t C,
   return (static_cast<size_t>(3) * B * heads * L * DP + static_cast<size_t>(B) * L * C) * 2 + 256;
 }
 
+extern "C" size_t vtm_attention_lora_workspace_bytes(int32_t B, int32_t L, int32_t C, int32_t heads, int32_t R_qkv,
+                                                     int32_t R_o) {
+  const size_t base = vtm_attention_workspace_bytes(B, L, C, heads);
+  if (base == 0 || R_qkv < 0 || R_o < 0) return 0;
+  // T of the QKV GEMM, then of the output projection, in one [B*L, max(R_qkv, R_o)] buffer after o
+  return base + static_cast<size_t>(B) * L * (R_qkv > R_o ? R_qkv : R_o) * 2;
+}
+
 namespace vtm {
 namespace {
 // len_dev: NULL, or the sequence length on the device with L the rows of the buffers (vtm_attention_dev)
 int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev, int32_t B,
                    int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, const int32_t* len_dev, void* y_dev,
-                   void* ws_dev, size_t ws_bytes, void* stream_) {
+                   void* ws_dev, size_t ws_bytes, void* stream_, const vtm_lora_t* lora_qkv = nullptr,
+                   const vtm_lora_t* lora_o = nullptr) {
   if (!x_dev || !w_qkv_dev || !w_o_dev || !y_dev || !ws_dev) return VTM_E_NULL;
   if (B <= 0 || L <= 0 || C <= 0 || heads <= 0 || C % heads != 0) return VTM_E_SHAPE;
   const int d = C / heads;
   if (d % 8 != 0 || C % 8 != 0) return VTM_E_SHAPE;
   if (d > FA_MAX_HEAD_DIM || (flags & ~1) != 0) return VTM_E_UNSUPPORTED;
-  if (ws_bytes < vtm_attention_workspace_bytes(B, L, C, heads)) return VTM_E_WS;
+  int Rq = 0, Ro = 0;
+  int rc = lora_rank(lora_qkv, &Rq);
+  if (rc) return rc;
+  rc = lora_rank(lora_o, &Ro);
+  if (rc) return rc;
+  if (ws_bytes < vtm_attention_lora_workspace_bytes(B, L, C, heads, Rq, Ro)) return VTM_E_WS;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int DP = fa_padded_row(d);
   __half* qkv = static_cast<__half*>(ws_dev);
@@ -577,19 +609,28 @@ int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev
   const size_t slab = static_cast<size_t>(B) * heads * L * DP;    // one of q, k, v for all samples
   __half* kh = qkv + slab;
   __half* vh = kh + slab;
-  int rc;
+  __half* t = o + static_cast<size_t>(M) * C;                      // LoRA T buffer [M, max(Rq, Ro)]
+  const __half* uq = Rq ? static_cast<const __half*>(lora_qkv->up_dev) : nullptr;
+  if (Rq) {
+    rc = vtm_linear_f16(x_dev, lora_qkv->down_dev, nullptr, M, Rq, C, t, Rq, stream_);
+    if (rc) return rc;
+  }
   if (flags & 1) {
     // shared: q and k of sample 0 (the only ones the flash kernel reads), v of every sample
-    rc = launch_head_proj(x_dev, w_qkv_dev, qkv, 1, L, C, C, heads, DP, 0, 2, stream, static_cast<long long>(slab));
+    rc = launch_head_proj(x_dev, w_qkv_dev, qkv, 1, L, C, C, heads, DP, 0, 2, stream, static_cast<long long>(slab), t,
+                          uq, Rq);
     if (rc) return rc;
     rc = launch_head_proj(x_dev, static_cast<const __half*>(w_qkv_dev) + static_cast<size_t>(2) * C * C, vh, B, L, C, C,
-                          heads, DP, 2, 1, stream);
+                          heads, DP, 2, 1, stream, 0, t, Rq ? uq + static_cast<size_t>(2) * C * Rq : nullptr, Rq);
   } else {
-    rc = launch_head_proj(x_dev, w_qkv_dev, qkv, B, L, C, C, heads, DP, 0, 3, stream);
+    rc = launch_head_proj(x_dev, w_qkv_dev, qkv, B, L, C, C, heads, DP, 0, 3, stream, 0, t, uq, Rq);
   }
   if (rc) return rc;
   rc = launch_fa_any(qkv, kh, vh, o, B, L, L, C, heads, DP, scale, flags & 1, stream, len_dev);
   if (rc) return rc;
+  if (Ro)
+    return vtm_linear_lora_f16(o, w_o_dev, b_o_dev, nullptr, 0, lora_o, M, C, C, y_dev, C, t,
+                               static_cast<size_t>(M) * Ro * 2, stream_);
   return vtm_linear_f16(o, w_o_dev, b_o_dev, M, C, C, y_dev, C, stream_);
 }
 }  // namespace
@@ -610,6 +651,14 @@ extern "C" int vtm_attention_dev(const void* x_dev, const void* w_qkv_dev, const
                              ws_dev, ws_bytes, stream_);
 }
 
+extern "C" int vtm_attention_lora(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
+                                  const vtm_lora_t* lora_qkv, const vtm_lora_t* lora_o, int32_t B, int32_t L, int32_t C,
+                                  int32_t heads, float scale, int32_t flags, const int32_t* len_dev, void* y_dev,
+                                  void* ws_dev, size_t ws_bytes, void* stream_) {
+  return vtm::attention_impl(x_dev, w_qkv_dev, w_o_dev, b_o_dev, B, L, C, heads, scale, flags, len_dev, y_dev, ws_dev,
+                             ws_bytes, stream_, lora_qkv, lora_o);
+}
+
 extern "C" int vtm_attention(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
                              int32_t B, int32_t L, int32_t C, int32_t heads, float scale, void* y_dev,
                              void* ws_dev, size_t ws_bytes, void* stream_) {
@@ -626,30 +675,82 @@ extern "C" size_t vtm_cross_attention_workspace_bytes(int32_t B, int32_t Lq, int
           static_cast<size_t>(B) * Lq * C) * 2 + 512;
 }
 
-extern "C" int vtm_cross_attention(const void* x_dev, const void* ctx_dev, const void* w_q_dev, const void* w_kv_dev,
-                                   const void* w_o_dev, const void* b_o_dev, const void* resid_dev, int32_t B, int32_t Lq,
-                                   int32_t Lk, int32_t C, int32_t Cctx, int32_t heads, float scale, void* y_dev,
-                                   void* ws_dev, size_t ws_bytes, void* stream_) {
-  using namespace vtm;
+extern "C" size_t vtm_cross_attention_lora_workspace_bytes(int32_t B, int32_t Lq, int32_t Lk, int32_t C, int32_t heads,
+                                                           int32_t R_q, int32_t R_kv, int32_t R_o) {
+  const size_t base = vtm_cross_attention_workspace_bytes(B, Lq, Lk, C, heads);
+  if (base == 0 || R_q < 0 || R_kv < 0 || R_o < 0) return 0;
+  // T of to_q, then of to_out, in one [B*Lq, max(R_q, R_o)] buffer; T of to_k / to_v [B*Lk, R_kv]
+  return base + (static_cast<size_t>(B) * Lq * (R_q > R_o ? R_q : R_o) + static_cast<size_t>(B) * Lk * R_kv) * 2;
+}
+
+namespace vtm {
+namespace {
+int cross_attention_impl(const void* x_dev, const void* ctx_dev, const void* w_q_dev, const void* w_kv_dev,
+                         const void* w_o_dev, const void* b_o_dev, const void* resid_dev, const vtm_lora_t* lora_q,
+                         const vtm_lora_t* lora_kv, const vtm_lora_t* lora_o, int32_t B, int32_t Lq, int32_t Lk,
+                         int32_t C, int32_t Cctx, int32_t heads, float scale, void* y_dev, void* ws_dev, size_t ws_bytes,
+                         void* stream_) {
   if (!x_dev || !ctx_dev || !w_q_dev || !w_kv_dev || !w_o_dev || !y_dev || !ws_dev) return VTM_E_NULL;
   if (B <= 0 || Lq <= 0 || Lk <= 0 || C <= 0 || Cctx <= 0 || heads <= 0 || C % heads != 0) return VTM_E_SHAPE;
   const int d = C / heads;
   if (d % 8 != 0 || C % 8 != 0 || Cctx % 8 != 0) return VTM_E_SHAPE;
   if (d > FA_MAX_HEAD_DIM) return VTM_E_UNSUPPORTED;
-  if (ws_bytes < vtm_cross_attention_workspace_bytes(B, Lq, Lk, C, heads)) return VTM_E_WS;
+  int Rq = 0, Rkv = 0, Ro = 0;
+  int rc = lora_rank(lora_q, &Rq);
+  if (rc) return rc;
+  rc = lora_rank(lora_kv, &Rkv);
+  if (rc) return rc;
+  rc = lora_rank(lora_o, &Ro);
+  if (rc) return rc;
+  if (ws_bytes < vtm_cross_attention_lora_workspace_bytes(B, Lq, Lk, C, heads, Rq, Rkv, Ro)) return VTM_E_WS;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int DP = fa_padded_row(d);
   __half* qh = static_cast<__half*>(ws_dev);
   __half* kh = qh + static_cast<size_t>(B) * heads * Lq * DP;
   __half* vh = kh + static_cast<size_t>(B) * heads * Lk * DP;
   __half* o = vh + static_cast<size_t>(B) * heads * Lk * DP;
-  int rc = launch_head_proj(x_dev, w_q_dev, qh, B, Lq, C, C, heads, DP, 0, 1, stream);
+  const int M = B * Lq;
+  __half* tq = o + static_cast<size_t>(M) * C;                      // T of to_q / to_out [M, max(Rq, Ro)]
+  __half* tkv = tq + static_cast<size_t>(M) * (Rq > Ro ? Rq : Ro);  // T of to_k / to_v [B * Lk, Rkv]
+  if (Rq) {
+    rc = vtm_linear_f16(x_dev, lora_q->down_dev, nullptr, M, Rq, C, tq, Rq, stream_);
+    if (rc) return rc;
+  }
+  rc = launch_head_proj(x_dev, w_q_dev, qh, B, Lq, C, C, heads, DP, 0, 1, stream, 0, tq, Rq ? lora_q->up_dev : nullptr,
+                        Rq);
   if (rc) return rc;
-  rc = launch_head_proj(ctx_dev, w_kv_dev, kh, B, Lk, Cctx, C, heads, DP, 1, 2, stream);
+  if (Rkv) {
+    rc = vtm_linear_f16(ctx_dev, lora_kv->down_dev, nullptr, B * Lk, Rkv, Cctx, tkv, Rkv, stream_);
+    if (rc) return rc;
+  }
+  rc = launch_head_proj(ctx_dev, w_kv_dev, kh, B, Lk, Cctx, C, heads, DP, 1, 2, stream, 0, tkv,
+                        Rkv ? lora_kv->up_dev : nullptr, Rkv);
   if (rc) return rc;
   rc = launch_fa_any(qh, kh, vh, o, B, Lq, Lk, C, heads, DP, scale, 0, stream);
   if (rc) return rc;
-  const int M = B * Lq;
+  if (Ro)
+    return vtm_linear_lora_f16(o, w_o_dev, b_o_dev, resid_dev, C, lora_o, M, C, C, y_dev, C, tq,
+                               static_cast<size_t>(M) * Ro * 2, stream_);
   if (resid_dev) return vtm_linear_residual_f16(o, w_o_dev, b_o_dev, resid_dev, C, M, C, C, y_dev, C, stream_);
   return vtm_linear_f16(o, w_o_dev, b_o_dev, M, C, C, y_dev, C, stream_);
+}
+}  // namespace
+}  // namespace vtm
+
+extern "C" int vtm_cross_attention(const void* x_dev, const void* ctx_dev, const void* w_q_dev, const void* w_kv_dev,
+                                   const void* w_o_dev, const void* b_o_dev, const void* resid_dev, int32_t B, int32_t Lq,
+                                   int32_t Lk, int32_t C, int32_t Cctx, int32_t heads, float scale, void* y_dev,
+                                   void* ws_dev, size_t ws_bytes, void* stream_) {
+  return vtm::cross_attention_impl(x_dev, ctx_dev, w_q_dev, w_kv_dev, w_o_dev, b_o_dev, resid_dev, nullptr, nullptr,
+                                   nullptr, B, Lq, Lk, C, Cctx, heads, scale, y_dev, ws_dev, ws_bytes, stream_);
+}
+
+extern "C" int vtm_cross_attention_lora(const void* x_dev, const void* ctx_dev, const void* w_q_dev,
+                                        const void* w_kv_dev, const void* w_o_dev, const void* b_o_dev,
+                                        const void* resid_dev, const vtm_lora_t* lora_q, const vtm_lora_t* lora_kv,
+                                        const vtm_lora_t* lora_o, int32_t B, int32_t Lq, int32_t Lk, int32_t C,
+                                        int32_t Cctx, int32_t heads, float scale, void* y_dev, void* ws_dev,
+                                        size_t ws_bytes, void* stream_) {
+  return vtm::cross_attention_impl(x_dev, ctx_dev, w_q_dev, w_kv_dev, w_o_dev, b_o_dev, resid_dev, lora_q, lora_kv,
+                                   lora_o, B, Lq, Lk, C, Cctx, heads, scale, y_dev, ws_dev, ws_bytes, stream_);
 }

@@ -10,6 +10,12 @@
 // tile i+1 overlap the epilogue of tile i.
 // A work item is (m_tile, b, [nt0, nt1)); CTAs stride over work items (persistent grid = #SMs).
 //
+// K tail (TAIL = true): after its k_chunks chunks of (A, Bm) the producer loads wk.t_chunks further chunks from a second
+// operand pair (T [M, R] through tmap_t, U [N, R] through tmap_u) into the same ring, and the consumers add them to the
+// same accumulators:  D = [A | T] [Bm | U]^T.  This is how a LoRA's low-rank update x D^T U^T joins its projection
+// (T = x D^T, computed beforehand): R extra K columns, every epilogue unchanged.  TMA zero-fills the boxes past R, so the
+// stage's byte count is the same as for a main chunk.  TAIL = false compiles to the plain mainloop.
+//
 // Epilogues read one ROW per thread: after its mainloop a warpgroup writes its fp32 accumulators to a row-major
 // staging area in shared memory, and thread t of the warpgroup then owns row (t % 64) and column half (t / 64) of its
 // 64 rows, so that a warp holds 32 consecutive rows of one half.
@@ -71,6 +77,7 @@ struct Work {
   int m_tiles, n_tiles;
   int tiles_per_split, n_splits;
   int k_chunks;
+  int t_chunks;         // K-tail chunks (TAIL kernels only): ceil(R / BK)
   int total;
   // Order of the work items.  0: m tile fastest.  1: n split fastest (plain GEMMs): the splits of one m tile run on
   // neighbouring CTAs at the same time, so the A tile comes from HBM once and from L2 afterwards.
@@ -81,6 +88,7 @@ struct Work {
     m_tiles = (M + BM - 1) / BM;
     n_tiles = (N + BN - 1) / BN;
     k_chunks = (K + BK - 1) / BK;
+    t_chunks = 0;
     const long long base = static_cast<long long>(m_tiles) * B;
     int s = 1;
     while (base * s < static_cast<long long>(target_items_per_sm) * sms && s * 2 <= n_tiles &&
@@ -139,10 +147,19 @@ __device__ __forceinline__ void warp_store_rows64(uint32_t scratch, const uint32
   __syncwarp();
 }
 
-template <class Epi>
+// The K tail's tensor maps as one kernel parameter: empty without a tail, so that the plain kernels take the same
+// parameters as before the tail existed.
+template <bool TAIL>
+struct TailMaps {
+  CUtensorMap t, u;
+};
+template <>
+struct TailMaps<false> {};
+
+template <class Epi, bool TAIL>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-            const Work wk, Epi epi) {
+            const __grid_constant__ TailMaps<TAIL> tail, const Work wk, Epi epi) {
   using C = Cfg<Epi::SCRATCH_PER_WARP>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -164,6 +181,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if constexpr (TAIL) {
+      tma_prefetch_desc(&tail.t);
+      tma_prefetch_desc(&tail.u);
+    }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), CONSUMER_WARPS);
@@ -182,12 +203,24 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         int m_tile, b, nt0, nt1;
         wk.decode(w, &m_tile, &b, &nt0, &nt1);
         for (int nt = nt0; nt < nt1; ++nt) {
-          for (int kc = 0; kc < wk.k_chunks; ++kc) {
+          const int kn = TAIL ? wk.k_chunks + wk.t_chunks : wk.k_chunks;
+          for (int kc = 0; kc < kn; ++kc) {
             const uint32_t sa = smem_base + stage * STAGE_BYTES;
             mbar_wait(empty_bar(stage), phase ^ 1u);
             mbar_arrive_expect_tx(full_bar(stage), STAGE_BYTES);
-            tma_load_3d(sa, &tmap_a, full_bar(stage), kc * BK, m_tile * BM, b);
-            tma_load_3d(sa + A_BYTES, &tmap_b, full_bar(stage), kc * BK, nt * BN, b);
+            if constexpr (TAIL) {
+              if (kc < wk.k_chunks) {
+                tma_load_3d(sa, &tmap_a, full_bar(stage), kc * BK, m_tile * BM, b);
+                tma_load_3d(sa + A_BYTES, &tmap_b, full_bar(stage), kc * BK, nt * BN, b);
+              } else {
+                const int kt = kc - wk.k_chunks;
+                tma_load_3d(sa, &tail.t, full_bar(stage), kt * BK, m_tile * BM, b);
+                tma_load_3d(sa + A_BYTES, &tail.u, full_bar(stage), kt * BK, nt * BN, b);
+              }
+            } else {
+              tma_load_3d(sa, &tmap_a, full_bar(stage), kc * BK, m_tile * BM, b);
+              tma_load_3d(sa + A_BYTES, &tmap_b, full_bar(stage), kc * BK, nt * BN, b);
+            }
             if (++stage == STAGES) { stage = 0; phase ^= 1u; }
           }
         }
@@ -223,7 +256,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       for (int nt = nt0; nt < nt1; ++nt) {
         // one wgmma group stays in flight: the stage of chunk kc - 1 is released once chunk kc has been issued
         int prev = -1;
-        for (int kc = 0; kc < wk.k_chunks; ++kc) {
+        const int kn = TAIL ? wk.k_chunks + wk.t_chunks : wk.k_chunks;
+        for (int kc = 0; kc < kn; ++kc) {
           mbar_wait(full_bar(stage), phase);
           const uint32_t sa = smem_base + stage * STAGE_BYTES;
           const uint64_t adesc = wgmma_desc_sw128_kmajor(sa + cg * 64 * 128);
@@ -262,9 +296,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   }
 }
 
-template <class Epi>
-inline int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Work& wk, const Epi& epi, int sms,
-                  cudaStream_t stream) {
+template <class Epi, bool TAIL>
+inline int launch_impl(const CUtensorMap& ta, const CUtensorMap& tb, const TailMaps<TAIL>& tail, const Work& wk,
+                       const Epi& epi, int sms, cudaStream_t stream) {
   using C = Cfg<Epi::SCRATCH_PER_WARP>;
   const size_t smem = C::SMEM_BYTES;
   // shared-memory opt-in: once per instantiation and device (a per-function, per-device attribute; immutable afterwards)
@@ -273,14 +307,39 @@ inline int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Work& wk, 
   int rc = cuda_rc(cudaGetDevice(&dev));
   if (rc) return rc;
   if (dev < 0 || dev >= 64 || !opted[dev]) {
-    rc = cuda_rc(cudaFuncSetAttribute(gemm_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    rc = cuda_rc(cudaFuncSetAttribute(gemm_kernel<Epi, TAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       static_cast<int>(smem)));
     if (rc) return rc;
     if (dev >= 0 && dev < 64) opted[dev] = true;
   }
   const int grid = wk.total < sms ? wk.total : sms;
-  gemm_kernel<Epi><<<grid, THREADS, smem, stream>>>(ta, tb, wk, epi);
+  gemm_kernel<Epi, TAIL><<<grid, THREADS, smem, stream>>>(ta, tb, tail, wk, epi);
   return launch_rc();
+}
+
+template <class Epi>
+inline int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Work& wk, const Epi& epi, int sms,
+                  cudaStream_t stream) {
+  return launch_impl<Epi, false>(ta, tb, TailMaps<false>{}, wk, epi, sms, stream);
+}
+
+// With the K tail: tt / tu from make_tail.
+template <class Epi>
+inline int launch_tail(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tt, const CUtensorMap& tu,
+                       const Work& wk, const Epi& epi, int sms, cudaStream_t stream) {
+  return launch_impl<Epi, true>(ta, tb, TailMaps<true>{tt, tu}, wk, epi, sms, stream);
+}
+
+// The K tail of a GEMM with M rows and N columns: T [M, R] and U [N, R] fp16 (R % 8 == 0, 16-byte aligned), and the
+// tail's chunk count in wk (after wk.plan).
+inline int make_tail(const void* t_dev, const void* u_dev, int R, int M, int N, CUtensorMap* tt, CUtensorMap* tu,
+                     Work* wk) {
+  int rc = make_tmap_3d_f16(tt, t_dev, R, M, 1, R, static_cast<uint64_t>(M) * R, BK, BM);
+  if (rc) return rc;
+  rc = make_tmap_3d_f16(tu, u_dev, R, N, 1, R, static_cast<uint64_t>(N) * R, BK, BN);
+  if (rc) return rc;
+  wk->t_chunks = (R + BK - 1) / BK;
+  return 0;
 }
 
 inline int device_sms(int* sms) { return cached_sm_count(sms); }

@@ -212,13 +212,30 @@ struct GegluEpi {
 
 namespace vtm {
 namespace {
-int linear_impl(const void* a_dev, const void* w_dev, const void* bias_dev, const void* resid_dev, long long ldr,
-                int M, int N, int K, void* d_dev, long long ldd, cudaStream_t stream) {
+// Argument checks of the store GEMM (linear_impl) and of the GEGLU GEMM (geglu_impl), also run by the LoRA entry points
+// before their first launch.
+int linear_args(const void* a_dev, const void* w_dev, const void* resid_dev, long long ldr, int M, int N, int K,
+                const void* d_dev, long long ldd) {
   if (!a_dev || !w_dev || !d_dev) return VTM_E_NULL;
   if (M <= 0 || N <= 0 || K <= 0 || (K % 8) != 0 || (N % 8) != 0 || (ldd % 8) != 0 || ldd < N) return VTM_E_SHAPE;
   if (resid_dev && ((ldr % 8) != 0 || ldr < N)) return VTM_E_SHAPE;
+  return VTM_OK;
+}
+
+int geglu_args(const void* a_dev, const void* w_il_dev, int M, int N, int K, const void* d_dev, long long ldd) {
+  if (!a_dev || !w_il_dev || !d_dev) return VTM_E_NULL;
+  if (M <= 0 || N <= 0 || K <= 0 || (K % 8) != 0 || (N % 64) != 0 || (ldd % 8) != 0 || ldd < N / 2) return VTM_E_SHAPE;
+  return VTM_OK;
+}
+
+// t_dev / u_dev / R: the K tail (T [M, R], U [N, R]); R == 0 runs the plain mainloop
+int linear_impl(const void* a_dev, const void* w_dev, const void* bias_dev, const void* resid_dev, long long ldr,
+                int M, int N, int K, void* d_dev, long long ldd, cudaStream_t stream, const void* t_dev = nullptr,
+                const void* u_dev = nullptr, int R = 0) {
+  int rc = linear_args(a_dev, w_dev, resid_dev, ldr, M, N, K, d_dev, ldd);
+  if (rc) return rc;
   int sms = 0;
-  int rc = gemm::device_sms(&sms);
+  rc = gemm::device_sms(&sms);
   if (rc) return rc;
   StoreEpi epi;
   epi.d = static_cast<__half*>(d_dev);
@@ -233,7 +250,57 @@ int linear_impl(const void* a_dev, const void* w_dev, const void* bias_dev, cons
   gemm::Work wk;
   wk.plan(M, N, K, 1, sms, 16, 1);
   wk.n_fastest = 1;
-  return gemm::launch<StoreEpi>(ta, tb, wk, epi, sms, stream);
+  if (R == 0) return gemm::launch<StoreEpi>(ta, tb, wk, epi, sms, stream);
+  CUtensorMap tt, tu;
+  rc = gemm::make_tail(t_dev, u_dev, R, M, N, &tt, &tu, &wk);
+  if (rc) return rc;
+  return gemm::launch_tail<StoreEpi>(ta, tb, tt, tu, wk, epi, sms, stream);
+}
+
+int geglu_impl(const void* a_dev, const void* w_il_dev, const void* bias_il_dev, int M, int N, int K, void* d_dev,
+               long long ldd, cudaStream_t stream, const void* t_dev = nullptr, const void* u_il_dev = nullptr,
+               int R = 0) {
+  int rc = geglu_args(a_dev, w_il_dev, M, N, K, d_dev, ldd);
+  if (rc) return rc;
+  int sms = 0;
+  rc = gemm::device_sms(&sms);
+  if (rc) return rc;
+  GegluEpi epi;
+  epi.d = static_cast<__half*>(d_dev);
+  epi.bias = static_cast<const __half*>(bias_il_dev);
+  epi.ldd = ldd; epi.M = M; epi.N = N; epi.row0 = 0; epi.scratch = 0;
+  CUtensorMap ta, tb;
+  rc = make_tmap_3d_f16(&ta, a_dev, K, M, 1, K, static_cast<uint64_t>(M) * K, gemm::BK, gemm::BM);
+  if (rc) return rc;
+  rc = make_tmap_3d_f16(&tb, w_il_dev, K, N, 1, K, static_cast<uint64_t>(N) * K, gemm::BK, gemm::BN);
+  if (rc) return rc;
+  gemm::Work wk;
+  wk.plan(M, N, K, 1, sms, 16, 1);
+  wk.n_fastest = 1;
+  if (R == 0) return gemm::launch<GegluEpi>(ta, tb, wk, epi, sms, stream);
+  CUtensorMap tt, tu;
+  rc = gemm::make_tail(t_dev, u_il_dev, R, M, N, &tt, &tu, &wk);
+  if (rc) return rc;
+  return gemm::launch_tail<GegluEpi>(ta, tb, tt, tu, wk, epi, sms, stream);
+}
+
+// Checks a LoRA descriptor and its workspace for a GEMM with M rows; *R_out = its rank (0 for no LoRA).
+int lora_args(const vtm_lora_t* lora, int M, const void* ws_dev, size_t ws_bytes, int* R_out) {
+  *R_out = 0;
+  if (!lora || lora->R == 0) return VTM_OK;
+  if (!lora->down_dev || !lora->up_dev || !ws_dev) return VTM_E_NULL;
+  if (lora->R < 0 || lora->R % 8 != 0) return VTM_E_SHAPE;
+  if (ws_bytes < vtm_linear_lora_workspace_bytes(M, lora->R)) return VTM_E_WS;
+  // T and U are read through tensor maps: 16-byte aligned (D is checked when its map is made, before any launch)
+  if (reinterpret_cast<uintptr_t>(ws_dev) % 16 != 0 || reinterpret_cast<uintptr_t>(lora->up_dev) % 16 != 0)
+    return VTM_E_SHAPE;
+  *R_out = lora->R;
+  return VTM_OK;
+}
+
+// T = fp16(a D^T) [M, R] into the workspace, for the K tail of a LoRA-adapted projection (arguments checked).
+int lora_down(const vtm_lora_t* lora, const void* a_dev, int M, int K, void* ws_dev, cudaStream_t stream) {
+  return linear_impl(a_dev, lora->down_dev, nullptr, nullptr, 0, M, lora->R, K, ws_dev, lora->R, stream);
 }
 }  // namespace
 }  // namespace vtm
@@ -252,24 +319,45 @@ extern "C" int vtm_linear_residual_f16(const void* a_dev, const void* w_dev, con
 
 extern "C" int vtm_linear_geglu_f16(const void* a_dev, const void* w_il_dev, const void* bias_il_dev, int32_t M,
                                     int32_t N, int32_t K, void* d_dev, int64_t ldd, void* stream_) {
+  return vtm::geglu_impl(a_dev, w_il_dev, bias_il_dev, M, N, K, d_dev, ldd, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" size_t vtm_linear_lora_workspace_bytes(int32_t M, int32_t R) {
+  if (M <= 0 || R <= 0) return 0;
+  return static_cast<size_t>(M) * R * 2;
+}
+
+extern "C" int vtm_linear_lora_f16(const void* a_dev, const void* w_dev, const void* bias_dev, const void* resid_dev,
+                                   int64_t ldr, const vtm_lora_t* lora, int32_t M, int32_t N, int32_t K, void* d_dev,
+                                   int64_t ldd, void* ws_dev, size_t ws_bytes, void* stream_) {
   using namespace vtm;
-  if (!a_dev || !w_il_dev || !d_dev) return VTM_E_NULL;
-  if (M <= 0 || N <= 0 || K <= 0 || (K % 8) != 0 || (N % 64) != 0 || (ldd % 8) != 0 || ldd < N / 2) return VTM_E_SHAPE;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  int sms = 0;
-  int rc = gemm::device_sms(&sms);
+  int rc = linear_args(a_dev, w_dev, resid_dev, ldr, M, N, K, d_dev, ldd);
   if (rc) return rc;
-  GegluEpi epi;
-  epi.d = static_cast<__half*>(d_dev);
-  epi.bias = static_cast<const __half*>(bias_il_dev);
-  epi.ldd = ldd; epi.M = M; epi.N = N; epi.row0 = 0; epi.scratch = 0;
-  CUtensorMap ta, tb;
-  rc = make_tmap_3d_f16(&ta, a_dev, K, M, 1, K, static_cast<uint64_t>(M) * K, gemm::BK, gemm::BM);
+  int R = 0;
+  rc = lora_args(lora, M, ws_dev, ws_bytes, &R);
   if (rc) return rc;
-  rc = make_tmap_3d_f16(&tb, w_il_dev, K, N, 1, K, static_cast<uint64_t>(N) * K, gemm::BK, gemm::BN);
+  if (R) {
+    rc = lora_down(lora, a_dev, M, K, ws_dev, stream);
+    if (rc) return rc;
+  }
+  return linear_impl(a_dev, w_dev, bias_dev, resid_dev, ldr, M, N, K, d_dev, ldd, stream, ws_dev,
+                     R ? lora->up_dev : nullptr, R);
+}
+
+extern "C" int vtm_linear_geglu_lora_f16(const void* a_dev, const void* w_il_dev, const void* bias_il_dev,
+                                         const vtm_lora_t* lora, int32_t M, int32_t N, int32_t K, void* d_dev,
+                                         int64_t ldd, void* ws_dev, size_t ws_bytes, void* stream_) {
+  using namespace vtm;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int rc = geglu_args(a_dev, w_il_dev, M, N, K, d_dev, ldd);
   if (rc) return rc;
-  gemm::Work wk;
-  wk.plan(M, N, K, 1, sms, 16, 1);
-  wk.n_fastest = 1;
-  return gemm::launch<GegluEpi>(ta, tb, wk, epi, sms, stream);
+  int R = 0;
+  rc = lora_args(lora, M, ws_dev, ws_bytes, &R);
+  if (rc) return rc;
+  if (R) {
+    rc = lora_down(lora, a_dev, M, K, ws_dev, stream);
+    if (rc) return rc;
+  }
+  return geglu_impl(a_dev, w_il_dev, bias_il_dev, M, N, K, d_dev, ldd, stream, ws_dev, R ? lora->up_dev : nullptr, R);
 }

@@ -335,6 +335,24 @@ def unmerge_add(y: torch.Tensor, row_map: torch.Tensor, resid: Optional[torch.Te
     return out
 
 
+def _lora_arg(lora, K: int, N: int, name: str):
+    """lora = None or (down [R, K], up [N, R]) fp16 CUDA tensors (lora.pack) -> (VtmLora or None, R)."""
+    if lora is None:
+        return None, 0
+    down, up = lora
+    _require(down, torch.float16, f"{name} lora down")
+    _require(up, torch.float16, f"{name} lora up")
+    R = down.shape[0]
+    if tuple(down.shape) != (R, K) or tuple(up.shape) != (N, R) or R % 8 != 0:
+        raise RuntimeError(f"vidtome_b200: {name} LoRA must be down [R, {K}] and up [{N}, R] with R % 8 == 0, got "
+                           f"{tuple(down.shape)} and {tuple(up.shape)}")
+    return _lib.VtmLora(down.data_ptr(), up.data_ptr(), R), R
+
+
+def _lora_ref(desc):
+    return None if desc is None else C.byref(desc)
+
+
 def linear(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
     """D = A W^T (+ bias) on the wgmma GEMM.  a [M, K], w [N, K] fp16."""
     _require(a, torch.float16, "a")
@@ -350,8 +368,10 @@ def linear(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     return d
 
 
-def linear_residual(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], resid: torch.Tensor) -> torch.Tensor:
-    """D = (A W^T + bias) + resid, with torch's fp16 roundings (`lin(x) + h`).  a [M, K], w [N, K], resid [M, N]."""
+def linear_residual(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], resid: torch.Tensor,
+                    lora=None) -> torch.Tensor:
+    """D = (A W^T + bias) + resid, with torch's fp16 roundings (`lin(x) + h`).  a [M, K], w [N, K], resid [M, N].
+    lora = (down [R, K], up [N, R]) adds the LoRA term T up^T, T = fp16(A down^T), inside the projection's sum."""
     _require(a, torch.float16, "a")
     _require(w, torch.float16, "w")
     _require(resid, torch.float16, "resid")
@@ -362,6 +382,17 @@ def linear_residual(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tenso
     d = torch.empty((M, N), dtype=torch.float16, device=a.device)
     if bias is not None:
         _require(bias, torch.float16, "bias")
+    desc, R = _lora_arg(lora, K, N, "linear_residual")
+    if desc is not None:
+        lib = _lib.load()
+        ws_bytes = lib.vtm_linear_lora_workspace_bytes(M, R)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=a.device)
+        with _Timed("FF2", 2.0 * M * (N + R) * K + 2.0 * M * N * R, 2.0 * (M * K + N * K + 2 * M * N)):
+            check(lib.vtm_linear_lora_f16(a.data_ptr(), w.data_ptr(), _ptr(bias), resid.data_ptr(), N, C.byref(desc), M,
+                                          N, K, d.data_ptr(), N, ws.data_ptr(), ws_bytes, _stream()),
+                  "vtm_linear_lora_f16")
+        STATS.launches += 2
+        return d
     with _Timed("FF2", 2.0 * M * N * K, 2.0 * (M * K + N * K + 2 * M * N)):
         check(_lib.load().vtm_linear_residual_f16(a.data_ptr(), w.data_ptr(), _ptr(bias), resid.data_ptr(), N, M, N, K,
                                                   d.data_ptr(), N, _stream()), "vtm_linear_residual_f16")
@@ -382,8 +413,9 @@ def interleave_geglu(w: torch.Tensor, bias: Optional[torch.Tensor]):
     return wi, bi
 
 
-def linear_geglu(a: torch.Tensor, w_il: torch.Tensor, bias_il: Optional[torch.Tensor]) -> torch.Tensor:
-    """GEGLU projection: [h | gate] = A W^T + b, D = h * gelu(gate).  w_il / bias_il interleaved (interleave_geglu)."""
+def linear_geglu(a: torch.Tensor, w_il: torch.Tensor, bias_il: Optional[torch.Tensor], lora=None) -> torch.Tensor:
+    """GEGLU projection: [h | gate] = A W^T + b, D = h * gelu(gate).  w_il / bias_il interleaved (interleave_geglu).
+    lora = (down [R, K], up [N, R]) with up's rows interleaved like w_il: the LoRA term joins the projection's sum."""
     _require(a, torch.float16, "a")
     _require(w_il, torch.float16, "w_il")
     M, K = a.shape
@@ -391,6 +423,17 @@ def linear_geglu(a: torch.Tensor, w_il: torch.Tensor, bias_il: Optional[torch.Te
     d = torch.empty((M, N // 2), dtype=torch.float16, device=a.device)
     if bias_il is not None:
         _require(bias_il, torch.float16, "bias_il")
+    desc, R = _lora_arg(lora, K, N, "linear_geglu")
+    if desc is not None:
+        lib = _lib.load()
+        ws_bytes = lib.vtm_linear_lora_workspace_bytes(M, R)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=a.device)
+        with _Timed("FF1", 2.0 * M * (N + R) * K + 2.0 * M * N * R, 2.0 * (M * K + N * K + M * N // 2)):
+            check(lib.vtm_linear_geglu_lora_f16(a.data_ptr(), w_il.data_ptr(), _ptr(bias_il), C.byref(desc), M, N, K,
+                                                d.data_ptr(), N // 2, ws.data_ptr(), ws_bytes, _stream()),
+                  "vtm_linear_geglu_lora_f16")
+        STATS.launches += 2
+        return d
     with _Timed("FF1", 2.0 * M * N * K, 2.0 * (M * K + N * K + M * N // 2)):
         check(_lib.load().vtm_linear_geglu_f16(a.data_ptr(), w_il.data_ptr(), _ptr(bias_il), M, N, K, d.data_ptr(), N // 2,
                                                _stream()), "vtm_linear_geglu_f16")
@@ -405,15 +448,33 @@ def layer_norm(x: torch.Tensor, ln) -> torch.Tensor:
 
 
 def attention(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, b_o: Optional[torch.Tensor], heads: int,
-              scale: float, shared_qk: bool = False, seq_len: Optional[torch.Tensor] = None) -> torch.Tensor:
+              scale: float, shared_qk: bool = False, seq_len: Optional[torch.Tensor] = None, lora_qkv=None,
+              lora_o=None) -> torch.Tensor:
     """KD.  x [B, L, C] fp16 -> [B, L, C].  shared_qk: PnP injection — the attention map of sample 0 for every sample.
     seq_len: a 1-element int32 CUDA tensor; the sequence is then the first seq_len rows of x (rows past it must be
-    finite) and only those rows of the result are defined."""
+    finite) and only those rows of the result are defined.  lora_qkv = (down [R, C], up [3C, R]) and lora_o =
+    (down [R, C], up [C, R]): LoRA terms of the QKV GEMM and of to_out[0] (vtm_attention_lora)."""
     _require(x, torch.float16, "x")
     _require(w_qkv, torch.float16, "w_qkv")
     _require(w_o, torch.float16, "w_o")
     B, L, Cc = x.shape
     lib = _lib.load()
+    if lora_qkv is not None or lora_o is not None:
+        dq, rq = _lora_arg(lora_qkv, Cc, 3 * Cc, "attention qkv")
+        do, ro = _lora_arg(lora_o, Cc, Cc, "attention out")
+        ws_bytes = lib.vtm_attention_lora_workspace_bytes(B, L, Cc, heads, rq, ro)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        y = torch.empty_like(x)
+        if seq_len is not None:
+            _require(seq_len, torch.int32, "seq_len")
+        flops = 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc + 8.0 * B * L * Cc * (rq + ro)
+        with _Timed("KD", flops, 4.0 * B * L * Cc + 8.0 * Cc * Cc):
+            check(lib.vtm_attention_lora(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), _lora_ref(dq),
+                                         _lora_ref(do), B, L, Cc, heads, float(scale), 1 if shared_qk else 0,
+                                         _ptr(seq_len), y.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
+                  "vtm_attention_lora")
+        STATS.launches += 3 + (rq > 0) + (ro > 0)
+        return y
     ws_bytes = lib.vtm_attention_workspace_bytes(B, L, Cc, heads)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
     y = torch.empty_like(x)
@@ -434,8 +495,11 @@ def attention(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, b_o: Opti
 
 
 def cross_attention(x: torch.Tensor, ctx: torch.Tensor, w_q: torch.Tensor, w_kv: torch.Tensor, w_o: torch.Tensor,
-                    b_o: Optional[torch.Tensor], heads: int, scale: float, resid: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """attn2 of the block: x [B, Lq, C] queries, ctx [B, Lk, Cctx] keys/values; returns o Wo^T + bo (+ resid)."""
+                    b_o: Optional[torch.Tensor], heads: int, scale: float, resid: Optional[torch.Tensor] = None,
+                    lora_q=None, lora_kv=None, lora_o=None) -> torch.Tensor:
+    """attn2 of the block: x [B, Lq, C] queries, ctx [B, Lk, Cctx] keys/values; returns o Wo^T + bo (+ resid).
+    lora_q = (down [R, C], up [C, R]), lora_kv = (down [R, Cctx], up [2C, R]), lora_o = (down [R, C], up [C, R]): LoRA
+    terms of to_q, to_k / to_v and to_out[0] (vtm_cross_attention_lora)."""
     _require(x, torch.float16, "x")
     _require(ctx, torch.float16, "ctx")
     _require(w_q, torch.float16, "w_q")
@@ -448,10 +512,25 @@ def cross_attention(x: torch.Tensor, ctx: torch.Tensor, w_q: torch.Tensor, w_kv:
     if resid is not None:
         _require(resid, torch.float16, "resid")
     lib = _lib.load()
+    flops = 4.0 * B * Lq * Lk * Cc + 4.0 * B * Lq * Cc * Cc + 4.0 * B * Lk * Cctx * Cc
+    if lora_q is not None or lora_kv is not None or lora_o is not None:
+        dq, rq = _lora_arg(lora_q, Cc, Cc, "cross_attention q")
+        dkv, rkv = _lora_arg(lora_kv, Cctx, 2 * Cc, "cross_attention kv")
+        do, ro = _lora_arg(lora_o, Cc, Cc, "cross_attention out")
+        ws_bytes = lib.vtm_cross_attention_lora_workspace_bytes(B, Lq, Lk, Cc, heads, rq, rkv, ro)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        y = torch.empty_like(x)
+        flops += 4.0 * B * Lq * Cc * (rq + ro) + 2.0 * B * Lk * (Cctx + 2 * Cc) * rkv
+        with _Timed("XA", flops, 2.0 * B * Lq * Cc * (3 if resid is not None else 2)):
+            check(lib.vtm_cross_attention_lora(x.data_ptr(), ctx.data_ptr(), w_q.data_ptr(), w_kv.data_ptr(),
+                                               w_o.data_ptr(), _ptr(b_o), _ptr(resid), _lora_ref(dq), _lora_ref(dkv),
+                                               _lora_ref(do), B, Lq, Lk, Cc, Cctx, heads, float(scale), y.data_ptr(),
+                                               ws.data_ptr(), ws_bytes, _stream()), "vtm_cross_attention_lora")
+        STATS.launches += 4 + (rq > 0) + (rkv > 0) + (ro > 0)
+        return y
     ws_bytes = lib.vtm_cross_attention_workspace_bytes(B, Lq, Lk, Cc, heads)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
     y = torch.empty_like(x)
-    flops = 4.0 * B * Lq * Lk * Cc + 4.0 * B * Lq * Cc * Cc + 4.0 * B * Lk * Cctx * Cc
     with _Timed("XA", flops, 2.0 * B * Lq * Cc * (3 if resid is not None else 2)):
         check(lib.vtm_cross_attention(x.data_ptr(), ctx.data_ptr(), w_q.data_ptr(), w_kv.data_ptr(), w_o.data_ptr(), _ptr(b_o),
                                       _ptr(resid), B, Lq, Lk, Cc, Cctx, heads, float(scale), y.data_ptr(), ws.data_ptr(),

@@ -22,6 +22,7 @@ import torch
 
 from . import merge, ops
 from ._lib import VtmSplit
+from .lora import linear_parts
 from .utils import (draw_coin, draw_randf, func_warper, init_generator, isinstance_str, join_frame, join_warper,
                     split_frame, split_warper)
 
@@ -361,8 +362,9 @@ _PLAIN_PROCESSORS = ("AttnProcessor", "AttnProcessor2_0", "XFormersAttnProcessor
 
 def _plain_attention_module(attn: torch.nn.Module) -> bool:
     """True only if replacing `attn.forward` by KD cannot change the result: `attn` is a stock diffusers-style
-    Attention whose projections are bare `torch.nn.Linear` (exact type: LoRA-compatible or PEFT-wrapped layers
-    carry extra terms and still expose `.weight`), to_q/to_k/to_v without bias, to_out = [Linear, Dropout(inactive)],
+    Attention whose projections are bare `torch.nn.Linear` or LoRA-adapted layers that lora.linear_parts reads (their
+    low-rank terms then run as extra K steps of KD's projection GEMMs; any other subclass or wrapper carries terms KD
+    would miss), to_q/to_k/to_v without bias, to_out = [Linear, Dropout(inactive)],
     no instance-level forward override (PnP installs one, utils/pnp_utils.py:99-101), no forward hooks, a default
     attention processor (or none), and none of the Attention options that alter the math (group / spatial norm,
     residual connection, output rescale, added KV projections).  Anything else goes through `self.attn1(...)`
@@ -377,9 +379,10 @@ def _plain_attention_module(attn: torch.nn.Module) -> bool:
     if not isinstance(to_out, (torch.nn.ModuleList, torch.nn.Sequential)) or len(to_out) < 1:
         return False
     linears = (attn.to_q, attn.to_k, attn.to_v, to_out[0])
-    if any(type(m) is not torch.nn.Linear for m in linears):
+    parts = [linear_parts(m) for m in linears]
+    if any(p is None for p in parts):
         return False
-    if any(m.bias is not None for m in linears[:3]):
+    if any(p[1] is not None for p in parts[:3]):
         return False
     for m in (attn,) + linears + tuple(to_out[1:]):
         if m._forward_hooks or m._forward_pre_hooks or getattr(m, "_forward_hooks_with_kwargs", None):
@@ -398,10 +401,11 @@ def _plain_attention_module(attn: torch.nn.Module) -> bool:
         return False
     if getattr(attn, "added_kv_proj_dim", None) is not None or getattr(attn, "add_k_proj", None) is not None:
         return False
-    C = attn.to_q.weight.shape[1]
-    if attn.to_q.weight.shape[0] != C or attn.to_k.weight.shape != attn.to_q.weight.shape:
+    wq, wk, wv, wo = (p[0] for p in parts)
+    C = wq.shape[1]
+    if wq.shape[0] != C or wk.shape != wq.shape:
         return False                       # inner dim != query dim or cross-attention shaped K/V
-    if attn.to_v.weight.shape != attn.to_q.weight.shape or to_out[0].weight.shape != (C, C):
+    if wv.shape != wq.shape or wo.shape != (C, C):
         return False
     from .attention import max_head_dim
     head_dim = C // int(attn.heads)

@@ -98,6 +98,162 @@ class BasicTransformerBlock(nn.Module):
         return hidden_states
 
 
+class LoRALinearLayer(nn.Module):
+    """diffusers' LoRALinearLayer (the adapter of LoRACompatibleLinear): up(down(x)), times network_alpha / rank when
+    network_alpha is set, computed in the adapter's dtype and cast back to the input's."""
+
+    def __init__(self, in_features: int, out_features: int, rank: int, network_alpha: Optional[float] = None):
+        super().__init__()
+        self.down = nn.Linear(in_features, rank, bias=False)
+        self.up = nn.Linear(rank, out_features, bias=False)
+        self.network_alpha = network_alpha
+        self.rank = rank
+
+    def forward(self, hidden_states):
+        orig_dtype = hidden_states.dtype
+        up = self.up(self.down(hidden_states.to(self.down.weight.dtype)))
+        if self.network_alpha is not None:
+            up = up * (self.network_alpha / self.rank)
+        return up.to(orig_dtype)
+
+
+class LoRACompatibleLinear(nn.Linear):
+    """diffusers' LoRACompatibleLinear: an nn.Linear whose forward adds `scale * lora_layer(x)` when it has one."""
+
+    def __init__(self, *args, lora_layer: Optional[LoRALinearLayer] = None, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.lora_layer = lora_layer
+
+    def forward(self, hidden_states, scale: float = 1.0):
+        if self.lora_layer is None:
+            return super().forward(hidden_states)
+        return super().forward(hidden_states) + scale * self.lora_layer(hidden_states)
+
+
+class PeftLoraLinear(nn.Module):
+    """peft's lora.Linear: `base_layer` plus, per active adapter, lora_B(lora_A(dropout(x))) * scaling, each adapter
+    computed in its own dtype, and the sum cast back to the base layer's output dtype."""
+
+    def __init__(self, base_layer: nn.Linear):
+        super().__init__()
+        self.base_layer = base_layer
+        self.lora_A = nn.ModuleDict()
+        self.lora_B = nn.ModuleDict()
+        self.lora_dropout = nn.ModuleDict()
+        self.scaling = {}
+        self.use_dora = {}
+        self.lora_bias = {}
+        self.fan_in_fan_out = False
+        self._active_adapter = []
+        self._disable_adapters = False
+        self.merged_adapters = []
+
+    def update_layer(self, name: str, r: int, lora_alpha: float, dropout: float = 0.0):
+        self.lora_A[name] = nn.Linear(self.base_layer.in_features, r, bias=False)
+        self.lora_B[name] = nn.Linear(r, self.base_layer.out_features, bias=False)
+        self.lora_dropout[name] = nn.Dropout(dropout) if dropout > 0 else nn.Identity()
+        self.scaling[name] = lora_alpha / r
+        self.use_dora[name] = False
+        self.lora_bias[name] = False
+        if name not in self._active_adapter:
+            self._active_adapter.append(name)
+
+    @property
+    def weight(self):
+        return self.base_layer.weight
+
+    @property
+    def bias(self):
+        return self.base_layer.bias
+
+    @property
+    def active_adapters(self):
+        return list(self._active_adapter)
+
+    def set_adapter(self, names):
+        self._active_adapter = [names] if isinstance(names, str) else list(names)
+
+    @property
+    def disable_adapters(self) -> bool:
+        return self._disable_adapters
+
+    @property
+    def merged(self) -> bool:
+        return bool(self.merged_adapters)
+
+    def forward(self, x):
+        result = self.base_layer(x)
+        if self.disable_adapters or self.merged:
+            return result
+        torch_result_dtype = result.dtype
+        for name in self.active_adapters:
+            if name not in self.lora_A:
+                continue
+            lora_A = self.lora_A[name]
+            xa = x.to(lora_A.weight.dtype)
+            result = result + self.lora_B[name](lora_A(self.lora_dropout[name](xa))) * self.scaling[name]
+        return result.to(torch_result_dtype)
+
+
+LORA_TARGETS = ("to_q", "to_k", "to_v", "to_out", "ff")
+
+
+def add_lora(net: nn.Module, rank: int, form: str = "peft", targets=LORA_TARGETS, dtype=None, seed: int = 7,
+             attns=("attn1", "attn2")) -> nn.Module:
+    """Wrap the chosen projections of every BasicTransformerBlock in `net` (a skeleton UNet or ControlNet) with one
+    seeded LoRA adapter of `rank`, as `load_lora_weights` does: form "diffusers" (LoRACompatibleLinear with a
+    LoRALinearLayer, network_alpha = rank / 2) or "peft" (PeftLoraLinear, adapter "default", lora_alpha = rank / 2).
+    targets: any of "to_q", "to_k", "to_v", "to_out" (to_out[0]) of the `attns` modules, and "ff" (both Linear layers of
+    the feed-forward).  Adapter weights are drawn so that the LoRA term is a sizeable fraction of the projection's
+    output (lora_B is not zero-initialised), in `dtype` (default: the base weight's)."""
+    if form not in ("diffusers", "peft"):
+        raise ValueError(f"add_lora: form must be 'diffusers' or 'peft', got {form!r}")
+    gen = torch.Generator().manual_seed(seed)
+
+    def wrap(lin: nn.Linear) -> nn.Module:
+        w = lin.weight
+        dt = dtype or w.dtype
+        K, N = lin.in_features, lin.out_features
+        a = torch.randn((rank, K), generator=gen) * K ** -0.5
+        b = torch.randn((N, rank), generator=gen) * (0.5 * rank ** -0.5)
+        if form == "diffusers":
+            layer = LoRALinearLayer(K, N, rank, network_alpha=rank / 2)
+            new = LoRACompatibleLinear(K, N, bias=lin.bias is not None, lora_layer=layer)
+            with torch.no_grad():
+                new.weight.copy_(lin.weight.cpu())
+                if lin.bias is not None:
+                    new.bias.copy_(lin.bias.cpu())
+                layer.down.weight.copy_(a)
+                layer.up.weight.copy_(b)
+            new = new.to(device=w.device, dtype=w.dtype)
+            layer.to(dtype=dt)
+            return new
+        new = PeftLoraLinear(lin)
+        new.update_layer("default", rank, rank / 2)
+        with torch.no_grad():
+            new.lora_A["default"].weight.copy_(a)
+            new.lora_B["default"].weight.copy_(b)
+        new.lora_A.to(device=w.device, dtype=dt)
+        new.lora_B.to(device=w.device, dtype=dt)
+        return new
+
+    for block in [m for m in net.modules() if type(m).__name__ in ("BasicTransformerBlock", "ToMeBlock")]:
+        for an in attns:
+            attn = getattr(block, an, None)
+            if attn is None:
+                continue
+            for t in ("to_q", "to_k", "to_v"):
+                if t in targets:
+                    setattr(attn, t, wrap(getattr(attn, t)))
+            if "to_out" in targets:
+                attn.to_out[0] = wrap(attn.to_out[0])
+        ff = getattr(block, "ff", None)
+        if ff is not None and "ff" in targets:
+            ff.proj = wrap(ff.proj)
+            ff.out = wrap(ff.out)
+    return net
+
+
 class ModelMixin(nn.Module):
     """Name-only stand-in for diffusers.ModelMixin (patch.py:279-280 matches the class name)."""
 
