@@ -399,6 +399,23 @@ int vtm_cross_attention_lora(const void* x_dev, const void* ctx_dev, const void*
                              int32_t C, int32_t Cctx, int32_t heads, float scale, void* y_dev, void* ws_dev,
                              size_t ws_bytes, void* stream);
 
+/*
+ * KT — the residual tail of PnP's feature-injected ResNet (utils/pnp_utils.py:146-162, `register_conv_control`):
+ *   out[b] = (shortcut[b] + h[src(b)]) / output_scale_factor
+ * with src(b) = b mod n for b in [n, 2n) and [2n, 3n) when `inject` is 1 (the source samples' conv2 output copied over
+ * the uncond and cond samples), and src(b) = b otherwise.
+ *   h_dev         conv2's output: [num_inputs * n, E] fp16, or only its source samples [n, E] when inject is 1
+ *   shortcut_dev  [num_inputs * n, E] fp16: conv_shortcut(input), or the input itself when the block has no shortcut
+ *   out_dev       [num_inputs * n, E] fp16;  E = sample_elems = C * H * W (any value); contiguous NCHW tensors
+ *   num_inputs    1..3 (VTM_E_UNSUPPORTED otherwise);  inject 0 or 1
+ * Rounding is that of torch's CUDA half ops: fp16(float(s) + float(h)), then fp16(float(sum) * (1.0f / osf)) (torch
+ * divides a CUDA tensor by a CPU scalar as a multiplication by the fp32 reciprocal).  output_scale_factor must be finite
+ * and non-zero (VTM_E_UNSUPPORTED).  Pointers must be 2-byte aligned (VTM_E_SHAPE); 16-byte vectors are used wherever the
+ * three streams share their offset from a 16-byte boundary.
+ */
+int vtm_resnet_tail_f16(const void* h_dev, const void* shortcut_dev, void* out_dev, int32_t n, int32_t num_inputs,
+                        int64_t sample_elems, float output_scale_factor, int32_t inject, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

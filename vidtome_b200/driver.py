@@ -6,11 +6,10 @@ Restates, on synthetic latents, the parts of the reference's Generator that sit 
   pred_noise      generate.py:238-279   (CFG batch cat([x, x]), UNet forward, guidance combine)
   pred_next_x     generate.py:281-311   (closed-form DDIM step)
   post_iter       generate.py:233-236   (reset global tokens after each step)
-  init_pnp        generate.py:313-319   (PnP self-attention injection schedule; with `source_latents`)
+  init_pnp        generate.py:313-319   (PnP self-attention and conv-feature injection schedules; with `source_latents`)
   pre_iter        generate.py:226-231   (PnP: set the timestep, fetch the source latents of the step)
   ControlNet      generate.py:56-63,264-275, utils/utils.py:280-295 (residuals of `controlnet`, with `control_images`)
-Text conditioning, VAE, ControlNet preprocessing, PnP's conv-feature injection and file IO are outside the hot path and
-not restated.
+Text conditioning, VAE, ControlNet preprocessing and file IO are outside the hot path and not restated.
 """
 from __future__ import annotations
 
@@ -45,7 +44,8 @@ class ChunkedDenoiser:
                  chunk_graphs: bool = False, source_latents: Optional[Callable[[int], torch.Tensor]] = None,
                  pnp_attn_t: float = 0.5, pnp_modules: Optional[Iterable[torch.nn.Module]] = None,
                  controlnet: Optional[torch.nn.Module] = None, control_images: Optional[torch.Tensor] = None,
-                 control_scale: float = 1.0):
+                 control_scale: float = 1.0, pnp_f_t: Optional[float] = None,
+                 pnp_conv_modules: Optional[Iterable[torch.nn.Module]] = None):
         """`cuda_graph=True`: after `graph_warmup` eager steps, the noise prediction of a whole step (every chunk:
         CFG batch, UNet forward with the merge path, guidance combine) is captured once into a CUDA graph and
         replayed; per step the host then issues one graph launch plus the DDIM update instead of ~250 kernel
@@ -80,6 +80,14 @@ class ChunkedDenoiser:
         those modules for a model without the diffusers up_blocks hierarchy).  The model must be patched with
         batch_size=3 and align_batch=True.  In every graph mode the injection is decided on the host when a graph is
         captured, so graphs are keyed by it as well; the injected ones are released once the schedule has passed.
+
+        `pnp_f_t` (with `source_latents`) adds PnP's conv-feature injection, the other half of the reference's default
+        PnP config (generate.py:64,315-319, `pnp_f_t: 0.8`): for the first int(n_timesteps * pnp_f_t) steps the ResNet
+        `unet.up_blocks[1].resnets[1]` (or `pnp_conv_modules` for a model without that hierarchy) adds the source
+        sample's conv2 output to the uncond and cond samples in place of their own (pnp.register_conv_control; on CUDA
+        fp16 its branch runs on the source samples only and the tail is one kernel).  The graph modes key their graphs
+        by both injections then: three phases (both, conv only, neither) when pnp_f_t >= pnp_attn_t.  With
+        `pnp_f_t=None` (the default) nothing of this is installed and the graph keys are those of attention-only PnP.
 
         `controlnet` with `control_images` ([flen, 3, H, W], the reference's prepare_control output) switches on
         ControlNet control (generate.py:56-63, `control: "depth"`, `"softedge"`, ...): every UNet call first runs the
@@ -123,7 +131,7 @@ class ChunkedDenoiser:
             raise ValueError("cuda_graph=True needs merge_global=False and randomize_chunks=False (static work)")
         if self.capture_global and self.shard:
             raise ValueError("capture_global=True does not capture the cross-rank exchange of shard=True")
-        # (chunk length, first in step, frame shape, PnP injection)
+        # (chunk length, first in step, frame shape, PnP injection[, PnP conv injection when pnp_f_t is set])
         #   -> (CUDAGraph, static x, static noise, static source, static control images)
         self._chunk_graphs = {}
         self._chunk_t = None        # the UNet's timestep input shared by the chunk graphs
@@ -144,10 +152,25 @@ class ChunkedDenoiser:
         self.source_latents = source_latents
         self.pnp_schedule: List[int] = []
         self._pnp_targets: List[torch.nn.Module] = []
+        if pnp_f_t is not None and source_latents is None:
+            raise ValueError("pnp_f_t (PnP conv injection) needs source_latents")
+        self.pnp_f_t = None if pnp_f_t is None else float(pnp_f_t)
+        self.pnp_conv_schedule: List[int] = []
         if source_latents is not None:
             self._init_pnp(n_timesteps, pnp_attn_t, pnp_modules)
+            if self.pnp_f_t is not None:
+                self._init_pnp_conv(n_timesteps, self.pnp_f_t, pnp_conv_modules)
 
-    # generate.py:60-68,313-319 (the attention half of init_pnp; conv injection is not restated)
+    # generate.py:64,315,318-319 (the conv half of init_pnp)
+    def _init_pnp_conv(self, n_timesteps: int, pnp_f_t: float, modules):
+        f_t = int(n_timesteps * pnp_f_t)
+        self.pnp_conv_schedule = self.timesteps[:f_t] if f_t >= 0 else []
+        if modules is None and not hasattr(getattr(self.unet, "unet", self.unet), "up_blocks"):
+            raise ValueError("pnp_f_t: the model has no up_blocks[1].resnets[1]; name the ResNet with pnp_conv_modules")
+        pnp.register_conv_control(self.unet, self.pnp_conv_schedule, num_inputs=3, modules=modules)
+        self._pnp_targets = self._pnp_targets + pnp._conv_targets(self.unet, modules)
+
+    # generate.py:60-68,313-319 (the attention half of init_pnp)
     def _init_pnp(self, n_timesteps: int, pnp_attn_t: float, modules):
         args = self.unet._tome_info["args"] if hasattr(self.unet, "_tome_info") else None
         if args is None or args["batch_size"] != 3 or not args["align_batch"]:
@@ -164,6 +187,12 @@ class ChunkedDenoiser:
     def injecting(self, t: int) -> bool:
         """True if the self-attention of step t takes its map from the source sample (pnp.injection_active)."""
         return self.source_latents is not None and (int(t) in self.pnp_schedule or int(t) == 1000)
+
+    def conv_injecting(self, t: int) -> bool:
+        """True if the controlled ResNet of step t takes the source sample's features (pnp_f_t set; the test of
+        utils/pnp_utils.py:146)."""
+        return (self.source_latents is not None and self.pnp_f_t is not None
+                and (int(t) in self.pnp_conv_schedule or int(t) == 1000))
 
     # generate.py:172-203
     def get_chunks(self, flen: int) -> List[torch.Tensor]:
@@ -268,7 +297,9 @@ class ChunkedDenoiser:
         return gens
 
     def _graph_key(self, x: torch.Tensor, t: int):
-        return tuple(x.shape), self.injecting(t)
+        if self.pnp_f_t is None:
+            return tuple(x.shape), self.injecting(t)
+        return tuple(x.shape), self.injecting(t), self.conv_injecting(t)
 
     def _capture(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor], ctrl: Optional[torch.Tensor]):
         """Capture `_all_noises` for inputs shaped like `x` (called after the eager warm-up steps, so that every
@@ -442,6 +473,10 @@ class ChunkedDenoiser:
         if not inject and any(k[3] for k in self._chunk_graphs):
             # the schedule is a prefix of the steps: the injected graphs never run again
             self._chunk_graphs = {k: v for k, v in self._chunk_graphs.items() if not k[3]}
+        conv = self.conv_injecting(t)
+        if self.pnp_f_t is not None and not conv and any(k[4] for k in self._chunk_graphs):
+            # so is the conv schedule
+            self._chunk_graphs = {k: v for k, v in self._chunk_graphs.items() if not k[4]}
         if self._chunk_t is None:
             self._chunk_t = torch.tensor(int(t), device=x.device, dtype=torch.long)
         self._chunk_t.fill_(int(t))
@@ -449,6 +484,8 @@ class ChunkedDenoiser:
         for k, chunk in enumerate(chunks):
             lo, hi = int(chunk[0]), int(chunk[-1]) + 1
             key = (hi - lo, self.merge_global and k == 0, tuple(x.shape[1:]), inject)
+            if self.pnp_f_t is not None:
+                key = key + (conv,)
             entry = self._chunk_graphs.get(key)
             if entry is None:
                 entry = self._capture_chunk(key, x[lo:hi], None if src is None else src[lo:hi],

@@ -539,6 +539,37 @@ def cross_attention(x: torch.Tensor, ctx: torch.Tensor, w_q: torch.Tensor, w_kv:
     return y
 
 
+def resnet_tail(h: torch.Tensor, shortcut: torch.Tensor, num_inputs: int, output_scale_factor: float, inject: bool,
+                out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """KT.  out = (shortcut + h') / output_scale_factor, h' = h with the first third (num_inputs = 3) or half (2) of the
+    batch copied over the next two (one) when `inject` (utils/pnp_utils.py:146-162).  shortcut [num_inputs * n, ...]
+    fp16; h like shortcut, or only its n source samples when injecting."""
+    _require(h, torch.float16, "h")
+    _require(shortcut, torch.float16, "shortcut")
+    B = shortcut.shape[0]
+    if num_inputs not in (1, 2, 3) or B % num_inputs:
+        raise RuntimeError(f"vidtome_b200: resnet_tail needs a batch of num_inputs * n samples, num_inputs in 1..3 "
+                           f"(got batch {B}, num_inputs {num_inputs})")
+    n = B // num_inputs
+    if h.shape[1:] != shortcut.shape[1:] or h.shape[0] not in ((n, B) if inject else (B,)):
+        raise RuntimeError(f"vidtome_b200: resnet_tail: h {tuple(h.shape)} does not fit shortcut {tuple(shortcut.shape)}"
+                           f" (inject={bool(inject)})")
+    if out is None:
+        out = torch.empty_like(shortcut)
+    else:
+        _require(out, torch.float16, "out")
+        if out.shape != shortcut.shape:
+            raise RuntimeError(f"vidtome_b200: resnet_tail: out {tuple(out.shape)} != shortcut {tuple(shortcut.shape)}")
+    E = shortcut[0].numel()
+    nbytes = 2.0 * E * (2 * B + (n if inject else B))
+    with _Timed("KT", 0.0, nbytes):
+        check(_lib.load().vtm_resnet_tail_f16(h.data_ptr(), shortcut.data_ptr(), out.data_ptr(), n, num_inputs, E,
+                                              float(output_scale_factor), int(bool(inject)), _stream()),
+              "vtm_resnet_tail_f16")
+    STATS.launches += 1
+    return out
+
+
 def keys_to_score_arg(keys: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """Unpack KA keys on the device with torch integer ops (test / debugging helper)."""
     o = (keys >> 32) & 0xFFFF

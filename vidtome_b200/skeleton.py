@@ -17,6 +17,7 @@ census, whose per-block residuals the skeleton UNet adds to its encoder blocks' 
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 from types import SimpleNamespace
 from typing import List, Optional, Tuple
@@ -254,6 +255,53 @@ def add_lora(net: nn.Module, rank: int, form: str = "peft", targets=LORA_TARGETS
     return net
 
 
+class ResnetBlock2D(nn.Module):
+    """diffusers' ResnetBlock2D as SD's UNet builds it: GroupNorm -> SiLU -> conv1 (3x3) -> + time embedding ->
+    GroupNorm -> SiLU -> dropout -> conv2 (3x3), plus a 1x1 conv_shortcut when the channel count changes, and
+    (shortcut + h) / output_scale_factor.  It carries every attribute the reference's PnP conv_forward reads
+    (utils/pnp_utils.py:110-164); no up- or downsampling, time_embedding_norm "default".  The GroupNorm affines are drawn
+    around (1, 0) rather than left at it, so that they take part in a comparison."""
+
+    def __init__(self, in_channels: int, out_channels: Optional[int] = None, temb_channels: Optional[int] = 1280,
+                 groups: int = 32, eps: float = 1e-5, output_scale_factor: float = 1.0, dropout: float = 0.0):
+        super().__init__()
+        out_channels = in_channels if out_channels is None else out_channels
+        self.norm1 = nn.GroupNorm(groups, in_channels, eps=eps, affine=True)
+        self.conv1 = nn.Conv2d(in_channels, out_channels, 3, padding=1)
+        self.time_emb_proj = nn.Linear(temb_channels, out_channels) if temb_channels else None
+        self.norm2 = nn.GroupNorm(groups, out_channels, eps=eps, affine=True)
+        self.dropout = nn.Dropout(dropout)
+        self.conv2 = nn.Conv2d(out_channels, out_channels, 3, padding=1)
+        self.nonlinearity = nn.SiLU()
+        self.upsample = None
+        self.downsample = None
+        self.time_embedding_norm = "default"
+        self.output_scale_factor = output_scale_factor
+        self.conv_shortcut = nn.Conv2d(in_channels, out_channels, 1) if in_channels != out_channels else None
+        with torch.no_grad():
+            for norm in (self.norm1, self.norm2):
+                norm.weight.normal_(1.0, 0.1)
+                norm.bias.normal_(0.0, 0.1)
+
+    def forward(self, input_tensor, temb, scale: float = 1.0):
+        h = self.conv1(self.nonlinearity(self.norm1(input_tensor)))
+        if temb is not None:
+            h = h + self.time_emb_proj(self.nonlinearity(temb))[:, :, None, None]
+        h = self.conv2(self.dropout(self.nonlinearity(self.norm2(h))))
+        shortcut = input_tensor if self.conv_shortcut is None else self.conv_shortcut(input_tensor)
+        return (shortcut + h) / self.output_scale_factor
+
+
+def timestep_embedding(timestep, batch: int, dim: int, device, dtype) -> torch.Tensor:
+    """diffusers' get_timestep_embedding(flip_sin_to_cos=True, downscale_freq_shift=0) of a scalar timestep (an int or a
+    0-dim / 1-element tensor, which may live on the device), broadcast to [batch, dim]."""
+    t = torch.as_tensor(timestep, device=device).reshape(-1)[:1].float()
+    half = dim // 2
+    freqs = torch.exp(torch.arange(half, dtype=torch.float32, device=device) * (-math.log(10000.0) / half))
+    args = t[:, None] * freqs[None]
+    return torch.cat([torch.cos(args), torch.sin(args)], dim=-1).to(dtype).expand(batch, dim)
+
+
 class ModelMixin(nn.Module):
     """Name-only stand-in for diffusers.ModelMixin (patch.py:279-280 matches the class name)."""
 
@@ -305,10 +353,16 @@ class SkeletonUNet(ModelMixin):
 
     `down_block_additional_residuals` / `mid_block_additional_residual` (a ControlNet's outputs) are added to the output
     state of the matching encoder block, the skeleton's stand-in for diffusers' skip-sample add: one residual per down
-    block in block order, one for the mid block, each shaped like that block's output [(B F), T, C]."""
+    block in block order, one for the mid block, each shaped like that block's output [(B F), T, C].
+
+    `pnp_conv=True` adds `resnet`, a ResnetBlock2D at the census position of diffusers' `up_blocks[1].resnets[1]` (the
+    target of PnP's conv-feature injection, utils/pnp_utils.py:168-169), run ahead of census block 8: it takes the
+    state of that resolution concatenated with a skip (the last encoder block's output there, 2C channels, as the
+    decoder's skip concatenation), gives C channels back to the state, and gets the sinusoidal embedding of the
+    timestep.  Its weights are drawn after all others, so the rest of the skeleton is the same with and without it."""
 
     def __init__(self, census: List[BlockSpec], in_channels: int = 4, cross_attention_dim: int = 768,
-                 hot_path_only: bool = True, max_downsample: Optional[int] = None):
+                 hot_path_only: bool = True, max_downsample: Optional[int] = None, pnp_conv: bool = False):
         super().__init__()
         keep = [i for i, s in enumerate(census) if max_downsample is None or s.downsample <= max_downsample]
         self.census_index = keep                  # position of every block in the full census
@@ -320,6 +374,21 @@ class SkeletonUNet(ModelMixin):
         dims = sorted({(s.downsample, s.dim) for s in self.census})
         self.lift = nn.ModuleDict({f"ds{ds}": nn.Linear(in_channels, dim) for ds, dim in dims})
         self.drop = nn.ModuleDict({f"ds{ds}": nn.Linear(dim, in_channels) for ds, dim in dims})
+        self.resnet = None
+        if pnp_conv:
+            if PNP_CONV_POSITION not in keep:
+                raise ValueError(f"pnp_conv=True needs census block {PNP_CONV_POSITION} (up_blocks[1]), which this "
+                                 f"census / max_downsample leaves out")
+            C = census[PNP_CONV_POSITION].dim
+            self.resnet = ResnetBlock2D(2 * C, C, temb_channels=TEMB_CHANNELS)
+
+    def _run_resnet(self, state: torch.Tensor, skip: torch.Tensor, timestep, hw: Tuple[int, int]) -> torch.Tensor:
+        """[(B F), T, C] state and skip -> the ResNet's [(B F), T, C] output."""
+        BF = state.shape[0]
+        nchw = lambda t: t.transpose(1, 2).reshape(BF, -1, *hw).contiguous()   # noqa: E731  (NCHW, as diffusers)
+        temb = timestep_embedding(timestep, BF, TEMB_CHANNELS, state.device, state.dtype)
+        out = self.resnet(torch.cat([nchw(state), nchw(skip)], dim=1), temb)
+        return out.flatten(2).transpose(1, 2).contiguous()
 
     def _residuals(self, down, mid) -> dict:
         """{census position: residual} of the encoder blocks; raises unless the residuals match them one-to-one."""
@@ -344,13 +413,19 @@ class SkeletonUNet(ModelMixin):
         state = {}
         eps = torch.zeros_like(sample)
         res = self._residuals(down_block_additional_residuals, mid_block_additional_residual)
+        skips = {}
         for pos, spec, block in zip(self.census_index, self.census, self.blocks):
             key = f"ds{spec.downsample}"
             if key not in state:
                 pooled = F.avg_pool2d(sample, spec.downsample) if spec.downsample > 1 else sample
                 tok = pooled.flatten(2).transpose(1, 2)                       # [(B F), T, 4]
                 state[key] = self.lift[key](tok)
+            if self.resnet is not None and pos == PNP_CONV_POSITION:
+                ds = spec.downsample
+                state[key] = self._run_resnet(state[key], skips.get(key, state[key]), timestep, (H // ds, W // ds))
             h = block(state[key], encoder_hidden_states=encoder_hidden_states, timestep=timestep)
+            if pos < self.mid_position:
+                skips[key] = h
             if pos in res:
                 if res[pos].shape != h.shape:
                     raise ValueError(f"additional residual for census block {pos}: shape {tuple(res[pos].shape)}, "
@@ -429,15 +504,29 @@ def pnp_attention_modules(net: SkeletonUNet) -> List[nn.Module]:
     return [b.attn1 for i, b in zip(net.census_index, net.blocks) if i in PNP_CENSUS_BLOCKS]
 
 
+# diffusers' up_blocks[1].resnets[1], PnP's conv-injection target (utils/pnp_utils.py:168-169), runs right before
+# up_blocks[1].attentions[1], census block 8.  SD's time embedding has 4 x 320 channels.
+PNP_CONV_POSITION = 8
+TEMB_CHANNELS = 1280
+
+
+def pnp_conv_module(net: SkeletonUNet) -> nn.Module:
+    """The ResNet PnP's conv injection controls (pnp.register_conv_control(modules=[...])) in a skeleton built with
+    pnp_conv=True."""
+    if getattr(net, "resnet", None) is None:
+        raise ValueError("pnp_conv_module: the skeleton has no stand-in ResNet (make_skeleton(..., pnp_conv=True))")
+    return net.resnet
+
+
 def make_skeleton(name: str = "sd15", hot_path_only: bool = True, max_downsample: Optional[int] = None,
-                  device="cuda", dtype=torch.float16, seed: int = 123) -> SkeletonUNet:
+                  device="cuda", dtype=torch.float16, seed: int = 123, pnp_conv: bool = False) -> SkeletonUNet:
     census = CENSUSES[name]()
     cad = 1024 if name == "sd21" else 768
     gen_state = torch.get_rng_state()
     torch.manual_seed(seed)
     try:
         net = SkeletonUNet(census, cross_attention_dim=cad, hot_path_only=hot_path_only,
-                           max_downsample=max_downsample)
+                           max_downsample=max_downsample, pnp_conv=pnp_conv)
     finally:
         torch.set_rng_state(gen_state)
     return net.to(device=device, dtype=dtype).eval()
