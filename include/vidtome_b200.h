@@ -416,6 +416,43 @@ int vtm_cross_attention_lora(const void* x_dev, const void* ctx_dev, const void*
 int vtm_resnet_tail_f16(const void* h_dev, const void* shortcut_dev, void* out_dev, int32_t n, int32_t num_inputs,
                         int64_t sample_elems, float output_scale_factor, int32_t inject, void* stream);
 
+/*
+ * KD with the residual in the out projection — the self-attention of an UNMERGED block, `attn1(norm1(h)) + h`
+ * (vidtome/patch.py:157-169 with merge and unmerge = do_nothing; DDIM inversion runs the UNet unpatched,
+ * invert.py:117-140):
+ *   y = fp16(fp16(o Wo^T + bo) + resid),  o = per-head softmax(q k^T * scale) v,  q,k,v = x Wq^T, x Wk^T, x Wv^T
+ *   x_dev [B, L, C] fp16 (norm1's output); resid_dev [B, L, C] fp16 (the block input h, required: VTM_E_NULL);
+ *   y_dev [B, L, C] fp16, not overlapping resid_dev.  B counts (sample x frame) items; each item attends only within
+ *   its own L rows.  Weights, head_dim limits and LoRA descriptors as vtm_attention_lora (NULL = no adapter); no
+ *   shared-q/k injection.  The result equals vtm_attention_ex (or vtm_attention_lora) followed by torch's half add,
+ *   bit for bit: the add is the out projection's residual epilogue of vtm_linear_residual_f16.
+ *   Workspace: vtm_attention_lora_workspace_bytes(B, L, C, heads, R_qkv, R_o) (vtm_attention_workspace_bytes without
+ *   adapters).
+ */
+int vtm_attention_residual(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
+                           const void* resid_dev, const vtm_lora_t* lora_qkv, const vtm_lora_t* lora_o, int32_t B,
+                           int32_t L, int32_t C, int32_t heads, float scale, void* y_dev, void* ws_dev,
+                           size_t ws_bytes, void* stream);
+
+/*
+ * KI — one DDIM step in place, with its coefficients and trajectory slot read on the device (replaces the update of
+ * invert.py:182-211, `pred_next_x(..., inversion=True)`, and stores what invert.py:132-138 saves):
+ *   s = *step_dev;  (a, r, c, d) = coef_dev[4 s .. 4 s + 3];  x <- c * ((x - a * eps) * r) + d * eps,  r = 1 / b;
+ *   if slot_dev != NULL and 0 <= slot_dev[s] < n_slots:  traj[slot_dev[s]] <- x  (traj_dev [n_slots, n])
+ * For inversion a = sigma_prev, b = mu_prev, c = mu, d = sigma; for sampling (generate.py:281-311) a = sigma, b = mu,
+ * c = mu_prev, d = sigma_prev.  Because the step is read on the device, one captured
+ * CUDA graph serves every step; the caller advances *step_dev.  A step outside [0, n_steps) leaves x unchanged.
+ *   x_dev, eps_dev [n] fp16 (any n >= 1), 2-byte aligned (VTM_E_SHAPE); coef_dev [n_steps, 4] fp32, 16-byte aligned;
+ *   step_dev, slot_dev int32, 4-byte aligned; slot_dev may be NULL (no trajectory; traj_dev and n_slots are then
+ *   ignored), otherwise traj_dev is required (VTM_E_NULL) and n_slots >= 1 (VTM_E_SHAPE).
+ * Rounding is that of torch's CUDA half ops on python-float coefficients: each product, difference and sum is computed
+ * in fp32 and rounded to fp16, and the division is a multiplication by the reciprocal, which torch computes in double
+ * and rounds once to fp32: r = (float)(1.0 / b) in the table reproduces `half_tensor / python_float` bit for bit.
+ * 16-byte vectors are used wherever x, eps and the slot share their offset from a 16-byte boundary.
+ */
+int vtm_ddim_update_f16(void* x_dev, const void* eps_dev, int64_t n, const float* coef_dev, const int32_t* slot_dev,
+                        const int32_t* step_dev, int32_t n_steps, void* traj_dev, int32_t n_slots, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -141,6 +141,9 @@ SIGNATURES = {
     "vtm_cross_attention_lora": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _LORA, _LORA, _LORA, _i32, _i32, _i32,
                                            _i32, _i32, _i32, C.c_float, _vp, _vp, _sz, _vp]),
     "vtm_resnet_tail_f16": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i64, C.c_float, _i32, _vp]),
+    "vtm_attention_residual": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _LORA, _LORA, _i32, _i32, _i32, _i32, C.c_float, _vp,
+                                         _vp, _sz, _vp]),
+    "vtm_ddim_update_f16": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp, _i32, _vp, _i32, _vp]),
 }
 
 _lib: Optional[C.CDLL] = None

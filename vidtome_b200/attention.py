@@ -73,6 +73,15 @@ def self_attention(attn: torch.nn.Module, x: torch.Tensor, shared_qk: bool = Fal
                          lora_o=lora_o)
 
 
+def self_attention_residual(attn: torch.nn.Module, x: torch.Tensor, resid: torch.Tensor) -> torch.Tensor:
+    """attn(x) + resid for an unmerged block (vidtome/patch.py:157-169 with do_nothing merges) through
+    vtm_attention_residual: the same kernels as self_attention, the add in the out projection's epilogue."""
+    w_qkv, w_o, b_o, lora_qkv, lora_o = _packed(attn, x)
+    heads = int(attn.heads)
+    scale = float(getattr(attn, "scale", (x.shape[-1] // heads) ** -0.5))
+    return ops.attention_residual(x, w_qkv, w_o, b_o, heads, scale, resid, lora_qkv=lora_qkv, lora_o=lora_o)
+
+
 def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:
     """True if `attn` is a stock diffusers-style cross-attention (to_q [C, C], to_k / to_v [C, Cctx] without bias,
     to_out = [Linear, Dropout], default processor, no hooks / overrides / options that alter the math).  The projections

@@ -589,7 +589,7 @@ namespace {
 int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev, int32_t B,
                    int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, const int32_t* len_dev, void* y_dev,
                    void* ws_dev, size_t ws_bytes, void* stream_, const vtm_lora_t* lora_qkv = nullptr,
-                   const vtm_lora_t* lora_o = nullptr) {
+                   const vtm_lora_t* lora_o = nullptr, const void* resid_dev = nullptr) {
   if (!x_dev || !w_qkv_dev || !w_o_dev || !y_dev || !ws_dev) return VTM_E_NULL;
   if (B <= 0 || L <= 0 || C <= 0 || heads <= 0 || C % heads != 0) return VTM_E_SHAPE;
   const int d = C / heads;
@@ -629,8 +629,9 @@ int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev
   rc = launch_fa_any(qkv, kh, vh, o, B, L, L, C, heads, DP, scale, flags & 1, stream, len_dev);
   if (rc) return rc;
   if (Ro)
-    return vtm_linear_lora_f16(o, w_o_dev, b_o_dev, nullptr, 0, lora_o, M, C, C, y_dev, C, t,
+    return vtm_linear_lora_f16(o, w_o_dev, b_o_dev, resid_dev, resid_dev ? C : 0, lora_o, M, C, C, y_dev, C, t,
                                static_cast<size_t>(M) * Ro * 2, stream_);
+  if (resid_dev) return vtm_linear_residual_f16(o, w_o_dev, b_o_dev, resid_dev, C, M, C, C, y_dev, C, stream_);
   return vtm_linear_f16(o, w_o_dev, b_o_dev, M, C, C, y_dev, C, stream_);
 }
 }  // namespace
@@ -657,6 +658,17 @@ extern "C" int vtm_attention_lora(const void* x_dev, const void* w_qkv_dev, cons
                                   void* ws_dev, size_t ws_bytes, void* stream_) {
   return vtm::attention_impl(x_dev, w_qkv_dev, w_o_dev, b_o_dev, B, L, C, heads, scale, flags, len_dev, y_dev, ws_dev,
                              ws_bytes, stream_, lora_qkv, lora_o);
+}
+
+// Self-attention of an unmerged block with its residual: attn1(norm1(h)) + h (vidtome/patch.py:157-169 with u = m =
+// do_nothing), the residual added in the out projection's epilogue as vtm_linear_residual_f16 does.
+extern "C" int vtm_attention_residual(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev,
+                                      const void* b_o_dev, const void* resid_dev, const vtm_lora_t* lora_qkv,
+                                      const vtm_lora_t* lora_o, int32_t B, int32_t L, int32_t C, int32_t heads,
+                                      float scale, void* y_dev, void* ws_dev, size_t ws_bytes, void* stream_) {
+  if (!resid_dev) return VTM_E_NULL;
+  return vtm::attention_impl(x_dev, w_qkv_dev, w_o_dev, b_o_dev, B, L, C, heads, scale, 0, nullptr, y_dev, ws_dev,
+                             ws_bytes, stream_, lora_qkv, lora_o, resid_dev);
 }
 
 extern "C" int vtm_attention(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,

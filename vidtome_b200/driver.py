@@ -9,10 +9,15 @@ Restates, on synthetic latents, the parts of the reference's Generator that sit 
   init_pnp        generate.py:313-319   (PnP self-attention and conv-feature injection schedules; with `source_latents`)
   pre_iter        generate.py:226-231   (PnP: set the timestep, fetch the source latents of the step)
   ControlNet      generate.py:56-63,264-275, utils/utils.py:280-295 (residuals of `controlnet`, with `control_images`)
+and, in ChunkedInverter, the reference's Inverter around its hot path:
+  ddim_inversion  invert.py:117-140     (reversed timesteps, frame batches, the kept latents)
+  pred_noise      invert.py:159-179     (UNet forward, optional ControlNet residuals)
+  pred_next_x     invert.py:182-211     (inversion=True branch)
 Text conditioning, VAE, ControlNet preprocessing and file IO are outside the hot path and not restated.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Callable, Iterable, List, Optional
 
 import numpy as np
@@ -545,3 +550,200 @@ class ChunkedDenoiser:
         for i in range(len(self.timesteps)):
             x = self.step(x, i)
         return x
+
+
+class ChunkedInverter:
+    """DDIM inversion of source latents in frame batches, invert.py:117-211 (`Inverter.ddim_inversion`, `pred_noise`,
+    `pred_next_x(..., inversion=True)`): the trajectory PnP generation reads (`ChunkedDenoiser(source_latents=...)`).
+
+    Per step, over the reversed DDIM timesteps, every batch of `batch_size` frames (the last one may be ragged) gets
+    the noise prediction of the UNet under torch.autocast("cuda", fp16) (invert.py:121) with its rows of `cond`
+    ([F | 1, 77, D]: one text embedding per frame as prepare_cond builds it, or one for all), optionally with the
+    residuals of `controlnet` on `control_images` ([F, 3, H, W]) scaled by `control_scale` (invert.py:170-176, no CFG
+    repeat); then the latents take the inversion step
+        x <- mu * (x - sigma_prev * eps) / mu_prev + sigma * eps.
+    The latents after every step whose timestep is in the save schedule (`save_steps` DDIM steps, the reference's
+    `timesteps_to_save`; only with `save_intermediate`) and after the last step are kept, as invert.py:132-138 saves
+    them, in one device tensor `trajectory` [n_saved, F, 4, h, w] ordered as `saved_timesteps`.
+
+    A patched model (apply_patch) runs inside patch._unmerged_blocks(), i.e. as the reference's unpatched UNet: no merge,
+    no draw, no PnP injection, and attn1 of stock modules through KD with the residual in its out projection.  An
+    unpatched model runs its own forward.  On CUDA fp16 latents the update is KI (vtm_ddim_update_f16), which also stores
+    the kept latents; elsewhere it is pred_next_x in torch ops (float64 schedule constants as ChunkedDenoiser).
+
+    `cuda_graph=True` (CUDA fp16 latents): after `graph_warmup` eager steps one CUDA graph covers a whole step, i.e.
+    every batch's ControlNet and UNet call and KI with the trajectory store.  The UNet's timestep input, KI's
+    coefficients and its trajectory slot are read on the device from a step counter the graph advances, so each further
+    step is one replay, bit-identical to eager stepping."""
+
+    def __init__(self, unet: torch.nn.Module, n_timesteps: int = 50, batch_size: int = 8,
+                 save_steps: Optional[int] = None, save_intermediate: bool = True, cond: Optional[torch.Tensor] = None,
+                 controlnet: Optional[torch.nn.Module] = None, control_images: Optional[torch.Tensor] = None,
+                 control_scale: float = 1.0, cuda_graph: bool = False, graph_warmup: int = 2):
+        if not isinstance(n_timesteps, int) or n_timesteps <= 0:
+            raise ValueError(f"n_timesteps must be a positive int (got {n_timesteps!r})")
+        if not isinstance(batch_size, int) or batch_size <= 0:
+            raise ValueError(f"batch_size must be a positive int (got {batch_size!r})")
+        save_steps = n_timesteps if save_steps is None else save_steps
+        if not isinstance(save_steps, int) or save_steps <= 0:
+            raise ValueError(f"save_steps must be a positive int (got {save_steps!r})")
+        if (controlnet is None) != (control_images is None):
+            raise ValueError("controlnet and control_images go together")
+        if control_images is not None and (control_images.dim() != 4 or control_images.shape[1] != 3):
+            raise ValueError(f"control_images must be [F, 3, H, W] (got {tuple(control_images.shape)})")
+        if cond is not None and (cond.dim() != 3 or cond.shape[1] != 77):
+            raise ValueError(f"cond must be [F | 1, 77, D] (got {tuple(cond.shape)})")
+        if cuda_graph and int(graph_warmup) < 1:
+            raise ValueError(f"cuda_graph=True needs graph_warmup >= 1 (got {graph_warmup!r}): the modules' packed "
+                             f"weights are created by an eager step, outside the graph's memory pool")
+        self.unet = unet
+        self.batch_size = batch_size
+        self.cond = cond
+        self.controlnet = controlnet
+        self.control_images = control_images
+        self.control_scale = control_scale
+        self.cuda_graph = bool(cuda_graph)
+        self.graph_warmup = int(graph_warmup)
+        self.alphas_cumprod = ddim_alphas_cumprod()
+        self.final_alpha_cumprod = self.alphas_cumprod[0]     # set_alpha_to_one=False in SD's config
+        self.timesteps = ddim_timesteps(n_timesteps)[::-1]    # invert.py:120: reversed(scheduler.timesteps)
+        to_save = set(ddim_timesteps(save_steps)) if save_intermediate else set()
+        saved = [t for t in self.timesteps if t in to_save]   # invert.py:132
+        if self.timesteps[-1] not in saved:                   # invert.py:137-138: the final latents
+            saved.append(self.timesteps[-1])
+        self.saved_timesteps: List[int] = saved
+        self._slot_of = {t: k for k, t in enumerate(saved)}
+        self.slots = [self._slot_of.get(t, -1) for t in self.timesteps]
+        self.trajectory: Optional[torch.Tensor] = None
+
+    def _patched(self) -> bool:
+        return any(hasattr(m, "_tome_info") for m in self._models())
+
+    def _models(self) -> List[torch.nn.Module]:
+        return [self.unet] + ([self.controlnet] if self.controlnet is not None else [])
+
+    def coefficients(self, i: int):
+        """(a, b, c, d) of step i for x <- c * ((x - a * eps) / b) + d * eps: (sigma_prev, mu_prev, mu, sigma),
+        invert.py:182-211 with inversion=True."""
+        t = self.timesteps[i]
+        alpha_prod_t = self.alphas_cumprod[t]
+        alpha_prod_t_prev = self.alphas_cumprod[self.timesteps[i - 1]] if i > 0 else self.final_alpha_cumprod
+        mu, sigma = float(alpha_prod_t ** 0.5), float((1 - alpha_prod_t) ** 0.5)
+        mu_prev, sigma_prev = float(alpha_prod_t_prev ** 0.5), float((1 - alpha_prod_t_prev) ** 0.5)
+        return sigma_prev, mu_prev, mu, sigma
+
+    # invert.py:182-211 (inversion=True branch)
+    def pred_next_x(self, x: torch.Tensor, eps: torch.Tensor, i: int) -> torch.Tensor:
+        sigma_prev, mu_prev, mu, sigma = self.coefficients(i)
+        pred_x0 = (x - sigma_prev * eps) / mu_prev
+        return mu * pred_x0 + sigma * eps
+
+    # invert.py:159-179
+    @torch.no_grad()
+    def pred_noise(self, x: torch.Tensor, cond: Optional[torch.Tensor], t, ctrl: Optional[torch.Tensor] = None):
+        kwargs = {}
+        if ctrl is not None:                                                # utils/utils.py:280-295
+            down, mid = self.controlnet(x, t, encoder_hidden_states=cond, controlnet_cond=ctrl, return_dict=False)
+            down = [d * self.control_scale for d in down]
+            mid *= self.control_scale
+            kwargs = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
+        return self.unet(x, t, encoder_hidden_states=cond, **kwargs).sample
+
+    def _batch_cond(self, lo: int, hi: int, flen: int) -> Optional[torch.Tensor]:
+        if self.cond is None:
+            return None
+        if self.cond.shape[0] == 1:
+            return self.cond.expand(hi - lo, -1, -1)
+        if self.cond.shape[0] != flen:
+            raise ValueError(f"cond has {self.cond.shape[0]} rows for {flen} frames (one per frame, or one for all)")
+        return self.cond[lo:hi]
+
+    def _all_noises(self, x: torch.Tensor, t, ctrl: Optional[torch.Tensor], out: Optional[torch.Tensor] = None):
+        flen = len(x)
+        noises = torch.empty_like(x) if out is None else out
+        for lo in range(0, flen, self.batch_size):                         # invert.py:124-129
+            hi = min(lo + self.batch_size, flen)
+            noises[lo:hi] = self.pred_noise(x[lo:hi], self._batch_cond(lo, hi, flen), t,
+                                            None if ctrl is None else ctrl[lo:hi])
+        return noises
+
+    def _device_tables(self, x: torch.Tensor):
+        from . import ops
+        coef = ops.ddim_table(self.coefficients(i) for i in range(len(self.timesteps))).to(x.device)
+        slots = torch.tensor(self.slots, dtype=torch.int32, device=x.device)
+        ts = torch.tensor(self.timesteps, dtype=torch.int64, device=x.device)
+        step = torch.zeros(1, dtype=torch.int32, device=x.device)
+        return coef, slots, ts, step
+
+    @torch.no_grad()
+    def invert(self, x: torch.Tensor) -> torch.Tensor:
+        """Invert the clean latents x [F, 4, h, w] (invert.py:117-140).  Returns the final latents (the last entry of
+        `trajectory`); `x` itself is not modified."""
+        if x.dim() != 4:
+            raise ValueError(f"latents must be [F, 4, h, w] (got {tuple(x.shape)})")
+        ctrl = None
+        if self.controlnet is not None:
+            if len(self.control_images) != len(x):
+                raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
+            ctrl = self.control_images.to(x)
+        if self.cond is not None:
+            self._batch_cond(0, 0, len(x))                                 # check the row count up front
+        kernel = x.is_cuda and x.dtype == torch.float16
+        if self.cuda_graph and not kernel:
+            raise ValueError("cuda_graph=True needs CUDA fp16 latents: the captured step updates them with KI")
+        x = x.clone()
+        traj = torch.empty((len(self.saved_timesteps),) + tuple(x.shape), dtype=x.dtype, device=x.device)
+        scope = patch._unmerged_blocks() if self._patched() else contextlib.nullcontext()
+        with scope:
+            if kernel:
+                self._invert_device(x, ctrl, traj)
+            else:
+                with torch.autocast(x.device.type, dtype=torch.float16, enabled=x.is_cuda):
+                    for i, t in enumerate(self.timesteps):
+                        x = self.pred_next_x(x, self._all_noises(x, t, ctrl), i)
+                        if self.slots[i] >= 0:
+                            traj[self.slots[i]] = x
+        self.trajectory = traj
+        return traj[-1]
+
+    def _invert_device(self, x: torch.Tensor, ctrl: Optional[torch.Tensor], traj: torch.Tensor):
+        from . import ops
+        coef, slots, ts, step = self._device_tables(x)
+        n = len(self.timesteps)
+        eager = n if not self.cuda_graph else min(self.graph_warmup, n)
+        with torch.autocast("cuda", dtype=torch.float16):
+            for i in range(eager):
+                eps = self._all_noises(x, self.timesteps[i], ctrl)
+                ops.ddim_update(x, eps, coef, step, slots, traj)
+                step.add_(1)
+        if eager == n:
+            return
+        graph = torch.cuda.CUDAGraph()
+        torch.cuda.synchronize(x.device)
+        with torch.cuda.graph(graph), torch.autocast("cuda", dtype=torch.float16, cache_enabled=False):
+            gt = torch.index_select(ts, 0, step)                          # the UNet's timestep input, [1]
+            eps = self._all_noises(x, gt, ctrl)
+            ops.ddim_update(x, eps, coef, step, slots, traj)
+            step.add_(1)
+        for _ in range(eager, n):
+            graph.replay()
+        torch.cuda.synchronize(x.device)
+        del graph
+
+    def source_latents(self, frame_ids=None) -> Callable[[int], torch.Tensor]:
+        """The callable ChunkedDenoiser(source_latents=...) takes: t -> the inverted latents at timestep t [flen, 4,
+        h, w] (the reference's load_latent, generate.py:321-341), for the frames `frame_ids` (all when None).  A
+        timestep that was not kept raises."""
+        if self.trajectory is None:
+            raise RuntimeError("source_latents: call invert() first")
+        traj = self.trajectory if frame_ids is None else self.trajectory[:, torch.as_tensor(frame_ids).tolist()]
+
+        def load(t: int) -> torch.Tensor:
+            k = self._slot_of.get(int(t))
+            if k is None:
+                raise KeyError(f"no inverted latents were kept at timestep {int(t)} (kept: {self.saved_timesteps}); "
+                               f"PnP needs one at every generation timestep: invert with save_intermediate=True and "
+                               f"save_steps equal to the generation's n_timesteps")
+            return traj[k]
+
+        return load

@@ -494,6 +494,71 @@ def attention(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, b_o: Opti
     return y
 
 
+def ddim_table(coefficients) -> torch.Tensor:
+    """[n_steps, 4] fp32 rows (a, r, c, d) for ddim_update from python-float (a, b, c, d) per step: r = 1 / b in double,
+    rounded once to fp32, which is the reciprocal torch multiplies by for `half_tensor / b` (div_true_kernel_cuda)."""
+    return torch.tensor([(a, 1.0 / b, c, d) for a, b, c, d in coefficients], dtype=torch.float32)
+
+
+def attention_residual(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, b_o: Optional[torch.Tensor],
+                       heads: int, scale: float, resid: torch.Tensor, lora_qkv=None, lora_o=None) -> torch.Tensor:
+    """KD with the residual in the out projection: attention(x, ...) + resid, bit for bit as torch's half add, for an
+    unmerged block (`attn1(norm1(h)) + h`).  x, resid [B, L, C] fp16; lora_qkv / lora_o as in `attention`."""
+    _require(x, torch.float16, "x")
+    _require(w_qkv, torch.float16, "w_qkv")
+    _require(w_o, torch.float16, "w_o")
+    _require(resid, torch.float16, "resid")
+    B, L, Cc = x.shape
+    if resid.shape != x.shape:
+        raise RuntimeError(f"attention_residual: resid {tuple(resid.shape)} must be shaped like x {tuple(x.shape)}")
+    lib = _lib.load()
+    dq, rq = _lora_arg(lora_qkv, Cc, 3 * Cc, "attention qkv")
+    do, ro = _lora_arg(lora_o, Cc, Cc, "attention out")
+    ws_bytes = lib.vtm_attention_lora_workspace_bytes(B, L, Cc, heads, rq, ro)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+    y = torch.empty_like(x)
+    flops = 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc + 8.0 * B * L * Cc * (rq + ro)
+    with _Timed("KD", flops, 6.0 * B * L * Cc + 8.0 * Cc * Cc):
+        check(lib.vtm_attention_residual(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), resid.data_ptr(),
+                                         _lora_ref(dq), _lora_ref(do), B, L, Cc, heads, float(scale), y.data_ptr(),
+                                         ws.data_ptr(), ws_bytes, _stream()), "vtm_attention_residual")
+    STATS.launches += 3 + (rq > 0) + (ro > 0)
+    return y
+
+
+def ddim_update(x: torch.Tensor, eps: torch.Tensor, coef: torch.Tensor, step: torch.Tensor,
+                slots: Optional[torch.Tensor] = None, traj: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """KI, in place on x: with s = step[0] and (a, r, c, d) = coef[s], x <- c * ((x - a * eps) * r) + d * eps in torch's
+    CUDA half roundings, and traj[slots[s]] <- x when slots[s] >= 0.  r = float(1.0 / b) (ddim_table) reproduces torch's
+    `/ b`.  x, eps fp16 of one shape; coef [n_steps, 4] fp32;
+    step a 1-element int32 tensor (read on the device, not advanced); slots [n_steps] int32 with traj [n_slots, *x.shape]
+    fp16, or both None."""
+    _require(x, torch.float16, "x")
+    _require(eps, torch.float16, "eps")
+    _require(coef, torch.float32, "coef")
+    _require(step, torch.int32, "step")
+    if eps.shape != x.shape:
+        raise RuntimeError(f"ddim_update: eps {tuple(eps.shape)} must be shaped like x {tuple(x.shape)}")
+    if coef.dim() != 2 or coef.shape[1] != 4 or step.numel() != 1:
+        raise RuntimeError("ddim_update: coef must be [n_steps, 4] and step a 1-element tensor")
+    if (slots is None) != (traj is None):
+        raise RuntimeError("ddim_update: slots and traj go together")
+    n_slots = 0
+    if slots is not None:
+        _require(slots, torch.int32, "slots")
+        _require(traj, torch.float16, "traj")
+        if tuple(slots.shape) != (coef.shape[0],) or traj.shape[1:] != x.shape:
+            raise RuntimeError(f"ddim_update: slots must be [{coef.shape[0]}] and traj [n_slots, {tuple(x.shape)}]")
+        n_slots = traj.shape[0]
+    n = x.numel()
+    with _Timed("KI", 6.0 * n, 2.0 * n * (3 + (slots is not None))):
+        check(_lib.load().vtm_ddim_update_f16(x.data_ptr(), eps.data_ptr(), n, coef.data_ptr(), _ptr(slots),
+                                              step.data_ptr(), coef.shape[0], _ptr(traj), n_slots, _stream()),
+              "vtm_ddim_update_f16")
+    STATS.launches += 1
+    return x
+
+
 def cross_attention(x: torch.Tensor, ctx: torch.Tensor, w_q: torch.Tensor, w_kv: torch.Tensor, w_o: torch.Tensor,
                     b_o: Optional[torch.Tensor], heads: int, scale: float, resid: Optional[torch.Tensor] = None,
                     lora_q=None, lora_kv=None, lora_o=None) -> torch.Tensor:

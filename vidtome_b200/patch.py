@@ -14,6 +14,7 @@ global tokens exist, drawn from `module.generator` on the generator's device (me
 """
 from __future__ import annotations
 
+import contextlib
 import math
 from dataclasses import dataclass, field
 from typing import Any, Callable, Dict, List, Optional, Tuple, Type
@@ -77,6 +78,30 @@ GLOBAL_EXCHANGE = "recurrence"
 # (VtmSplit.prefix_coin), so nothing is read back to the host.  Results are bit-identical to the host coin.  It needs
 # both sets to be equally long (equal chunks); eagerly, a block whose sets differ keeps the host coin.
 DEVICE_COIN = False
+
+# Depth of _unmerged_blocks() contexts: while > 0 every ToMeBlock runs as the reference's UNPATCHED block.
+_UNMERGED = 0
+
+
+@contextlib.contextmanager
+def _unmerged_blocks():
+    """Run patched models as the reference runs them before apply_patch, for DDIM inversion (invert.py:117-140 runs
+    first, on the unpatched UNet; SURVEY App. C.13).  Inside, a ToMeBlock builds no merge plan (nothing is drawn,
+    `global_tokens` is left alone), its pre-hook forks no generator, and no PnP injection runs whatever `t` the marked
+    modules hold (pnp.injection_active).  attn1 of a stock module (_plain_attention_module) runs as norm1 -> KD with the
+    residual in its out projection (vtm_attention_residual), PnP-marked modules included; any other attn1 runs its own
+    forward.  attn2 and ff go through the library as they do outside."""
+    global _UNMERGED
+    _UNMERGED += 1
+    try:
+        yield
+    finally:
+        _UNMERGED -= 1
+
+
+def unmerged_active() -> bool:
+    """True inside _unmerged_blocks()."""
+    return _UNMERGED > 0
 
 
 class GlobalTokenStore:
@@ -431,56 +456,72 @@ def make_diffusers_tome_block(block_class: Type[torch.nn.Module]) -> Type[torch.
                     encoder_attention_mask=None, timestep=None, cross_attention_kwargs=None,
                     class_labels=None) -> torch.Tensor:
             plan = None
-            if self.use_ada_layer_norm:                                       # patch.py:139-146
-                norm_hidden_states = self.norm1(hidden_states, timestep)
-            elif self.use_ada_layer_norm_zero:
-                norm_hidden_states, gate_msa, shift_mlp, scale_mlp, gate_mlp = self.norm1(
-                    hidden_states, timestep, class_labels, hidden_dtype=hidden_states.dtype)
-            else:
-                ln = _fusable_layer_norm(self.norm1, hidden_states) if hidden_states.is_cuda else None
-                if ln is not None:
-                    # norm1 fused into the merge kernels: only the kept rows are ever normalised
-                    plan = build_merge_plan(self, hidden_states, self._tome_info, ln=ln)
-                norm_hidden_states = None if plan is not None else self.norm1(hidden_states)
-
-            if plan is None:
-                plan = build_merge_plan(self, norm_hidden_states, self._tome_info)  # patch.py:149-150
-            if plan is not None:
-                norm_hidden_states = plan.merged_tokens
-
-            # 1. Self-Attention (patch.py:154-162)
+            unmerged = _UNMERGED > 0
             cross_attention_kwargs = cross_attention_kwargs if cross_attention_kwargs is not None else {}
             only_cross = getattr(self, "only_cross_attention", False)
             from . import attention as _attention
-            if (plan is not None and _attention.ENABLED and not only_cross and attention_mask is None
-                    and not cross_attention_kwargs and _plain_attention_module(self.attn1)):
-                # KD; with PnP control registered (pnp.py) and the timestep inside the injection schedule, the attention
-                # map of the source sample is applied to every sample's values (utils/pnp_utils.py:57-68,87-91)
-                shared = False
-                if getattr(self.attn1, "_vtm_pnp", 0):
-                    from . import pnp as _pnp
-                    shared = _pnp.injection_active(self.attn1)
-                    if shared and norm_hidden_states.shape[0] != self.attn1._vtm_pnp:
-                        raise RuntimeError("PnP injection needs one merged token set per input (batch_size == num_inputs)")
-                attn_output = _attention.self_attention(self.attn1, norm_hidden_states, shared_qk=shared,
-                                                        seq_len=plan.seq_len)                             # KD
-            elif plan is not None and plan.seq_len is not None:
-                raise RuntimeError("GlobalTokenStore: the merged tokens are sized for capacity with their length on the "
-                                   "device, which only the library's self-attention (KD) reads; this block's attn1 "
-                                   "runs its own forward")
+            ln1 = None
+            if (unmerged and hidden_states.is_cuda and hidden_states.dtype == torch.float16 and _attention.ENABLED
+                    and not self.use_ada_layer_norm and not self.use_ada_layer_norm_zero and not only_cross
+                    and attention_mask is None and not cross_attention_kwargs and _plain_attention_module(self.attn1)):
+                ln1 = _fusable_layer_norm(self.norm1, hidden_states)
+            if ln1 is not None:
+                # unmerged (_unmerged_blocks): attn1(norm1(h)) + h, the add in the out projection of KD
+                shape = hidden_states.shape
+                hidden_states = hidden_states.contiguous()
+                n1 = ops.layer_norm(hidden_states.view(-1, shape[-1]), ln1).view(shape)
+                hidden_states = _attention.self_attention_residual(self.attn1, n1, hidden_states)
             else:
-                attn_output = self.attn1(
-                    norm_hidden_states,
-                    encoder_hidden_states=encoder_hidden_states if only_cross else None,
-                    attention_mask=attention_mask, **cross_attention_kwargs)
-            if self.use_ada_layer_norm_zero:
-                attn_output = gate_msa.unsqueeze(1) * attn_output            # patch.py:164-165
+                if self.use_ada_layer_norm:                                       # patch.py:139-146
+                    norm_hidden_states = self.norm1(hidden_states, timestep)
+                elif self.use_ada_layer_norm_zero:
+                    norm_hidden_states, gate_msa, shift_mlp, scale_mlp, gate_mlp = self.norm1(
+                        hidden_states, timestep, class_labels, hidden_dtype=hidden_states.dtype)
+                else:
+                    ln = (_fusable_layer_norm(self.norm1, hidden_states) if hidden_states.is_cuda and not unmerged
+                          else None)
+                    if ln is not None:
+                        # norm1 fused into the merge kernels: only the kept rows are ever normalised
+                        plan = build_merge_plan(self, hidden_states, self._tome_info, ln=ln)
+                    norm_hidden_states = None if plan is not None else self.norm1(hidden_states)
 
-            # Unmerge + residual (patch.py:168-169), fused into one pass
-            if plan is not None:
-                hidden_states = plan.unmerge_add(attn_output, hidden_states)
-            else:
-                hidden_states = attn_output + hidden_states
+                if plan is None and not unmerged:
+                    plan = build_merge_plan(self, norm_hidden_states, self._tome_info)  # patch.py:149-150
+                if plan is not None:
+                    norm_hidden_states = plan.merged_tokens
+
+                # 1. Self-Attention (patch.py:154-162)
+                if (plan is not None and _attention.ENABLED and not only_cross and attention_mask is None
+                        and not cross_attention_kwargs and _plain_attention_module(self.attn1)):
+                    # KD; with PnP control registered (pnp.py) and the timestep inside the injection schedule, the
+                    # attention map of the source sample is applied to every sample's values (utils/pnp_utils.py:57-68,
+                    # 87-91)
+                    shared = False
+                    if getattr(self.attn1, "_vtm_pnp", 0):
+                        from . import pnp as _pnp
+                        shared = _pnp.injection_active(self.attn1)
+                        if shared and norm_hidden_states.shape[0] != self.attn1._vtm_pnp:
+                            raise RuntimeError("PnP injection needs one merged token set per input "
+                                               "(batch_size == num_inputs)")
+                    attn_output = _attention.self_attention(self.attn1, norm_hidden_states, shared_qk=shared,
+                                                            seq_len=plan.seq_len)                             # KD
+                elif plan is not None and plan.seq_len is not None:
+                    raise RuntimeError("GlobalTokenStore: the merged tokens are sized for capacity with their length on "
+                                       "the device, which only the library's self-attention (KD) reads; this block's "
+                                       "attn1 runs its own forward")
+                else:
+                    attn_output = self.attn1(
+                        norm_hidden_states,
+                        encoder_hidden_states=encoder_hidden_states if only_cross else None,
+                        attention_mask=attention_mask, **cross_attention_kwargs)
+                if self.use_ada_layer_norm_zero:
+                    attn_output = gate_msa.unsqueeze(1) * attn_output            # patch.py:164-165
+
+                # Unmerge + residual (patch.py:168-169), fused into one pass
+                if plan is not None:
+                    hidden_states = plan.unmerge_add(attn_output, hidden_states)
+                else:
+                    hidden_states = attn_output + hidden_states
 
             attn2 = getattr(self, "attn2", None)
             if (attn2 is not None and FUSE_CROSS_ATTENTION and hidden_states.is_cuda and not self.use_ada_layer_norm
@@ -529,6 +570,8 @@ def hook_tome_model(model: torch.nn.Module):
     """Forward pre-hook recording the latent size (patch.py:206-212).  The UNet must be called with the
     latent as positional argument 0, as generate.py:275 does."""
     def hook(module, args):
+        if _UNMERGED:                        # an unpatched model records nothing (_unmerged_blocks)
+            return None
         module._tome_info["size"] = (args[0].shape[2], args[0].shape[3])
         return None
 
@@ -540,6 +583,8 @@ def hook_tome_module(module: torch.nn.Module):
     input's device the first time the block runs (and again if the block moves to another device), so that all
     blocks draw the same random target frames within one pass (patch.py:215-231)."""
     def hook(module, args):
+        if _UNMERGED:                        # an unpatched block has no generator (_unmerged_blocks)
+            return None
         device = args[0].device
         current = getattr(module, "generator", None)
         if current is None:

@@ -23,6 +23,8 @@ from typing import Iterable, Optional, Sequence
 
 import torch
 
+from . import patch
+
 RES_DICT = {1: [1, 2], 2: [0, 1, 2], 3: [0, 1, 2]}       # utils/pnp_utils.py:97 (blocks 4 - 11 of the decoder)
 
 
@@ -38,7 +40,10 @@ def _targets(model, modules: Optional[Iterable[torch.nn.Module]]):
 
 
 def injection_active(attn: torch.nn.Module) -> bool:
-    """utils/pnp_utils.py:57-58: `self.injection_schedule is not None and (self.t in self.injection_schedule or self.t == 1000)`."""
+    """utils/pnp_utils.py:57-58: `self.injection_schedule is not None and (self.t in self.injection_schedule or self.t == 1000)`.
+    Always False inside patch._unmerged_blocks(): DDIM inversion runs before PnP is registered (invert.py:117-140)."""
+    if patch.unmerged_active():
+        return False
     sched = getattr(attn, "injection_schedule", None)
     t = getattr(attn, "t", None)
     return sched is not None and t is not None and (t in sched or t == 1000)
