@@ -453,6 +453,35 @@ int vtm_attention_residual(const void* x_dev, const void* w_qkv_dev, const void*
 int vtm_ddim_update_f16(void* x_dev, const void* eps_dev, int64_t n, const float* coef_dev, const int32_t* slot_dev,
                         const int32_t* step_dev, int32_t n_steps, void* traj_dev, int32_t n_slots, void* stream);
 
+/*
+ * KG1 / KG2 / NchwEpi — the entry and exit of diffusers' Transformer2DModel.forward, the module that owns every
+ * BasicTransformerBlock of the UNet and works on NCHW activations (third-party code, not part of the reference; its
+ * arithmetic is torch's):
+ *   residual = x;  x = GroupNorm(groups, C)(x);  x = proj_in(x);  x -> [n, HW, C] tokens;  blocks;  x -> NCHW;
+ *   x = proj_out(x);  return x + residual                (proj_in / proj_out: 1x1 Conv2d, or Linear on the token side)
+ * x_dev is a contiguous NCHW fp16 tensor [n, C, HW], 2-byte aligned (16-byte aligned and HW % 8 == 0 for the vector
+ * paths), C % groups == 0 (VTM_E_SHAPE).
+ *
+ * vtm_group_norm_stats_f16: stats_dev [n, groups, 2] fp32 = (mean, rstd) of every (sample, group), a contiguous run of
+ *   (C / groups) * HW halfs; rstd = 1 / sqrt(var + eps) with the biased variance; fp32 throughout, combined pairwise
+ *   (Chan et al.) so that a large mean does not cancel.  stats_dev 8-byte aligned, eps >= 0.  Workspace:
+ *   vtm_group_norm_stats_workspace_bytes(n, C, HW, groups) (0 unless long runs are split over CTAs; VTM_E_WS).
+ * vtm_group_norm_tokens_f16: y_dev [n, HW, C] fp16 token-major, 16-byte aligned, C % 8 == 0,
+ *   y[i, p, c] = fp16(fma((float(x[i, c, p]) - mean) * rstd, gamma[c], beta[c])) with fp32 round-to-nearest steps;
+ *   gamma_dev / beta_dev [C] fp16, NULL = 1 / 0.  n <= 65535.
+ * vtm_linear_nchw_residual_f16: D[i, o, p] = fp16(fp16(sum_k A[i HW + p, k] W[o, k] + bias[o]) + R[i, o, p]),
+ *   a_dev [n * HW, K] token-major rows, w_dev [N, K], bias_dev [N] or NULL, resid_dev [n, N, HW] or NULL, d_dev
+ *   [n, N, HW]; K % 8 == 0, N % 8 == 0.  The mainloop, the bias and the two roundings are vtm_linear_residual_f16's:
+ *   the result equals that entry's followed by a transpose, bit for bit.  d_dev may equal resid_dev.
+ */
+size_t vtm_group_norm_stats_workspace_bytes(int32_t n, int32_t C, int32_t HW, int32_t groups);
+int vtm_group_norm_stats_f16(const void* x_dev, int32_t n, int32_t C, int32_t HW, int32_t groups, float eps,
+                             float* stats_dev, void* ws_dev, size_t ws_bytes, void* stream);
+int vtm_group_norm_tokens_f16(const void* x_dev, const float* stats_dev, const void* gamma_dev, const void* beta_dev,
+                              int32_t n, int32_t C, int32_t HW, int32_t groups, void* y_dev, void* stream);
+int vtm_linear_nchw_residual_f16(const void* a_dev, const void* w_dev, const void* bias_dev, const void* resid_dev,
+                                 int32_t n, int32_t HW, int32_t N, int32_t K, void* d_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

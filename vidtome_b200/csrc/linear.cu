@@ -101,6 +101,101 @@ struct StoreEpi {
   __device__ __forceinline__ void end(int, int, int) {}
 };
 
+// StoreEpi's arithmetic with the output (and the optional residual) in NCHW: GEMM row m = i HW + p is token p of sample
+// i, and D[i, o, p] = fp16(fp16(acc + bias[o]) + R[i, o, p]) for D, R [n, N, HW] contiguous.  This is the exit of
+// diffusers' Transformer2DModel.forward (proj_out, the permute back to NCHW and `+ residual`).
+// A thread holds one token, so for one channel a warp covers only 64 contiguous bytes of D.  The two warps that hold the
+// same 64 columns of a warpgroup's 64 rows therefore share their two staging areas (8 KB) as S[channel][token], 128
+// bytes per channel: each thread writes its 64 values as 2-byte stores (a warp's lanes are consecutive tokens: 64
+// contiguous bytes, no bank conflict), the 64 threads meet at a named barrier, and thread t then takes the 16-byte
+// chunk t % 8 (eight tokens) of channels t / 8 + 8 j, so that eight lanes write (and read R) one channel's 128 bytes.
+// The chunk's place in D follows from its first token alone, (m / HW, m % HW), computed once per work item: with
+// HW % 8 == 0 a chunk never straddles a sample, whatever the M tile does.  Otherwise (HW = 1, or D / R not 16-byte
+// aligned) each of the eight tokens is placed and stored on its own.
+struct NchwEpi {
+  static constexpr uint32_t SCRATCH_PER_WARP = gemm::STAGE_STORE_BYTES;
+  static constexpr bool WHOLE_ROWS = false;
+  __half* d;
+  const __half* bias;
+  const __half* resid;   // optional, laid out as d
+  int M, N, HW;
+  int vec_ok;            // HW % 8 == 0 and d, resid 16-byte aligned
+  int m_chunk;           // first of this thread's eight tokens in the store phase
+  long long off_chunk;   // (m_chunk / HW) N HW + m_chunk % HW
+  uint32_t scratch;      // the pair's 8 KB
+
+  __device__ __forceinline__ void set_scratch(uint32_t a) { scratch = a - ((threadIdx.x >> 5) & 1) * SCRATCH_PER_WARP; }
+  __device__ __forceinline__ void begin(int m_tile, int, int row_in_tile) {
+    m_chunk = m_tile * gemm::BM + (row_in_tile & ~63) + 8 * (threadIdx.x & 7);
+    const int i = m_chunk / HW;
+    off_chunk = static_cast<long long>(i) * N * HW + (m_chunk - i * HW);
+  }
+  __device__ __forceinline__ void tile(const gemm::Acc& acc, int col0, int ncols) {
+    const int t64 = threadIdx.x & 63;
+    // barriers 1 and 2 are the mainloop's: 3 + 2 (consumer warpgroup) + (column half)
+    const uint32_t bar = 3 + 2 * ((threadIdx.x >> 7) - 1) + ((threadIdx.x >> 6) & 1);
+#pragma unroll 1
+    for (int cb = 0; cb < ncols; cb += 64) {
+      uint32_t r[64];
+      acc.ld64(cb, r);
+      const int c0 = col0 + cb;
+      const uint32_t col = scratch + 2u * t64;                 // S[0][this thread's token]
+#pragma unroll
+      for (int v8 = 0; v8 < 8; ++v8) {
+        // without a bias the addend is -0, and acc + (-0) is acc bit for bit (+0 would turn a -0 accumulator into +0):
+        // one code path, the same bits as StoreEpi's two
+        uint4 bv = make_uint4(0x80008000u, 0x80008000u, 0x80008000u, 0x80008000u);
+        if (bias && c0 + 8 * v8 < N) bv = __ldg(reinterpret_cast<const uint4*>(bias + c0 + 8 * v8));
+        const __half2* b2 = reinterpret_cast<const __half2*>(&bv);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 bf = __half22float2(b2[e]);
+          const int c = 8 * v8 + 2 * e;
+          const uint32_t pk = pack_f16x2(__fadd_rn(__uint_as_float(r[c]), bf.x), __fadd_rn(__uint_as_float(r[c + 1]), bf.y));
+          asm volatile("st.shared.u16 [%0], %1;" ::"r"(col + 128u * c), "h"(static_cast<uint16_t>(pk & 0xffffu)) : "memory");
+          asm volatile("st.shared.u16 [%0], %1;" ::"r"(col + 128u * (c + 1)), "h"(static_cast<uint16_t>(pk >> 16)) : "memory");
+        }
+      }
+      bar_sync_named(bar, 64);
+      const int lim = min(N - c0, ncols - cb);                  // channels of this chunk that exist
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int ch = 8 * j + (t64 >> 3);
+        if (ch >= lim || m_chunk >= M) continue;
+        uint4 v;
+        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+                     : "r"(scratch + 128u * ch + 16u * (t64 & 7))
+                     : "memory");
+        const long long ch_off = static_cast<long long>(c0 + ch) * HW;
+        if (vec_ok) {
+          const long long o = off_chunk + ch_off;
+          if (resid) {
+            const uint4 rv = *reinterpret_cast<const uint4*>(resid + o);
+            __half2* a = reinterpret_cast<__half2*>(&v);
+            const __half2* b2 = reinterpret_cast<const __half2*>(&rv);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) a[e] = __hadd2(a[e], b2[e]);
+          }
+          *reinterpret_cast<uint4*>(d + o) = v;
+        } else {
+          const __half* h = reinterpret_cast<const __half*>(&v);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) {
+            const int m = m_chunk + e;
+            if (m >= M) break;
+            const int i = m / HW;
+            const long long o = static_cast<long long>(i) * N * HW + (m - i * HW) + ch_off;
+            d[o] = resid ? __hadd(h[e], resid[o]) : h[e];
+          }
+        }
+      }
+      bar_sync_named(bar, 64);                                  // S may be overwritten
+    }
+  }
+  __device__ __forceinline__ void end(int, int, int) {}
+};
+
 // gelu(g) = 0.5 g (1 + erf(g / sqrt 2)) with ONE MUFU op: for t = |g|, log2(erfc(t / sqrt 2)) is smooth and close to a
 // parabola, so h = erfc(t / sqrt 2) / 2 = 2^(p(t) - 1) with a degree-7 polynomial p (p(0) = 0), fitted minimax to
 // log2(erfc(t / sqrt 2)) on [0, 5.94].  The fit bounds the exponent's absolute error (5.7e-6), i.e. h's RELATIVE error
@@ -284,6 +379,35 @@ int geglu_impl(const void* a_dev, const void* w_il_dev, const void* bias_il_dev,
   return gemm::launch_tail<GegluEpi>(ta, tb, tt, tu, wk, epi, sms, stream);
 }
 
+int linear_nchw_impl(const void* a_dev, const void* w_dev, const void* bias_dev, const void* resid_dev, int n, int HW,
+                     int N, int K, void* d_dev, cudaStream_t stream) {
+  if (!a_dev || !w_dev || !d_dev) return VTM_E_NULL;
+  if (n <= 0 || HW <= 0 || N <= 0 || K <= 0 || (K % 8) != 0 || (N % 8) != 0) return VTM_E_SHAPE;
+  const long long M = static_cast<long long>(n) * HW;
+  if (M > 0x7fffffffLL - gemm::BM) return VTM_E_SHAPE;
+  if (reinterpret_cast<uintptr_t>(d_dev) % 2 != 0 || reinterpret_cast<uintptr_t>(resid_dev) % 2 != 0) return VTM_E_SHAPE;
+  int sms = 0;
+  int rc = gemm::device_sms(&sms);
+  if (rc) return rc;
+  NchwEpi epi;
+  epi.d = static_cast<__half*>(d_dev);
+  epi.bias = static_cast<const __half*>(bias_dev);
+  epi.resid = static_cast<const __half*>(resid_dev);
+  epi.M = static_cast<int>(M); epi.N = N; epi.HW = HW;
+  epi.vec_ok = HW % 8 == 0 && reinterpret_cast<uintptr_t>(d_dev) % 16 == 0 &&
+               reinterpret_cast<uintptr_t>(resid_dev) % 16 == 0;
+  epi.m_chunk = 0; epi.off_chunk = 0; epi.scratch = 0;
+  CUtensorMap ta, tb;
+  rc = make_tmap_3d_f16(&ta, a_dev, K, M, 1, K, static_cast<uint64_t>(M) * K, gemm::BK, gemm::BM);
+  if (rc) return rc;
+  rc = make_tmap_3d_f16(&tb, w_dev, K, N, 1, K, static_cast<uint64_t>(N) * K, gemm::BK, gemm::BN);
+  if (rc) return rc;
+  gemm::Work wk;
+  wk.plan(static_cast<int>(M), N, K, 1, sms, 16, 1);
+  wk.n_fastest = 1;
+  return gemm::launch<NchwEpi>(ta, tb, wk, epi, sms, stream);
+}
+
 // Checks a LoRA descriptor and its workspace for a GEMM with M rows; *R_out = its rank (0 for no LoRA).
 int lora_args(const vtm_lora_t* lora, int M, const void* ws_dev, size_t ws_bytes, int* R_out) {
   *R_out = 0;
@@ -315,6 +439,12 @@ extern "C" int vtm_linear_residual_f16(const void* a_dev, const void* w_dev, con
                                        void* stream_) {
   if (!resid_dev) return VTM_E_NULL;
   return vtm::linear_impl(a_dev, w_dev, bias_dev, resid_dev, ldr, M, N, K, d_dev, ldd, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int vtm_linear_nchw_residual_f16(const void* a_dev, const void* w_dev, const void* bias_dev,
+                                            const void* resid_dev, int32_t n, int32_t HW, int32_t N, int32_t K,
+                                            void* d_dev, void* stream_) {
+  return vtm::linear_nchw_impl(a_dev, w_dev, bias_dev, resid_dev, n, HW, N, K, d_dev, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int vtm_linear_geglu_f16(const void* a_dev, const void* w_il_dev, const void* bias_il_dev, int32_t M,

@@ -635,6 +635,70 @@ def resnet_tail(h: torch.Tensor, shortcut: torch.Tensor, num_inputs: int, output
     return out
 
 
+def group_norm_stats(x: torch.Tensor, groups: int, eps: float) -> torch.Tensor:
+    """KG1.  x [n, C, ...] contiguous NCHW fp16 -> [n, groups, 2] fp32 (mean, rstd) of torch's group_norm."""
+    _require(x, torch.float16, "x")
+    n, Cc = x.shape[:2]
+    HW = x[0, 0].numel()
+    lib = _lib.load()
+    stats = torch.empty((n, groups, 2), dtype=torch.float32, device=x.device)
+    ws_bytes = lib.vtm_group_norm_stats_workspace_bytes(n, Cc, HW, groups)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device) if ws_bytes else None
+    with _Timed("KG1", 0.0, 2.0 * x.numel()):
+        check(lib.vtm_group_norm_stats_f16(x.data_ptr(), n, Cc, HW, groups, float(eps), stats.data_ptr(), _ptr(ws),
+                                           ws_bytes, _stream()), "vtm_group_norm_stats_f16")
+    STATS.launches += 2 if ws_bytes else 1
+    return stats
+
+
+def group_norm_tokens(x: torch.Tensor, gn) -> torch.Tensor:
+    """KG1 + KG2.  GroupNorm of x [n, C, h, w] (contiguous NCHW fp16) written as token-major rows [n, h * w, C]:
+    `group_norm(x).permute(0, 2, 3, 1).reshape(n, h * w, C)` without the NCHW intermediate.
+    gn = (weight [C] or None, bias [C] or None, eps, num_groups)."""
+    weight, bias, eps, groups = gn
+    stats = group_norm_stats(x, groups, eps)
+    n, Cc = x.shape[:2]
+    HW = x[0, 0].numel()
+    if weight is not None:
+        _require(weight, torch.float16, "weight")
+    if bias is not None:
+        _require(bias, torch.float16, "bias")
+    y = torch.empty((n, HW, Cc), dtype=torch.float16, device=x.device)
+    with _Timed("KG2", 0.0, 4.0 * x.numel()):
+        check(_lib.load().vtm_group_norm_tokens_f16(x.data_ptr(), stats.data_ptr(), _ptr(weight), _ptr(bias), n, Cc, HW,
+                                                    groups, y.data_ptr(), _stream()), "vtm_group_norm_tokens_f16")
+    STATS.launches += 1
+    return y
+
+
+def linear_nchw_residual(tokens: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor],
+                         residual: Optional[torch.Tensor], hw: Tuple[int, int]) -> torch.Tensor:
+    """D[i, o, y, x] = (tokens[i * h * w + y * w + x] W^T + bias)[o] + residual[i, o, y, x] with torch's fp16 roundings
+    (`conv(x) + residual`): the projection GEMM storing NCHW.  tokens [n * h * w, K], w [N, K] (a 1x1 conv's weight
+    viewed as a matrix, or a Linear's), residual [n, N, h, w] or None -> [n, N, h, w]."""
+    _require(tokens, torch.float16, "tokens")
+    _require(w, torch.float16, "w")
+    M, K = tokens.shape
+    N = w.shape[0]
+    h, wd = hw
+    HW = h * wd
+    if w.dim() != 2 or w.shape[1] != K or HW <= 0 or M % HW:
+        raise RuntimeError(f"linear_nchw_residual: tokens {tuple(tokens.shape)} / w {tuple(w.shape)} / hw {hw} do not fit")
+    n = M // HW
+    if bias is not None:
+        _require(bias, torch.float16, "bias")
+    if residual is not None:
+        _require(residual, torch.float16, "residual")
+        if tuple(residual.shape) != (n, N, h, wd):
+            raise RuntimeError(f"linear_nchw_residual: residual must be {(n, N, h, wd)}, got {tuple(residual.shape)}")
+    d = torch.empty((n, N, h, wd), dtype=torch.float16, device=tokens.device)
+    with _Timed("PO", 2.0 * M * N * K, 2.0 * (M * K + N * K + (2 if residual is not None else 1) * M * N)):
+        check(_lib.load().vtm_linear_nchw_residual_f16(tokens.data_ptr(), w.data_ptr(), _ptr(bias), _ptr(residual), n, HW,
+                                                       N, K, d.data_ptr(), _stream()), "vtm_linear_nchw_residual_f16")
+    STATS.launches += 1
+    return d
+
+
 def keys_to_score_arg(keys: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """Unpack KA keys on the device with torch integer ops (test / debugging helper)."""
     o = (keys >> 32) & 0xFFFF

@@ -63,6 +63,11 @@ FUSE_FEED_FORWARD = True
 # Run a stock cross-attention (norm2 + attn2 + residual, patch.py:171-185) through the CUDA library (attention.py).
 FUSE_CROSS_ATTENTION = True
 
+# Run the entry and exit of every diffusers Transformer2DModel of a patched model (GroupNorm -> proj_in -> token-major
+# rows, and proj_out -> NCHW + residual) through the CUDA library (transformer2d.py); modules it cannot serve keep their
+# own forward (transformer2d.ineligibility).
+FUSE_TRANSFORMER_IO = True
+
 # How `merge_global=True` obtains the global token set when several ranks each hold one chunk:
 #   "recurrence" — the reference's semantics (patch.py:59-82): whatever the previous chunk processed by THIS
 #                  process left in module.global_tokens;
@@ -566,6 +571,27 @@ def make_diffusers_tome_block(block_class: Type[torch.nn.Module]) -> Type[torch.
     return ToMeBlock
 
 
+def make_library_transformer2d(wrapper_class: Type[torch.nn.Module]) -> Type[torch.nn.Module]:
+    """Patched class for a diffusers Transformer2DModel: the library path of transformer2d.py while FUSE_TRANSFORMER_IO
+    is on and the call is eligible, else the class's own forward.  It does not depend on merging, so it stays on the
+    library path inside _unmerged_blocks() too.  The module gets no `_tome_info`: update_patch and collect_from_patch
+    see what they saw before."""
+
+    class ToMeTransformer2D(wrapper_class):
+        # the original class, restored by remove_patch
+        _parent = wrapper_class
+
+        def forward(self, hidden_states, *args, **kwargs):
+            from . import transformer2d as _t2d
+            # keyword arguments library_forward does not restate (a later diffusers release's) go to the class's forward
+            if (FUSE_TRANSFORMER_IO and not args and _t2d.LIBRARY_KWARGS.issuperset(kwargs)
+                    and _t2d.ineligibility(self, hidden_states) is None):
+                return _t2d.library_forward(self, hidden_states, **kwargs)
+            return super().forward(hidden_states, *args, **kwargs)
+
+    return ToMeTransformer2D
+
+
 def hook_tome_model(model: torch.nn.Module):
     """Forward pre-hook recording the latent size (patch.py:206-212).  The UNet must be called with the
     latent as positional argument 0, as generate.py:275 does."""
@@ -671,6 +697,8 @@ def apply_patch(
                 if not hasattr(module, "use_ada_layer_norm_zero") and is_diffusers:
                     module.use_ada_layer_norm = False
                     module.use_ada_layer_norm_zero = False
+            elif is_diffusers and isinstance_str(module, "Transformer2DModel"):
+                module.__class__ = make_library_transformer2d(module.__class__)
 
     return model
 
@@ -703,7 +731,7 @@ def remove_patch(model: torch.nn.Module):
                 for handle in info["hooks"]:
                     handle.remove()
                 info["hooks"].clear()
-            if module.__class__.__name__ == "ToMeBlock":
+            if module.__class__.__name__ in ("ToMeBlock", "ToMeTransformer2D"):
                 module.__class__ = module._parent
     return roots[-1]
 

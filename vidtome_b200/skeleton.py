@@ -302,6 +302,89 @@ def timestep_embedding(timestep, batch: int, dim: int, device, dtype) -> torch.T
     return torch.cat([torch.cos(args), torch.sin(args)], dim=-1).to(dtype).expand(batch, dim)
 
 
+@dataclass
+class Transformer2DModelOutput:
+    sample: torch.Tensor
+
+
+class Transformer2DModel(nn.Module):
+    """diffusers' Transformer2DModel with continuous input, as SD's UNet builds it around every BasicTransformerBlock:
+    GroupNorm(32, C, eps=1e-6) -> proj_in -> tokens -> transformer_blocks -> NCHW -> proj_out -> + residual, with
+    proj_in / proj_out 1x1 convolutions on the NCHW side (SD1.x) or, with `use_linear_projection`, Linear layers on the
+    token side (SD2.x).  The block is handed in, so that the skeleton's census blocks are the ones that run inside.
+    `torch_calls` counts runs of this torch forward, as tests count `Attention.forward`."""
+
+    torch_calls = 0
+
+    def __init__(self, in_channels: int, block: nn.Module, use_linear_projection: bool = False, norm_num_groups: int = 32):
+        super().__init__()
+        self.is_input_continuous = True
+        self.is_input_vectorized = False
+        self.is_input_patches = False
+        self.use_linear_projection = use_linear_projection
+        self.in_channels = in_channels
+        inner = in_channels
+        self.norm = nn.GroupNorm(norm_num_groups, in_channels, eps=1e-6, affine=True)
+        if use_linear_projection:
+            self.proj_in = nn.Linear(in_channels, inner)
+            self.proj_out = nn.Linear(inner, in_channels)
+        else:
+            self.proj_in = nn.Conv2d(in_channels, inner, kernel_size=1, stride=1, padding=0)
+            self.proj_out = nn.Conv2d(inner, in_channels, kernel_size=1, stride=1, padding=0)
+        self.transformer_blocks = nn.ModuleList([block])
+        with torch.no_grad():             # drawn around (1, 0), so that the affine takes part in a comparison
+            self.norm.weight.normal_(1.0, 0.1)
+            self.norm.bias.normal_(0.0, 0.1)
+
+    def forward(self, hidden_states, encoder_hidden_states=None, timestep=None, cross_attention_kwargs=None,
+                attention_mask=None, encoder_attention_mask=None, class_labels=None, return_dict: bool = True):
+        Transformer2DModel.torch_calls += 1
+        batch, _, height, width = hidden_states.shape
+        residual = hidden_states
+        hidden_states = self.norm(hidden_states)
+        if not self.use_linear_projection:
+            hidden_states = self.proj_in(hidden_states)
+            inner = hidden_states.shape[1]
+            hidden_states = hidden_states.permute(0, 2, 3, 1).reshape(batch, height * width, inner)
+        else:
+            inner = hidden_states.shape[1]
+            hidden_states = hidden_states.permute(0, 2, 3, 1).reshape(batch, height * width, inner)
+            hidden_states = self.proj_in(hidden_states)
+        for block in self.transformer_blocks:
+            hidden_states = block(hidden_states, attention_mask=attention_mask,
+                                  encoder_hidden_states=encoder_hidden_states,
+                                  encoder_attention_mask=encoder_attention_mask, timestep=timestep,
+                                  cross_attention_kwargs=cross_attention_kwargs, class_labels=class_labels)
+        if not self.use_linear_projection:
+            hidden_states = hidden_states.reshape(batch, height, width, inner).permute(0, 3, 1, 2).contiguous()
+            hidden_states = self.proj_out(hidden_states)
+        else:
+            hidden_states = self.proj_out(hidden_states)
+            hidden_states = hidden_states.reshape(batch, height, width, inner).permute(0, 3, 1, 2).contiguous()
+        output = hidden_states + residual
+        if not return_dict:
+            return (output,)
+        return Transformer2DModelOutput(sample=output)
+
+
+def _make_wrappers(blocks, census, transformer_io: Optional[str]) -> Optional[nn.ModuleList]:
+    """One Transformer2DModel per census block (transformer_io "conv" or "linear"), or None."""
+    if transformer_io is None:
+        return None
+    if transformer_io not in ("conv", "linear"):
+        raise ValueError(f"transformer_io must be None, 'conv' or 'linear', got {transformer_io!r}")
+    return nn.ModuleList([Transformer2DModel(s.dim, b, use_linear_projection=transformer_io == "linear")
+                          for s, b in zip(census, blocks)])
+
+
+def _to_nchw(tokens: torch.Tensor, hw: Tuple[int, int]) -> torch.Tensor:
+    return tokens.transpose(1, 2).reshape(tokens.shape[0], -1, *hw).contiguous()
+
+
+def _to_tokens(nchw: torch.Tensor) -> torch.Tensor:
+    return nchw.flatten(2).transpose(1, 2)
+
+
 class ModelMixin(nn.Module):
     """Name-only stand-in for diffusers.ModelMixin (patch.py:279-280 matches the class name)."""
 
@@ -359,10 +442,16 @@ class SkeletonUNet(ModelMixin):
     target of PnP's conv-feature injection, utils/pnp_utils.py:168-169), run ahead of census block 8: it takes the
     state of that resolution concatenated with a skip (the last encoder block's output there, 2C channels, as the
     decoder's skip concatenation), gives C channels back to the state, and gets the sinusoidal embedding of the
-    timestep.  Its weights are drawn after all others, so the rest of the skeleton is the same with and without it."""
+    timestep.  Its weights are drawn after all others, so the rest of the skeleton is the same with and without it.
+
+    `transformer_io="conv"` / `"linear"` adds `wrappers`, one Transformer2DModel around every census block, as diffusers'
+    UNet has: the state of each resolution is then kept NCHW [(B F), C, h, w] and every block is called through its
+    wrapper (additional residuals are NCHW as well, shaped like the wrapper's output).  The wrappers' weights are drawn
+    last of all, so every other parameter is the same with and without them."""
 
     def __init__(self, census: List[BlockSpec], in_channels: int = 4, cross_attention_dim: int = 768,
-                 hot_path_only: bool = True, max_downsample: Optional[int] = None, pnp_conv: bool = False):
+                 hot_path_only: bool = True, max_downsample: Optional[int] = None, pnp_conv: bool = False,
+                 transformer_io: Optional[str] = None):
         super().__init__()
         keep = [i for i, s in enumerate(census) if max_downsample is None or s.downsample <= max_downsample]
         self.census_index = keep                  # position of every block in the full census
@@ -381,12 +470,15 @@ class SkeletonUNet(ModelMixin):
                                  f"census / max_downsample leaves out")
             C = census[PNP_CONV_POSITION].dim
             self.resnet = ResnetBlock2D(2 * C, C, temb_channels=TEMB_CHANNELS)
+        self.wrappers = _make_wrappers(self.blocks, self.census, transformer_io)
 
     def _run_resnet(self, state: torch.Tensor, skip: torch.Tensor, timestep, hw: Tuple[int, int]) -> torch.Tensor:
-        """[(B F), T, C] state and skip -> the ResNet's [(B F), T, C] output."""
+        """[(B F), T, C] state and skip -> the ResNet's [(B F), T, C] output (NCHW in and out with wrappers)."""
         BF = state.shape[0]
-        nchw = lambda t: t.transpose(1, 2).reshape(BF, -1, *hw).contiguous()   # noqa: E731  (NCHW, as diffusers)
         temb = timestep_embedding(timestep, BF, TEMB_CHANNELS, state.device, state.dtype)
+        if self.wrappers is not None:
+            return self.resnet(torch.cat([state, skip], dim=1), temb)
+        nchw = lambda t: t.transpose(1, 2).reshape(BF, -1, *hw).contiguous()   # noqa: E731  (NCHW, as diffusers)
         out = self.resnet(torch.cat([nchw(state), nchw(skip)], dim=1), temb)
         return out.flatten(2).transpose(1, 2).contiguous()
 
@@ -414,16 +506,22 @@ class SkeletonUNet(ModelMixin):
         eps = torch.zeros_like(sample)
         res = self._residuals(down_block_additional_residuals, mid_block_additional_residual)
         skips = {}
-        for pos, spec, block in zip(self.census_index, self.census, self.blocks):
+        for i, (pos, spec, block) in enumerate(zip(self.census_index, self.census, self.blocks)):
             key = f"ds{spec.downsample}"
+            ds = spec.downsample
             if key not in state:
                 pooled = F.avg_pool2d(sample, spec.downsample) if spec.downsample > 1 else sample
                 tok = pooled.flatten(2).transpose(1, 2)                       # [(B F), T, 4]
                 state[key] = self.lift[key](tok)
+                if self.wrappers is not None:
+                    state[key] = _to_nchw(state[key], (H // ds, W // ds))
             if self.resnet is not None and pos == PNP_CONV_POSITION:
-                ds = spec.downsample
                 state[key] = self._run_resnet(state[key], skips.get(key, state[key]), timestep, (H // ds, W // ds))
-            h = block(state[key], encoder_hidden_states=encoder_hidden_states, timestep=timestep)
+            if self.wrappers is not None:
+                h = self.wrappers[i](state[key], encoder_hidden_states=encoder_hidden_states, timestep=timestep,
+                                     return_dict=False)[0]
+            else:
+                h = block(state[key], encoder_hidden_states=encoder_hidden_states, timestep=timestep)
             if pos < self.mid_position:
                 skips[key] = h
             if pos in res:
@@ -434,6 +532,8 @@ class SkeletonUNet(ModelMixin):
             state[key] = h
         for key, h in state.items():
             ds = int(key[2:])
+            if self.wrappers is not None:
+                h = _to_tokens(h)
             out = self.drop[key](h).transpose(1, 2).reshape(BF, Cin, H // ds, W // ds)
             if ds > 1:
                 out = F.interpolate(out, scale_factor=ds, mode="nearest")
@@ -453,7 +553,7 @@ class ControlNetModel(ModelMixin):
     of zeros, so that the residuals are not all zero and their path shows in the UNet's prediction."""
 
     def __init__(self, census: List[BlockSpec], in_channels: int = 4, cond_channels: int = 3,
-                 cross_attention_dim: int = 768, hot_path_only: bool = True):
+                 cross_attention_dim: int = 768, hot_path_only: bool = True, transformer_io: Optional[str] = None):
         super().__init__()
         mid = mid_position(census)
         self.census_index = list(range(mid + 1))
@@ -465,6 +565,8 @@ class ControlNetModel(ModelMixin):
         self.lift = nn.ModuleDict({f"ds{ds}": nn.Linear(in_channels, dim) for ds, dim in dims})
         self.cond_lift = nn.ModuleDict({f"ds{ds}": nn.Linear(cond_channels, dim) for ds, dim in dims})
         self.zero_convs = nn.ModuleList([nn.Linear(s.dim, s.dim) for s in self.census])
+        # as in SkeletonUNet: NCHW state, blocks called through their Transformer2DModel, NCHW residuals out
+        self.wrappers = _make_wrappers(self.blocks, self.census, transformer_io)
 
     def forward(self, sample: torch.Tensor, timestep=None, encoder_hidden_states=None, controlnet_cond=None,
                 return_dict: bool = False):
@@ -477,13 +579,20 @@ class ControlNetModel(ModelMixin):
             raise ValueError(f"controlnet_cond {tuple(controlnet_cond.shape[2:])} is not a whole multiple of the "
                              f"latent {h}x{w}")
         state, outs = {}, []
-        for spec, block, zero_conv in zip(self.census, self.blocks, self.zero_convs):
+        for i, (spec, block, zero_conv) in enumerate(zip(self.census, self.blocks, self.zero_convs)):
             key, ds = f"ds{spec.downsample}", spec.downsample
             if key not in state:
                 pooled = F.avg_pool2d(sample, ds) if ds > 1 else sample
                 cpooled = F.avg_pool2d(controlnet_cond, f * ds) if f * ds > 1 else controlnet_cond
                 state[key] = (self.lift[key](pooled.flatten(2).transpose(1, 2))
                               + self.cond_lift[key](cpooled.flatten(2).transpose(1, 2)))
+                if self.wrappers is not None:
+                    state[key] = _to_nchw(state[key], (h // ds, w // ds))
+            if self.wrappers is not None:
+                state[key] = self.wrappers[i](state[key], encoder_hidden_states=encoder_hidden_states,
+                                              timestep=timestep, return_dict=False)[0]
+                outs.append(_to_nchw(zero_conv(_to_tokens(state[key])), (h // ds, w // ds)))
+                continue
             state[key] = block(state[key], encoder_hidden_states=encoder_hidden_states, timestep=timestep)
             outs.append(zero_conv(state[key]))
         down, mid = outs[:-1], outs[-1]
@@ -519,28 +628,30 @@ def pnp_conv_module(net: SkeletonUNet) -> nn.Module:
 
 
 def make_skeleton(name: str = "sd15", hot_path_only: bool = True, max_downsample: Optional[int] = None,
-                  device="cuda", dtype=torch.float16, seed: int = 123, pnp_conv: bool = False) -> SkeletonUNet:
+                  device="cuda", dtype=torch.float16, seed: int = 123, pnp_conv: bool = False,
+                  transformer_io: Optional[str] = None) -> SkeletonUNet:
     census = CENSUSES[name]()
     cad = 1024 if name == "sd21" else 768
     gen_state = torch.get_rng_state()
     torch.manual_seed(seed)
     try:
         net = SkeletonUNet(census, cross_attention_dim=cad, hot_path_only=hot_path_only,
-                           max_downsample=max_downsample, pnp_conv=pnp_conv)
+                           max_downsample=max_downsample, pnp_conv=pnp_conv, transformer_io=transformer_io)
     finally:
         torch.set_rng_state(gen_state)
     return net.to(device=device, dtype=dtype).eval()
 
 
 def make_controlnet(name: str = "sd15", hot_path_only: bool = True, device="cuda", dtype=torch.float16,
-                    seed: int = 321) -> ControlNetModel:
+                    seed: int = 321, transformer_io: Optional[str] = None) -> ControlNetModel:
     """The ControlNet stand-in for make_skeleton(name): the encoder half of the same census, seeded the same way."""
     census = CENSUSES[name]()
     cad = 1024 if name == "sd21" else 768
     gen_state = torch.get_rng_state()
     torch.manual_seed(seed)
     try:
-        net = ControlNetModel(census, cross_attention_dim=cad, hot_path_only=hot_path_only)
+        net = ControlNetModel(census, cross_attention_dim=cad, hot_path_only=hot_path_only,
+                              transformer_io=transformer_io)
     finally:
         torch.set_rng_state(gen_state)
     return net.to(device=device, dtype=dtype).eval()
