@@ -11,6 +11,11 @@
  *     passed as void* (torch.cuda.current_stream().cuda_stream);
  *   - token matrices are fp16, row-major, rows of C contiguous halfs, C % 8 == 0, 16-byte aligned;
  *   - index maps are int32; "batch stride 0" means one map shared by all samples (align_batch);
+ *   - alignment, where an entry point below states none: GEMM operands (A, W, bias, resid, D, LoRA down / up), the
+ *     attention entry points' x, ctx, weights, bias, resid and y, and every workspace are 16-byte aligned (they are read
+ *     through TMA tensor maps or 16-byte vector accesses); row strides (ldd, ldr, K, C) are multiples of 8 halfs.
+ *     Index maps, keys and the other int32 / int64 / fp32 buffers are aligned to their element size.  Results do not
+ *     depend on where a buffer sits beyond that, nor on what a workspace held before the call, except where stated;
  *   - the functions never allocate, never synchronise the stream, and never throw; the only process-wide
  *     state is a handful of write-once memoised lookups (driver entry point, SM count, per-kernel shared-memory opt-in
  *     and occupancy), immutable after first use, so calls are re-entrant across streams and devices;
@@ -464,7 +469,9 @@ int vtm_ddim_update_f16(void* x_dev, const void* eps_dev, int64_t n, const float
  *
  * vtm_group_norm_stats_f16: stats_dev [n, groups, 2] fp32 = (mean, rstd) of every (sample, group), a contiguous run of
  *   (C / groups) * HW halfs; rstd = 1 / sqrt(var + eps) with the biased variance; fp32 throughout, combined pairwise
- *   (Chan et al.) so that a large mean does not cancel.  stats_dev 8-byte aligned, eps >= 0.  Workspace:
+ *   (Chan et al.) so that a large mean does not cancel.  The partial sums start at x's first 16-byte boundary, so their
+ *   rounding depends on x's offset from one: calls with the same offset agree bit for bit.  stats_dev 8-byte aligned,
+ *   eps >= 0.  Workspace:
  *   vtm_group_norm_stats_workspace_bytes(n, C, HW, groups) (0 unless long runs are split over CTAs; VTM_E_WS).
  * vtm_group_norm_tokens_f16: y_dev [n, HW, C] fp16 token-major, 16-byte aligned, C % 8 == 0,
  *   y[i, p, c] = fp16(fma((float(x[i, c, p]) - mean) * rstd, gamma[c], beta[c])) with fp32 round-to-nearest steps;
@@ -472,7 +479,8 @@ int vtm_ddim_update_f16(void* x_dev, const void* eps_dev, int64_t n, const float
  * vtm_linear_nchw_residual_f16: D[i, o, p] = fp16(fp16(sum_k A[i HW + p, k] W[o, k] + bias[o]) + R[i, o, p]),
  *   a_dev [n * HW, K] token-major rows, w_dev [N, K], bias_dev [N] or NULL, resid_dev [n, N, HW] or NULL, d_dev
  *   [n, N, HW]; K % 8 == 0, N % 8 == 0.  The mainloop, the bias and the two roundings are vtm_linear_residual_f16's:
- *   the result equals that entry's followed by a transpose, bit for bit.  d_dev may equal resid_dev.
+ *   the result equals that entry's followed by a transpose, bit for bit.  d_dev may equal resid_dev.  d_dev and resid_dev
+ *   need only be 2-byte aligned (16-byte aligned with HW % 8 == 0 takes the vector stores); the result is the same.
  */
 size_t vtm_group_norm_stats_workspace_bytes(int32_t n, int32_t C, int32_t HW, int32_t groups);
 int vtm_group_norm_stats_f16(const void* x_dev, int32_t n, int32_t C, int32_t HW, int32_t groups, float eps,

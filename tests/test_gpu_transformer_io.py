@@ -75,12 +75,15 @@ def _stats_steps(R, runs):
     return -(-piece // (8 * 256)) + 2 + 5 + 8 + S
 
 
-def _check_stats(x, groups, eps=1e-6, what=""):
+def _check_stats(x, groups, eps=1e-6, what="", got=None):
     """Every pairwise update rounds a handful of fp32 operations: after `steps` of them the mean is off by at most
     steps * 4 u max|x|, and M2 (a sum of squared deviations, never a difference of large sums) by steps * 8 u relative
-    plus what the mean's error moves it by, 4 max|x - mean| e_mean."""
+    plus what the mean's error moves it by, 4 max|x - mean| e_mean.  `got`: statistics the caller computed (else they
+    are computed here)."""
     n, C, HW = x.shape
-    got, ws_bytes = _stats(x, groups, eps)
+    ws_bytes = None
+    if got is None:
+        got, ws_bytes = _stats(x, groups, eps)
     x64 = x.double().view(n, groups, -1)
     R = x64.shape[-1]
     mean = x64.mean(-1)
