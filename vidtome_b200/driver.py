@@ -9,11 +9,12 @@ Restates, on synthetic latents, the parts of the reference's Generator that sit 
   init_pnp        generate.py:313-319   (PnP self-attention and conv-feature injection schedules; with `source_latents`)
   pre_iter        generate.py:226-231   (PnP: set the timestep, fetch the source latents of the step)
   ControlNet      generate.py:56-63,264-275, utils/utils.py:280-295 (residuals of `controlnet`, with `control_images`)
+  SD2-depth       generate.py:131-132,255-262 (each frame's depth map appended to the UNet input, with `depth`)
 and, in ChunkedInverter, the reference's Inverter around its hot path:
   ddim_inversion  invert.py:117-140     (reversed timesteps, frame batches, the kept latents)
-  pred_noise      invert.py:159-179     (UNet forward, optional ControlNet residuals)
+  pred_noise      invert.py:159-179     (UNet forward, optional depth channel, optional ControlNet residuals)
   pred_next_x     invert.py:182-211     (inversion=True branch)
-Text conditioning, VAE, ControlNet preprocessing and file IO are outside the hot path and not restated.
+Text conditioning, VAE, ControlNet and depth preprocessing and file IO are outside the hot path and not restated.
 """
 from __future__ import annotations
 
@@ -39,6 +40,32 @@ def ddim_timesteps(n_timesteps: int, num_train_timesteps: int = 1000) -> List[in
     return [int(t) + 1 for t in (np.arange(0, n_timesteps) * ratio).round()[::-1]]
 
 
+def _rows(frames: dict, lo: int, hi: int) -> dict:
+    """Frames lo..hi-1 of every per-frame input ({"src" | "ctrl" | "depth": [flen, ...]}) of a step."""
+    return {k: v[lo:hi] for k, v in frames.items()}
+
+
+def _check_depth_arg(depth: Optional[torch.Tensor], controlnet: Optional[torch.nn.Module]):
+    if depth is None:
+        return
+    if depth.dim() != 4 or depth.shape[1] != 1:
+        raise ValueError(f"depth must be [flen, 1, h, w] (got {tuple(depth.shape)})")
+    if controlnet is not None:
+        raise ValueError("depth and controlnet are exclusive: the reference's ControlNets are SD1.5 models with a "
+                         "4-channel input, and its configs use no control with the depth model")
+
+
+def _check_depth(depth: torch.Tensor, x: torch.Tensor, model: torch.nn.Module):
+    """One depth map per frame at the latents' resolution, for a model that takes the latent channels + 1."""
+    if len(depth) != len(x) or depth.shape[2:] != x.shape[2:]:
+        raise ValueError(f"depth is {tuple(depth.shape)}, the latents {tuple(x.shape)}: it needs one map per frame at "
+                         f"the latents' resolution")
+    n = getattr(getattr(model, "config", None), "in_channels", getattr(model, "in_channels", None))
+    if isinstance(n, int) and n != x.shape[1] + 1:
+        raise ValueError(f"depth: the model takes {n} input channels, not the latents' {x.shape[1]} and one depth "
+                         f"channel")
+
+
 class ChunkedDenoiser:
     """Chunked classifier-free-guidance DDIM sampling on a (patched) UNet, generate.py:205-311."""
 
@@ -50,7 +77,7 @@ class ChunkedDenoiser:
                  pnp_attn_t: float = 0.5, pnp_modules: Optional[Iterable[torch.nn.Module]] = None,
                  controlnet: Optional[torch.nn.Module] = None, control_images: Optional[torch.Tensor] = None,
                  control_scale: float = 1.0, pnp_f_t: Optional[float] = None,
-                 pnp_conv_modules: Optional[Iterable[torch.nn.Module]] = None):
+                 pnp_conv_modules: Optional[Iterable[torch.nn.Module]] = None, depth: Optional[torch.Tensor] = None):
         """`cuda_graph=True`: after `graph_warmup` eager steps, the noise prediction of a whole step (every chunk:
         CFG batch, UNet forward with the merge path, guidance combine) is captured once into a CUDA graph and
         replayed; per step the host then issues one graph launch plus the DDIM update instead of ~250 kernel
@@ -101,7 +128,17 @@ class ChunkedDenoiser:
         patched too (apply_patch(include_control=True) on a StableDiffusionControlNetPipeline); its blocks then draw
         from their own generators and keep their own global tokens, which every graph mode registers and resets like
         the UNet's.  The control images are a static input of every graph.  One control mode at a time: ControlNet
-        and PnP (`source_latents`) are refused together, as the reference takes one (generate.py:61-68)."""
+        and PnP (`source_latents`) are refused together, as the reference takes one (generate.py:61-68).
+
+        `depth` ([flen, 1, h, w], the reference's prepare_depth output: one depth map per frame at latent resolution,
+        normalised to [-1, 1]) runs SD2-depth (stabilityai/stable-diffusion-2-depth, `sd_version: "depth"`), whose UNet
+        takes 5 input channels: every UNet call gets the chunk's depth maps, cast to the latents' dtype (generate.py:
+        131-132), repeated over the batch ([x | x], or [source | x | x] with PnP) and appended as a fifth channel
+        (generate.py:255-262).  Depth combines with PnP (the reference's default `control: "pnp"`) and with every graph
+        mode, in each of which the depth maps are a static input like the control images; graph keys do not change.
+        Depth with `controlnet` is refused: the reference's ControlNets are SD1.5 models with a 4-channel input."""
+        _check_depth_arg(depth, controlnet)
+        self.depth = depth
         if controlnet is not None and source_latents is not None:
             raise ValueError("controlnet and source_latents (PnP) are exclusive: the reference runs one control mode "
                              "(generate.py:61-68)")
@@ -119,7 +156,8 @@ class ChunkedDenoiser:
         self.shard = bool(shard)
         self.cuda_graph = bool(cuda_graph)
         self.graph_warmup = int(graph_warmup)
-        self._graph = None          # (CUDAGraph, static x, static timestep, static noise, shape[, slot index state])
+        self._graph = None          # (CUDAGraph, static x, static timestep, static noise, key[, slot index state],
+                                    #  static per-frame inputs)
         self._eager_steps = 0
         self.capture_global = bool(capture_global)
         self.chunk_graphs = bool(chunk_graphs)
@@ -137,7 +175,7 @@ class ChunkedDenoiser:
         if self.capture_global and self.shard:
             raise ValueError("capture_global=True does not capture the cross-rank exchange of shard=True")
         # (chunk length, first in step, frame shape, PnP injection[, PnP conv injection when pnp_f_t is set])
-        #   -> (CUDAGraph, static x, static noise, static source, static control images)
+        #   -> (CUDAGraph, static x, static noise, static per-frame inputs {"src" | "ctrl" | "depth": tensor})
         self._chunk_graphs = {}
         self._chunk_t = None        # the UNet's timestep input shared by the chunk graphs
         self._stores = []           # patch.GlobalTokenStore of every block (chunk_graphs with merge_global)
@@ -230,9 +268,9 @@ class ChunkedDenoiser:
     # generate.py:238-279
     @torch.no_grad()
     def pred_noise(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None,
-                   ctrl: Optional[torch.Tensor] = None) -> torch.Tensor:
+                   ctrl: Optional[torch.Tensor] = None, depth: Optional[torch.Tensor] = None) -> torch.Tensor:
         """`src`: the source latents of the chunk (PnP), prepended to the batch.  `ctrl`: the control images of the
-        chunk (ControlNet)."""
+        chunk (ControlNet).  `depth`: the depth maps of the chunk (SD2-depth), appended to every sample as a channel."""
         flen = len(x)
         text = None if self.cond is None else self.cond.repeat_interleave(flen, dim=0)
         latent_model_input = torch.cat([x, x])                                # classifier-free guidance
@@ -240,6 +278,8 @@ class ChunkedDenoiser:
         if src is not None:
             latent_model_input = torch.cat([src.to(x), latent_model_input])
             batch_size += 1
+        if depth is not None:                                                 # generate.py:256-262
+            latent_model_input = torch.cat([latent_model_input, depth.repeat(batch_size, 1, 1, 1).to(x)], dim=1)
         kwargs = {}
         if ctrl is not None:                                                  # generate.py:264-273
             controlnet_cond = ctrl.repeat(batch_size, 1, 1, 1)
@@ -276,15 +316,15 @@ class ChunkedDenoiser:
                                    "use 'allgather' for ragged chunks")
         return chunks
 
-    def _all_noises(self, x: torch.Tensor, t, src: Optional[torch.Tensor] = None,
-                    ctrl: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _all_noises(self, x: torch.Tensor, t, frames: dict) -> torch.Tensor:
+        """`frames`: the step's per-frame inputs besides the latents, {"src" | "ctrl" | "depth": [flen, ...]} (those in
+        use), passed to pred_noise under these names."""
         noises = torch.zeros_like(x)
         for chunk in self._step_chunks(len(x)):
             # chunks are contiguous frame ranges (possibly visited in another order): slice instead of indexing with
             # a host tensor, which would cost a synchronous host->device copy per chunk per step
             lo, hi = int(chunk[0]), int(chunk[-1]) + 1
-            noises[lo:hi] = self.pred_noise(x[lo:hi], t, None if src is None else src[lo:hi],
-                                            None if ctrl is None else ctrl[lo:hi])
+            noises[lo:hi] = self.pred_noise(x[lo:hi], t, **_rows(frames, lo, hi))
         return noises
 
     def _models(self) -> List[torch.nn.Module]:
@@ -306,22 +346,21 @@ class ChunkedDenoiser:
             return tuple(x.shape), self.injecting(t)
         return tuple(x.shape), self.injecting(t), self.conv_injecting(t)
 
-    def _capture(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor], ctrl: Optional[torch.Tensor]):
+    def _capture(self, x: torch.Tensor, t: int, frames: dict):
         """Capture `_all_noises` for inputs shaped like `x` (called after the eager warm-up steps, so that every
         lazily created piece of state — generators forked by the hook, cached packed weights, the library handle,
         allocator pools — already exists)."""
         self._graph = None                                                   # release the previous graph first
         gx = x.clone()
-        gsrc = None if src is None else src.to(x).clone()                    # the source latents, set per replay
-        gctrl = None if ctrl is None else ctrl.clone()                       # the control images, set per replay
+        gframes = {k: v.clone() for k, v in frames.items()}                # the per-frame inputs, set per replay
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)      # the UNet's timestep input, set per replay
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = self._all_noises(gx, gt, gsrc, gctrl)
-        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gsrc, gctrl)
+            gn = self._all_noises(gx, gt, gframes)
+        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gframes)
 
     @staticmethod
     def slot_index(chunks: List[torch.Tensor], flen: int) -> torch.Tensor:
@@ -337,7 +376,7 @@ class ChunkedDenoiser:
             raise RuntimeError("slot_index: the chunks must cover every frame exactly once")
         return torch.stack([fwd, inv])
 
-    def _capture_slots(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor], ctrl: Optional[torch.Tensor]):
+    def _capture_slots(self, x: torch.Tensor, t: int, frames: dict):
         """Capture the noise prediction of one step over chunk slots (capture_global=True): slot k runs chunk k of the
         step's visiting order on gx[k * chunk_size:(k + 1) * chunk_size].  get_chunks is not called here, so capturing
         consumes no draw of the host RNG that eager stepping would not."""
@@ -347,8 +386,7 @@ class ChunkedDenoiser:
                                f"{patch.GLOBAL_EXCHANGE!r}): the cross-rank exchange is not captured")
         self._graph = None                                                   # release the previous graph first
         gx = x.clone()
-        gsrc = None if src is None else src.to(x).clone()                   # source latents in slot order
-        gctrl = None if ctrl is None else ctrl.clone()                      # control images in slot order
+        gframes = {k: v.clone() for k, v in frames.items()}                # the per-frame inputs in slot order
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
@@ -359,33 +397,29 @@ class ChunkedDenoiser:
         with torch.cuda.graph(graph):
             gn = torch.zeros_like(gx)
             for k in range(flen // cs):
-                s = slice(k * cs, (k + 1) * cs)
-                gn[s] = self.pred_noise(gx[s], gt, None if gsrc is None else gsrc[s],
-                                        None if gctrl is None else gctrl[s])
+                lo, hi = k * cs, (k + 1) * cs
+                gn[lo:hi] = self.pred_noise(gx[lo:hi], gt, **_rows(gframes, lo, hi))
         idx_dev = torch.empty((2, flen), dtype=torch.int64, device=x.device)
         idx_host = torch.empty((2, flen), dtype=torch.int64).pin_memory()
         copied = torch.cuda.Event()          # the pinned buffer is rewritten only after its last upload has run
-        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), idx_dev, idx_host, copied, gsrc, gctrl)
+        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), idx_dev, idx_host, copied, gframes)
 
-    def _slot_noises(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None,
-                     ctrl: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _slot_noises(self, x: torch.Tensor, t: int, frames: dict) -> torch.Tensor:
         flen = len(x)
         if flen % self.chunk_size != 0:
             raise RuntimeError(f"capture_global=True needs a frame count divisible by chunk_size (got {flen} frames, "
                                f"chunk_size {self.chunk_size}): chunks of unequal length cannot share one graph")
         order = self.slot_index(self.get_chunks(flen), flen)        # the same host draws as eager stepping
         if self._graph is None or self._graph[4] != self._graph_key(x, t):
-            self._capture_slots(x, t, src, ctrl)
-        graph, gx, gt, gn, _, idx_dev, idx_host, copied, gsrc, gctrl = self._graph
+            self._capture_slots(x, t, frames)
+        graph, gx, gt, gn, _, idx_dev, idx_host, copied, gframes = self._graph
         copied.synchronize()
         idx_host.copy_(order)
         idx_dev.copy_(idx_host, non_blocking=True)
         copied.record()
         torch.index_select(x, 0, idx_dev[0], out=gx)                # latents -> slots
-        if gsrc is not None:
-            torch.index_select(src.to(x), 0, idx_dev[0], out=gsrc)
-        if gctrl is not None:
-            torch.index_select(ctrl, 0, idx_dev[0], out=gctrl)
+        for k, g in gframes.items():
+            torch.index_select(frames[k], 0, idx_dev[0], out=g)
         gt.fill_(int(t))
         graph.replay()
         return torch.index_select(gn, 0, idx_dev[1])                # slots -> frames
@@ -451,12 +485,11 @@ class ChunkedDenoiser:
             for model in self._models():
                 patch.update_patch(model, global_tokens=None)
 
-    def _capture_chunk(self, key, x: torch.Tensor, src: Optional[torch.Tensor], ctrl: Optional[torch.Tensor]):
-        """Capture the noise prediction of one chunk shaped like `x`; `key[1]` says whether it is the first chunk of a
-        step, i.e. whether the blocks' stores are empty when it runs."""
+    def _capture_chunk(self, key, x: torch.Tensor, frames: dict):
+        """Capture the noise prediction of one chunk shaped like `x` (with the chunk's rows of the per-frame inputs);
+        `key[1]` says whether it is the first chunk of a step, i.e. whether the blocks' stores are empty when it runs."""
         gx = x.clone()
-        gsrc = None if src is None else src.to(x).clone()
-        gctrl = None if ctrl is None else ctrl.clone()
+        gframes = {k: v.clone() for k, v in frames.items()}
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
@@ -464,12 +497,11 @@ class ChunkedDenoiser:
             st.filled = not key[1]
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = self.pred_noise(gx, self._chunk_t, gsrc, gctrl)
-        self._chunk_graphs[key] = (graph, gx, gn, gsrc, gctrl)
+            gn = self.pred_noise(gx, self._chunk_t, **gframes)
+        self._chunk_graphs[key] = (graph, gx, gn, gframes)
         return self._chunk_graphs[key]
 
-    def _chunk_graph_noises(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None,
-                            ctrl: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _chunk_graph_noises(self, x: torch.Tensor, t: int, frames: dict) -> torch.Tensor:
         flen = len(x)
         chunks = self.get_chunks(flen)                                      # the same host draws as eager stepping
         if not self._chunk_graphs:
@@ -493,14 +525,11 @@ class ChunkedDenoiser:
                 key = key + (conv,)
             entry = self._chunk_graphs.get(key)
             if entry is None:
-                entry = self._capture_chunk(key, x[lo:hi], None if src is None else src[lo:hi],
-                                            None if ctrl is None else ctrl[lo:hi])
-            graph, gx, gn, gsrc, gctrl = entry
+                entry = self._capture_chunk(key, x[lo:hi], _rows(frames, lo, hi))
+            graph, gx, gn, gframes = entry
             gx.copy_(x[lo:hi])
-            if gsrc is not None:
-                gsrc.copy_(src[lo:hi])
-            if gctrl is not None:
-                gctrl.copy_(ctrl[lo:hi])
+            for name, g in gframes.items():
+                g.copy_(frames[name][lo:hi])
             graph.replay()
             noises[lo:hi].copy_(gn)
         return noises
@@ -509,37 +538,37 @@ class ChunkedDenoiser:
     @torch.no_grad()
     def step(self, x: torch.Tensor, i: int) -> torch.Tensor:
         t = self.timesteps[i]
-        src = None
+        frames = {}                                                          # the per-frame inputs, cast to x's dtype
+        if self.depth is not None:
+            _check_depth(self.depth, x, self.unet)
         if self.source_latents is not None:                                 # generate.py:226-231 (pre_iter)
             pnp.register_time(self.unet, t, modules=self._pnp_targets)
-            src = self.source_latents(t)
-        ctrl = None
+            frames["src"] = self.source_latents(t).to(x)
         if self.controlnet is not None:
             if len(self.control_images) != len(x):
                 raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
-            ctrl = self.control_images.to(x)                                # prepare_data's .to(self.init_noise)
+            frames["ctrl"] = self.control_images.to(x)                      # prepare_data's .to(self.init_noise)
+        if self.depth is not None:
+            frames["depth"] = self.depth.to(x)                              # prepare_data's .to(self.init_noise)
         if self.chunk_graphs and self.merge_global and x.is_cuda and not self._stores:
             self._install_stores()
         if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.chunk_graphs:
-            noises = self._chunk_graph_noises(x, t, src, ctrl)
+            noises = self._chunk_graph_noises(x, t, frames)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.capture_global:
-            noises = self._slot_noises(x, t, src, ctrl)
+            noises = self._slot_noises(x, t, frames)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup:
             if self._graph is None or self._graph[4] != self._graph_key(x, t):
-                self._capture(x, t, src, ctrl)
-            graph, gx, gt, gn = self._graph[:4]
-            gsrc, gctrl = self._graph[5:7]
+                self._capture(x, t, frames)
+            graph, gx, gt, gn, _, gframes = self._graph
             gx.copy_(x, non_blocking=True)
-            if gsrc is not None:
-                gsrc.copy_(src, non_blocking=True)
-            if gctrl is not None:
-                gctrl.copy_(ctrl, non_blocking=True)
+            for k, g in gframes.items():
+                g.copy_(frames[k], non_blocking=True)
             gt.fill_(int(t))
             graph.replay()
             noises = gn
         else:
             self._eager_steps += 1
-            noises = self._all_noises(x, t, src, ctrl)
+            noises = self._all_noises(x, t, frames)
         x = self.pred_next_x(x, noises, i)
         if self.merge_global:
             self._reset_global()
@@ -574,12 +603,18 @@ class ChunkedInverter:
     `cuda_graph=True` (CUDA fp16 latents): after `graph_warmup` eager steps one CUDA graph covers a whole step, i.e.
     every batch's ControlNet and UNet call and KI with the trajectory store.  The UNet's timestep input, KI's
     coefficients and its trajectory slot are read on the device from a step counter the graph advances, so each further
-    step is one replay, bit-identical to eager stepping."""
+    step is one replay, bit-identical to eager stepping.
+
+    `depth` ([F, 1, h, w], the reference's prepare_depth output) inverts with SD2-depth's 5-channel UNet: every UNet call
+    gets the batch's latents with its depth maps appended as a fifth channel, cast to the latents' dtype
+    (invert.py:161-166), eagerly and in the captured step.  The update and the trajectory keep the 4 latent channels.
+    Depth with `controlnet` is refused, as in ChunkedDenoiser."""
 
     def __init__(self, unet: torch.nn.Module, n_timesteps: int = 50, batch_size: int = 8,
                  save_steps: Optional[int] = None, save_intermediate: bool = True, cond: Optional[torch.Tensor] = None,
                  controlnet: Optional[torch.nn.Module] = None, control_images: Optional[torch.Tensor] = None,
-                 control_scale: float = 1.0, cuda_graph: bool = False, graph_warmup: int = 2):
+                 control_scale: float = 1.0, cuda_graph: bool = False, graph_warmup: int = 2,
+                 depth: Optional[torch.Tensor] = None):
         if not isinstance(n_timesteps, int) or n_timesteps <= 0:
             raise ValueError(f"n_timesteps must be a positive int (got {n_timesteps!r})")
         if not isinstance(batch_size, int) or batch_size <= 0:
@@ -596,6 +631,8 @@ class ChunkedInverter:
         if cuda_graph and int(graph_warmup) < 1:
             raise ValueError(f"cuda_graph=True needs graph_warmup >= 1 (got {graph_warmup!r}): the modules' packed "
                              f"weights are created by an eager step, outside the graph's memory pool")
+        _check_depth_arg(depth, controlnet)
+        self.depth = depth
         self.unet = unet
         self.batch_size = batch_size
         self.cond = cond
@@ -640,7 +677,10 @@ class ChunkedInverter:
 
     # invert.py:159-179
     @torch.no_grad()
-    def pred_noise(self, x: torch.Tensor, cond: Optional[torch.Tensor], t, ctrl: Optional[torch.Tensor] = None):
+    def pred_noise(self, x: torch.Tensor, cond: Optional[torch.Tensor], t, ctrl: Optional[torch.Tensor] = None,
+                   depth: Optional[torch.Tensor] = None):
+        if depth is not None:                                               # invert.py:161-166
+            x = torch.cat([x, depth.to(x)], dim=1)
         kwargs = {}
         if ctrl is not None:                                                # utils/utils.py:280-295
             down, mid = self.controlnet(x, t, encoder_hidden_states=cond, controlnet_cond=ctrl, return_dict=False)
@@ -658,13 +698,13 @@ class ChunkedInverter:
             raise ValueError(f"cond has {self.cond.shape[0]} rows for {flen} frames (one per frame, or one for all)")
         return self.cond[lo:hi]
 
-    def _all_noises(self, x: torch.Tensor, t, ctrl: Optional[torch.Tensor], out: Optional[torch.Tensor] = None):
+    def _all_noises(self, x: torch.Tensor, t, frames: dict, out: Optional[torch.Tensor] = None):
+        """`frames`: the per-frame inputs besides the latents, {"ctrl" | "depth": [F, ...]} (those in use)."""
         flen = len(x)
         noises = torch.empty_like(x) if out is None else out
         for lo in range(0, flen, self.batch_size):                         # invert.py:124-129
             hi = min(lo + self.batch_size, flen)
-            noises[lo:hi] = self.pred_noise(x[lo:hi], self._batch_cond(lo, hi, flen), t,
-                                            None if ctrl is None else ctrl[lo:hi])
+            noises[lo:hi] = self.pred_noise(x[lo:hi], self._batch_cond(lo, hi, flen), t, **_rows(frames, lo, hi))
         return noises
 
     def _device_tables(self, x: torch.Tensor):
@@ -681,11 +721,14 @@ class ChunkedInverter:
         `trajectory`); `x` itself is not modified."""
         if x.dim() != 4:
             raise ValueError(f"latents must be [F, 4, h, w] (got {tuple(x.shape)})")
-        ctrl = None
+        frames = {}
         if self.controlnet is not None:
             if len(self.control_images) != len(x):
                 raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
-            ctrl = self.control_images.to(x)
+            frames["ctrl"] = self.control_images.to(x)
+        if self.depth is not None:
+            _check_depth(self.depth, x, self.unet)
+            frames["depth"] = self.depth.to(x)
         if self.cond is not None:
             self._batch_cond(0, 0, len(x))                                 # check the row count up front
         kernel = x.is_cuda and x.dtype == torch.float16
@@ -696,24 +739,24 @@ class ChunkedInverter:
         scope = patch._unmerged_blocks() if self._patched() else contextlib.nullcontext()
         with scope:
             if kernel:
-                self._invert_device(x, ctrl, traj)
+                self._invert_device(x, frames, traj)
             else:
                 with torch.autocast(x.device.type, dtype=torch.float16, enabled=x.is_cuda):
                     for i, t in enumerate(self.timesteps):
-                        x = self.pred_next_x(x, self._all_noises(x, t, ctrl), i)
+                        x = self.pred_next_x(x, self._all_noises(x, t, frames), i)
                         if self.slots[i] >= 0:
                             traj[self.slots[i]] = x
         self.trajectory = traj
         return traj[-1]
 
-    def _invert_device(self, x: torch.Tensor, ctrl: Optional[torch.Tensor], traj: torch.Tensor):
+    def _invert_device(self, x: torch.Tensor, frames: dict, traj: torch.Tensor):
         from . import ops
         coef, slots, ts, step = self._device_tables(x)
         n = len(self.timesteps)
         eager = n if not self.cuda_graph else min(self.graph_warmup, n)
         with torch.autocast("cuda", dtype=torch.float16):
             for i in range(eager):
-                eps = self._all_noises(x, self.timesteps[i], ctrl)
+                eps = self._all_noises(x, self.timesteps[i], frames)
                 ops.ddim_update(x, eps, coef, step, slots, traj)
                 step.add_(1)
         if eager == n:
@@ -722,7 +765,7 @@ class ChunkedInverter:
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph), torch.autocast("cuda", dtype=torch.float16, cache_enabled=False):
             gt = torch.index_select(ts, 0, step)                          # the UNet's timestep input, [1]
-            eps = self._all_noises(x, gt, ctrl)
+            eps = self._all_noises(x, gt, frames)
             ops.ddim_update(x, eps, coef, step, slots, traj)
             step.add_(1)
         for _ in range(eager, n):

@@ -429,8 +429,8 @@ def mid_position(census: List[BlockSpec]) -> int:
 
 
 class SkeletonUNet(ModelMixin):
-    """forward(latent [(B F), 4, h, w], t, encoder_hidden_states) -> object with `.sample` of the latent's
-    shape.  For every block: the latent is average-pooled to the block's resolution, lifted to `dim`
+    """forward(latent [(B F), in_channels, h, w], t, encoder_hidden_states) -> object with `.sample`
+    [(B F), out_channels, h, w].  For every block: the latent is average-pooled to the block's resolution, lifted to `dim`
     channels by a fixed linear map, added to the running state of that resolution, run through the block,
     and projected back into the noise prediction.
 
@@ -447,22 +447,27 @@ class SkeletonUNet(ModelMixin):
     `transformer_io="conv"` / `"linear"` adds `wrappers`, one Transformer2DModel around every census block, as diffusers'
     UNet has: the state of each resolution is then kept NCHW [(B F), C, h, w] and every block is called through its
     wrapper (additional residuals are NCHW as well, shaped like the wrapper's output).  The wrappers' weights are drawn
-    last of all, so every other parameter is the same with and without them."""
+    last of all, so every other parameter is the same with and without them.
+
+    `out_channels` (default: `in_channels`) is the channel count of the prediction.  SD2-depth's UNet takes the 4 latent
+    channels and a depth channel and predicts the 4 latent channels: in_channels 5, out_channels 4
+    (make_skeleton(..., depth=True))."""
 
     def __init__(self, census: List[BlockSpec], in_channels: int = 4, cross_attention_dim: int = 768,
                  hot_path_only: bool = True, max_downsample: Optional[int] = None, pnp_conv: bool = False,
-                 transformer_io: Optional[str] = None):
+                 transformer_io: Optional[str] = None, out_channels: Optional[int] = None):
         super().__init__()
         keep = [i for i, s in enumerate(census) if max_downsample is None or s.downsample <= max_downsample]
         self.census_index = keep                  # position of every block in the full census
         self.census = [census[i] for i in keep]
         self.mid_position = mid_position(census)
         self.in_channels = in_channels
+        self.out_channels = in_channels if out_channels is None else out_channels
         self.blocks = nn.ModuleList(
             [BasicTransformerBlock(s.dim, s.heads, cross_attention_dim, hot_path_only) for s in self.census])
         dims = sorted({(s.downsample, s.dim) for s in self.census})
         self.lift = nn.ModuleDict({f"ds{ds}": nn.Linear(in_channels, dim) for ds, dim in dims})
-        self.drop = nn.ModuleDict({f"ds{ds}": nn.Linear(dim, in_channels) for ds, dim in dims})
+        self.drop = nn.ModuleDict({f"ds{ds}": nn.Linear(dim, self.out_channels) for ds, dim in dims})
         self.resnet = None
         if pnp_conv:
             if PNP_CONV_POSITION not in keep:
@@ -501,9 +506,9 @@ class SkeletonUNet(ModelMixin):
 
     def forward(self, sample: torch.Tensor, timestep=None, encoder_hidden_states=None,
                 down_block_additional_residuals=None, mid_block_additional_residual=None, **kwargs):
-        BF, Cin, H, W = sample.shape
+        BF, _, H, W = sample.shape
         state = {}
-        eps = torch.zeros_like(sample)
+        eps = sample.new_zeros((BF, self.out_channels, H, W))
         res = self._residuals(down_block_additional_residuals, mid_block_additional_residual)
         skips = {}
         for i, (pos, spec, block) in enumerate(zip(self.census_index, self.census, self.blocks)):
@@ -534,7 +539,7 @@ class SkeletonUNet(ModelMixin):
             ds = int(key[2:])
             if self.wrappers is not None:
                 h = _to_tokens(h)
-            out = self.drop[key](h).transpose(1, 2).reshape(BF, Cin, H // ds, W // ds)
+            out = self.drop[key](h).transpose(1, 2).reshape(BF, self.out_channels, H // ds, W // ds)
             if ds > 1:
                 out = F.interpolate(out, scale_factor=ds, mode="nearest")
             eps = eps + out
@@ -629,14 +634,17 @@ def pnp_conv_module(net: SkeletonUNet) -> nn.Module:
 
 def make_skeleton(name: str = "sd15", hot_path_only: bool = True, max_downsample: Optional[int] = None,
                   device="cuda", dtype=torch.float16, seed: int = 123, pnp_conv: bool = False,
-                  transformer_io: Optional[str] = None) -> SkeletonUNet:
+                  transformer_io: Optional[str] = None, depth: bool = False) -> SkeletonUNet:
+    """`depth=True`: the stand-in for SD2-depth's UNet (stabilityai/stable-diffusion-2-depth), which takes the latent
+    with each frame's depth map appended as a fifth channel and predicts the 4 latent channels."""
     census = CENSUSES[name]()
     cad = 1024 if name == "sd21" else 768
     gen_state = torch.get_rng_state()
     torch.manual_seed(seed)
     try:
-        net = SkeletonUNet(census, cross_attention_dim=cad, hot_path_only=hot_path_only,
-                           max_downsample=max_downsample, pnp_conv=pnp_conv, transformer_io=transformer_io)
+        net = SkeletonUNet(census, in_channels=5 if depth else 4, cross_attention_dim=cad, hot_path_only=hot_path_only,
+                           max_downsample=max_downsample, pnp_conv=pnp_conv, transformer_io=transformer_io,
+                           out_channels=4)
     finally:
         torch.set_rng_state(gen_state)
     return net.to(device=device, dtype=dtype).eval()
