@@ -440,6 +440,26 @@ int vtm_attention_residual(const void* x_dev, const void* w_qkv_dev, const void*
                            size_t ws_bytes, void* stream);
 
 /*
+ * vtm_attention_residual with PnP's source-frame injection, for the self-attention of an unmerged block during PnP
+ * generation (utils/pnp_utils.py:57-68, 86-91: `q[:B // num_inputs]`, `k[:B // num_inputs]` and
+ * `attn.repeat(num_inputs, 1, 1)` on a batch of [source | uncond | cond] frame items):
+ *   flags == 0:                   bit for bit vtm_attention_residual; qk_items is ignored.
+ *   flags == VTM_ATTN_SHARED_QK:  item b uses the attention map of item b mod qk_items, i.e. the queries and keys of item
+ *                                 b mod qk_items and its own values.  1 <= qk_items and B % qk_items == 0, else
+ *                                 VTM_E_SHAPE.  q and k are computed for the first qk_items items only (their part of
+ *                                 the workspace for the other items is left as it was).  The result equals, bit for
+ *                                 bit, vtm_attention_ex(VTM_ATTN_SHARED_QK) on the items {f, f + qk_items, ...} of each
+ *                                 f < qk_items, followed by torch's half add of the residual.
+ *   Other flag bits: VTM_E_UNSUPPORTED.  resid_dev == NULL: VTM_E_NULL.  Everything else as vtm_attention_residual,
+ *   workspace vtm_attention_lora_workspace_bytes(B, L, C, heads, R_qkv, R_o).  No allocation, no synchronisation:
+ *   capturable in a CUDA graph.
+ */
+int vtm_attention_residual_ex(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,
+                              const void* resid_dev, const vtm_lora_t* lora_qkv, const vtm_lora_t* lora_o, int32_t B,
+                              int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, int32_t qk_items,
+                              void* y_dev, void* ws_dev, size_t ws_bytes, void* stream);
+
+/*
  * KI — one DDIM step in place, with its coefficients and trajectory slot read on the device (replaces the update of
  * invert.py:182-211, `pred_next_x(..., inversion=True)`, and stores what invert.py:132-138 saves):
  *   s = *step_dev;  (a, r, c, d) = coef_dev[4 s .. 4 s + 3];  x <- c * ((x - a * eps) * r) + d * eps,  r = 1 / b;

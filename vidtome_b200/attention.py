@@ -73,13 +73,17 @@ def self_attention(attn: torch.nn.Module, x: torch.Tensor, shared_qk: bool = Fal
                          lora_o=lora_o)
 
 
-def self_attention_residual(attn: torch.nn.Module, x: torch.Tensor, resid: torch.Tensor) -> torch.Tensor:
+def self_attention_residual(attn: torch.nn.Module, x: torch.Tensor, resid: torch.Tensor,
+                            shared_items: Optional[int] = None) -> torch.Tensor:
     """attn(x) + resid for an unmerged block (vidtome/patch.py:157-169 with do_nothing merges) through
-    vtm_attention_residual: the same kernels as self_attention, the add in the out projection's epilogue."""
+    vtm_attention_residual: the same kernels as self_attention, the add in the out projection's epilogue.
+    shared_items: PnP injection on the block's frame items (utils/pnp_utils.py:57-68,86-91, vtm_attention_residual_ex):
+    item b uses the attention map of item b mod shared_items."""
     w_qkv, w_o, b_o, lora_qkv, lora_o = _packed(attn, x)
     heads = int(attn.heads)
     scale = float(getattr(attn, "scale", (x.shape[-1] // heads) ** -0.5))
-    return ops.attention_residual(x, w_qkv, w_o, b_o, heads, scale, resid, lora_qkv=lora_qkv, lora_o=lora_o)
+    return ops.attention_residual(x, w_qkv, w_o, b_o, heads, scale, resid, lora_qkv=lora_qkv, lora_o=lora_o,
+                                  shared_items=shared_items)
 
 
 def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:

@@ -8,7 +8,8 @@
 // warpgroup streaming K/V tiles of one head (contiguous runs of the head-major padded buffers written by the projection
 // epilogue) through an mbarrier ring, and CW = 3 (head_dim <= 80) or 2 wgmma consumer warpgroups running S = Q K^T, the
 // online softmax and O += P V with P kept in registers, each overlapping its softmax with its own P V.  A shared (PnP)
-// call serves G samples per CTA with one softmax (see flash_attn_kernel).
+// call serves G samples per CTA with one softmax (see flash_attn_kernel); its samples are `inputs` runs of `period` frames,
+// and sample f + j period reads the queries and keys of sample f.
 #include <stdlib.h>
 
 #include "gemm_sm90.cuh"
@@ -173,7 +174,11 @@ struct FaParams {
   int L, Lq, H, d, C, B;
   const int* len_dev; // DL: the sequence length on the device (self-attention, <= L == Lq, the buffers' row count)
   float scale_log2;   // softmax scale * log2(e)
-  int qk_shared;      // PnP injection (utils/pnp_utils.py:57-68,87-91): q and k of sample 0 for every sample, v per sample
+  // Whose q and k each sample reads.  The B samples are `inputs` runs of `period` frames: sample b = f + j period (frame
+  // f, input j) reads the q / k slab of sample f and its own v, and `groups` CTAs serve each frame, up to G inputs each.
+  // PnP injection (utils/pnp_utils.py:57-68,87-91) on merged tokens is period 1 (every sample reads sample 0), on the
+  // frames of an unmerged block period n (sample b reads sample b mod n); without sharing period = B, inputs = 1.
+  int period, inputs, groups;
 };
 
 constexpr size_t FA_SMEM_MAX = 227 * 1024;   // dynamic shared memory a CTA may opt in to on sm_90
@@ -273,11 +278,12 @@ __device__ __forceinline__ void fa_softmax(float (&s)[32], float (&m_r)[2], floa
 // DL (device length): the buffers hold p.L rows per head and sample, of which the first *p.len_dev are the sequence.  Query
 // tiles at or past it exit, and only keys below it take part, masked in the last tile exactly as keys past p.L are.
 //
-// G > 1 (shared calls only: every sample has the attention map of sample 0): the CTA serves samples G z .. G z + G - 1.
-// Each stage holds K of sample 0 and the V tiles of its G samples; S and the softmax are computed once and each sample's
-// O_g += P V_g is one wgmma per 16-key step, with the same shape as at G = 1, so every output element sees the same
-// roundings as in the CTA of its own sample.  Samples past B (the last group of a ragged split) read the V of sample
-// B - 1 and write nothing.
+// Shared calls (FaParams::period): CTA z serves frame f = z / groups and its inputs j0 .. j0 + G - 1, j0 = G (z mod
+// groups), i.e. the samples f + j period that all have the attention map of sample f.  At G > 1 each stage holds K of
+// sample f and the V tiles of the G samples; S and the softmax are computed once and each sample's O_g += P V_g is one
+// wgmma per 16-key step, with the same shape as at G = 1, so every output element sees the same roundings as in the CTA
+// of its own sample.  Inputs past the last (the last group of a ragged split) read the V of the frame's last input and
+// write nothing.  With period 1 this is the merged layout: samples G z .. G z + G - 1, clamped to B - 1.
 template <int KS, int G, bool DL>
 __global__ void __launch_bounds__(FaCfg<KS, G>::THREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
@@ -295,11 +301,14 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
   auto kv_empty = [&](int s) { return bars + 8u * (1 + STAGES + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
-  const int q0 = blockIdx.x * Cf::BQ, h = blockIdx.y, b0 = blockIdx.z * G;
+  const int q0 = blockIdx.x * Cf::BQ, h = blockIdx.y;
+  const int f = blockIdx.z / p.groups;                       // frame: the sample whose q / k the CTA reads
+  const int j0 = (blockIdx.z - f * p.groups) * G;            // first input of the CTA's group
+  const int b0 = f + j0 * p.period;                          // its sample
   const int seq = DL ? __ldg(p.len_dev) : p.L;               // keys that take part
   const int q_valid = DL ? seq : p.Lq;                       // query rows that are written
   if (DL && q0 >= q_valid) return;
-  const int sqk = (p.qk_shared ? 0 : b0) * p.H + h;          // slab of q / k
+  const int sqk = f * p.H + h;                               // slab of q / k
   const int nkv = (seq + FA_BKV - 1) / FA_BKV;
 
   if (threadIdx.x == 0) {
@@ -330,7 +339,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
         for (int a = 0; a < Cf::ATOMS; ++a) {
           tma_load_3d(st + a * Cf::KV_ATOM, &tm_k, kv_full(stage), 64 * a, j * FA_BKV, sqk);
           for (int g = 0; g < G; ++g) {
-            const int sv = (G == 1 ? b0 : min(b0 + g, p.B - 1)) * p.H + h;   // slab of v
+            const int sv = (G == 1 ? b0 : f + min(j0 + g, p.inputs - 1) * p.period) * p.H + h;   // slab of v
             tma_load_3d(st + (1 + g) * Cf::TILE_BYTES + a * Cf::KV_ATOM, &tm_v, kv_full(stage), 64 * a, j * FA_BKV, sv);
           }
         }
@@ -466,8 +475,8 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     if (row >= q_valid) continue;
 #pragma unroll
     for (int g = 0; g < G; ++g) {
-      if (G > 1 && b0 + g >= p.B) break;
-      __half* dst = p.o + (static_cast<size_t>(b0 + g) * p.Lq + row) * p.C + h * p.d;
+      if (G > 1 && j0 + g >= p.inputs) break;
+      __half* dst = p.o + (static_cast<size_t>(b0 + g * p.period) * p.Lq + row) * p.C + h * p.d;
 #pragma unroll
       for (int n = 0; n < DV / 8; ++n) {
         const int col = n * 8 + 2 * (lane & 3);
@@ -480,10 +489,13 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
 
 template <int KS, int G, bool DL>
 int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, int B, int Lq, int L, int C, int H,
-              int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev) {
+              int DP, float scale, int qk_period, cudaStream_t stream, const int* len_dev) {
   using Cf = FaCfg<KS, G>;
   if (H > 65535 || B > 65535 || Cf::ATOMS * 64 > DP) return VTM_E_SHAPE;
-  if (G > 1 && !qk_shared) return VTM_E_UNSUPPORTED;
+  if (G > 1 && !qk_period) return VTM_E_UNSUPPORTED;
+  const int period = qk_period ? qk_period : B;               // not shared: every sample is a frame of its own
+  if (period < 1 || B % period != 0) return VTM_E_SHAPE;
+  const int inputs = B / period, groups = (inputs + G - 1) / G;
   constexpr int BQ = Cf::BQ;
   const uint64_t BH = static_cast<uint64_t>(B) * H;
   CUtensorMap tq, tk, tv;
@@ -508,10 +520,10 @@ int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, i
   p.o = o;
   p.L = L; p.Lq = Lq; p.H = H; p.d = C / H; p.C = C; p.B = B;
   p.scale_log2 = scale * 1.4426950408889634f;
-  p.qk_shared = qk_shared;
+  p.period = period; p.inputs = inputs; p.groups = groups;
   p.len_dev = len_dev;
   const dim3 grid(static_cast<unsigned>((Lq + BQ - 1) / BQ), static_cast<unsigned>(H),
-                  static_cast<unsigned>((B + G - 1) / G));
+                  static_cast<unsigned>(period * groups));
   flash_attn_kernel<KS, G, DL><<<grid, Cf::THREADS, Cf::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   return launch_rc();
 }
@@ -519,32 +531,34 @@ int launch_fa(const __half* qh, const __half* kh, const __half* vh, __half* o, i
 // launch_fa<KS, g, DL> for a run-time group size 1 <= g <= G
 template <int KS, int G, bool DL>
 int launch_fa_group(int g, const __half* qh, const __half* kh, const __half* vh, __half* o, int B, int Lq, int L, int C,
-                    int H, int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev) {
+                    int H, int DP, float scale, int qk_period, cudaStream_t stream, const int* len_dev) {
   if constexpr (G > 1) {
-    if (g < G) return launch_fa_group<KS, G - 1, DL>(g, qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream, len_dev);
+    if (g < G) return launch_fa_group<KS, G - 1, DL>(g, qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_period, stream, len_dev);
   }
-  return launch_fa<KS, G, DL>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_shared, stream, len_dev);
+  return launch_fa<KS, G, DL>(qh, kh, vh, o, B, Lq, L, C, H, DP, scale, qk_period, stream, len_dev);
 }
 
-// Samples per CTA: 1, or for a shared call the fewest groups of at most fa_group_max(KS) samples, equally sized (so
-// that the last group reads as few clamped V tiles as possible).
-inline int fa_group(int KS, int B, int qk_shared) {
-  if (!qk_shared) return 1;
+// Samples per CTA: 1, or for a shared call the fewest groups of at most fa_group_max(KS) of a frame's `inputs` samples,
+// equally sized (so that the last group reads as few clamped V tiles as possible).
+inline int fa_group(int KS, int inputs, int qk_period) {
+  if (!qk_period) return 1;
   const int gmax = fa_group_max(KS);
-  const int groups = (B + gmax - 1) / gmax;
-  return (B + groups - 1) / groups;
+  const int groups = (inputs + gmax - 1) / gmax;
+  return (inputs + groups - 1) / groups;
 }
 
+// qk_period: 0 (not shared), or n >= 1 with B % n == 0: sample b reads the q / k slab of sample b mod n (FaParams).
 int launch_fa_any(const __half* qh, const __half* kh, const __half* vh, __half* o, int B, int Lq, int L, int C, int H,
-                  int DP, float scale, int qk_shared, cudaStream_t stream, const int* len_dev = nullptr) {
+                  int DP, float scale, int qk_period, cudaStream_t stream, const int* len_dev = nullptr) {
+  if (qk_period < 0 || (qk_period && B % qk_period != 0)) return VTM_E_SHAPE;
   const int ks = (C / H + 15) / 16;
-  const int g = fa_group(ks, B, qk_shared);
+  const int g = fa_group(ks, qk_period ? B / qk_period : 1, qk_period);
 #define VTM_FA_CASE(KS)                                                                                               \
   case KS:                                                                                                            \
     return len_dev ? launch_fa_group<KS, fa_group_max(KS), true>(g, qh, kh, vh, o, B, Lq, L, C, H, DP, scale,         \
-                                                                 qk_shared, stream, len_dev)                         \
+                                                                 qk_period, stream, len_dev)                         \
                    : launch_fa_group<KS, fa_group_max(KS), false>(g, qh, kh, vh, o, B, Lq, L, C, H, DP, scale,        \
-                                                                  qk_shared, stream, nullptr);
+                                                                  qk_period, stream, nullptr);
   if (C / H > FA_MAX_HEAD_DIM) return VTM_E_UNSUPPORTED;
   switch (ks) {
     VTM_FA_CASE(1)
@@ -585,16 +599,20 @@ extern "C" size_t vtm_attention_lora_workspace_bytes(int32_t B, int32_t L, int32
 
 namespace vtm {
 namespace {
-// len_dev: NULL, or the sequence length on the device with L the rows of the buffers (vtm_attention_dev)
+// len_dev: NULL, or the sequence length on the device with L the rows of the buffers (vtm_attention_dev).
+// qk_items (VTM_ATTN_SHARED_QK only): sample b reads the queries and keys of sample b mod qk_items (1 <= qk_items,
+// B % qk_items == 0).
 int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev, int32_t B,
                    int32_t L, int32_t C, int32_t heads, float scale, int32_t flags, const int32_t* len_dev, void* y_dev,
                    void* ws_dev, size_t ws_bytes, void* stream_, const vtm_lora_t* lora_qkv = nullptr,
-                   const vtm_lora_t* lora_o = nullptr, const void* resid_dev = nullptr) {
+                   const vtm_lora_t* lora_o = nullptr, const void* resid_dev = nullptr, int32_t qk_items = 1) {
   if (!x_dev || !w_qkv_dev || !w_o_dev || !y_dev || !ws_dev) return VTM_E_NULL;
   if (B <= 0 || L <= 0 || C <= 0 || heads <= 0 || C % heads != 0) return VTM_E_SHAPE;
   const int d = C / heads;
   if (d % 8 != 0 || C % 8 != 0) return VTM_E_SHAPE;
   if (d > FA_MAX_HEAD_DIM || (flags & ~1) != 0) return VTM_E_UNSUPPORTED;
+  const int period = (flags & 1) ? qk_items : 0;             // launch_fa_any's qk_period
+  if ((flags & 1) && (qk_items < 1 || B % qk_items != 0)) return VTM_E_SHAPE;
   int Rq = 0, Ro = 0;
   int rc = lora_rank(lora_qkv, &Rq);
   if (rc) return rc;
@@ -616,9 +634,10 @@ int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev
     if (rc) return rc;
   }
   if (flags & 1) {
-    // shared: q and k of sample 0 (the only ones the flash kernel reads), v of every sample
-    rc = launch_head_proj(x_dev, w_qkv_dev, qkv, 1, L, C, C, heads, DP, 0, 2, stream, static_cast<long long>(slab), t,
-                          uq, Rq);
+    // shared: q and k of samples 0 .. qk_items - 1 (the only ones the flash kernel reads: their first qk_items L rows of
+    // x and of T), v of every sample
+    rc = launch_head_proj(x_dev, w_qkv_dev, qkv, qk_items, L, C, C, heads, DP, 0, 2, stream,
+                          static_cast<long long>(slab), t, uq, Rq);
     if (rc) return rc;
     rc = launch_head_proj(x_dev, static_cast<const __half*>(w_qkv_dev) + static_cast<size_t>(2) * C * C, vh, B, L, C, C,
                           heads, DP, 2, 1, stream, 0, t, Rq ? uq + static_cast<size_t>(2) * C * Rq : nullptr, Rq);
@@ -626,7 +645,7 @@ int attention_impl(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev
     rc = launch_head_proj(x_dev, w_qkv_dev, qkv, B, L, C, C, heads, DP, 0, 3, stream, 0, t, uq, Rq);
   }
   if (rc) return rc;
-  rc = launch_fa_any(qkv, kh, vh, o, B, L, L, C, heads, DP, scale, flags & 1, stream, len_dev);
+  rc = launch_fa_any(qkv, kh, vh, o, B, L, L, C, heads, DP, scale, period, stream, len_dev);
   if (rc) return rc;
   if (Ro)
     return vtm_linear_lora_f16(o, w_o_dev, b_o_dev, resid_dev, resid_dev ? C : 0, lora_o, M, C, C, y_dev, C, t,
@@ -669,6 +688,19 @@ extern "C" int vtm_attention_residual(const void* x_dev, const void* w_qkv_dev, 
   if (!resid_dev) return VTM_E_NULL;
   return vtm::attention_impl(x_dev, w_qkv_dev, w_o_dev, b_o_dev, B, L, C, heads, scale, 0, nullptr, y_dev, ws_dev,
                              ws_bytes, stream_, lora_qkv, lora_o, resid_dev);
+}
+
+// The same with PnP's injection over the frames of an unmerged block (utils/pnp_utils.py:57-68,86-91): under
+// VTM_ATTN_SHARED_QK the batch is [source | uncond | cond] runs of qk_items frames, and item b uses the attention map
+// of item b mod qk_items.
+extern "C" int vtm_attention_residual_ex(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev,
+                                         const void* b_o_dev, const void* resid_dev, const vtm_lora_t* lora_qkv,
+                                         const vtm_lora_t* lora_o, int32_t B, int32_t L, int32_t C, int32_t heads,
+                                         float scale, int32_t flags, int32_t qk_items, void* y_dev, void* ws_dev,
+                                         size_t ws_bytes, void* stream_) {
+  if (!resid_dev) return VTM_E_NULL;
+  return vtm::attention_impl(x_dev, w_qkv_dev, w_o_dev, b_o_dev, B, L, C, heads, scale, flags, nullptr, y_dev, ws_dev,
+                             ws_bytes, stream_, lora_qkv, lora_o, resid_dev, qk_items);
 }
 
 extern "C" int vtm_attention(const void* x_dev, const void* w_qkv_dev, const void* w_o_dev, const void* b_o_dev,

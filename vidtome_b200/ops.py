@@ -501,9 +501,12 @@ def ddim_table(coefficients) -> torch.Tensor:
 
 
 def attention_residual(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, b_o: Optional[torch.Tensor],
-                       heads: int, scale: float, resid: torch.Tensor, lora_qkv=None, lora_o=None) -> torch.Tensor:
+                       heads: int, scale: float, resid: torch.Tensor, lora_qkv=None, lora_o=None,
+                       shared_items: Optional[int] = None) -> torch.Tensor:
     """KD with the residual in the out projection: attention(x, ...) + resid, bit for bit as torch's half add, for an
-    unmerged block (`attn1(norm1(h)) + h`).  x, resid [B, L, C] fp16; lora_qkv / lora_o as in `attention`."""
+    unmerged block (`attn1(norm1(h)) + h`).  x, resid [B, L, C] fp16; lora_qkv / lora_o as in `attention`.
+    shared_items: PnP injection over frame items (vtm_attention_residual_ex): item b uses the attention map of item
+    b mod shared_items (B % shared_items == 0); None: every item its own."""
     _require(x, torch.float16, "x")
     _require(w_qkv, torch.float16, "w_qkv")
     _require(w_o, torch.float16, "w_o")
@@ -519,9 +522,16 @@ def attention_residual(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, 
     y = torch.empty_like(x)
     flops = 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc + 8.0 * B * L * Cc * (rq + ro)
     with _Timed("KD", flops, 6.0 * B * L * Cc + 8.0 * Cc * Cc):
-        check(lib.vtm_attention_residual(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), resid.data_ptr(),
-                                         _lora_ref(dq), _lora_ref(do), B, L, Cc, heads, float(scale), y.data_ptr(),
-                                         ws.data_ptr(), ws_bytes, _stream()), "vtm_attention_residual")
+        if shared_items is None:
+            check(lib.vtm_attention_residual(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o),
+                                             resid.data_ptr(), _lora_ref(dq), _lora_ref(do), B, L, Cc, heads,
+                                             float(scale), y.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
+                  "vtm_attention_residual")
+        else:
+            check(lib.vtm_attention_residual_ex(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o),
+                                                resid.data_ptr(), _lora_ref(dq), _lora_ref(do), B, L, Cc, heads,
+                                                float(scale), 1, int(shared_items), y.data_ptr(), ws.data_ptr(),
+                                                ws_bytes, _stream()), "vtm_attention_residual_ex")
     STATS.launches += 3 + (rq > 0) + (ro > 0)
     return y
 

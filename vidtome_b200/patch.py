@@ -84,6 +84,15 @@ GLOBAL_EXCHANGE = "recurrence"
 # both sets to be equally long (equal chunks); eagerly, a block whose sets differ keeps the host coin.
 DEVICE_COIN = False
 
+# Run the self-attention of every block that does not merge at this call (block_merges) through the CUDA library during
+# generation too: norm1 -> KD with the residual in its out projection, as inside _unmerged_blocks(), for a stock attn1
+# (_plain_attention_module) up to attention.MAX_HEAD_DIM.  PnP-marked modules included: while their injection is active
+# item b of the [source | uncond | cond] frame batch uses the attention map of item b mod (B / num_inputs)
+# (vtm_attention_residual_ex).  Off by default: the library's flash kernel takes its softmax in fp32 where the module's
+# own forward rounds it in fp16 (torch's `softmax` / SDPA), so these blocks' results change within fp16 tolerance.
+# Read on every call, so it may be changed at any time.
+FUSE_UNMERGED_ATTENTION = False
+
 # Depth of _unmerged_blocks() contexts: while > 0 every ToMeBlock runs as the reference's UNPATCHED block.
 _UNMERGED = 0
 
@@ -245,17 +254,24 @@ def _global_stage_device_coin(module, table, mu, pi, g, ln, args, levels):
     return merged_tokens, pi, coin
 
 
-def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[str, Any],
-                     ln=None) -> Optional[MergePlan]:
-    """The body of compute_merge (vidtome/patch.py:14-91).  Returns None when the block is not merged
-    (downsample > max_downsample, patch.py:27,86-88).  With `ln = (weight, bias, eps)`, `x` is the RAW
-    hidden state and norm1 is applied inside the kernels that read it (K0, KC)."""
+def block_merges(x: torch.Tensor, tome_info: Dict[str, Any]) -> bool:
+    """Whether a block whose input `x` has x.shape[1] tokens per item merges at this call: its downsampling of the
+    latent recorded in tome_info["size"] is at most max_downsample (patch.py:15-17,27,86-88).  Decided before anything
+    is drawn from the block's generator."""
     original_h, original_w = tome_info["size"]
     original_tokens = original_h * original_w
     downsample = int(math.ceil(math.sqrt(original_tokens // x.shape[1])))    # patch.py:15-17
-    args = tome_info["args"]
-    if downsample > args["max_downsample"]:
+    return downsample <= tome_info["args"]["max_downsample"]
+
+
+def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[str, Any],
+                     ln=None) -> Optional[MergePlan]:
+    """The body of compute_merge (vidtome/patch.py:14-91).  Returns None when the block is not merged
+    (block_merges).  With `ln = (weight, bias, eps)`, `x` is the RAW hidden state and norm1 is applied inside the
+    kernels that read it (K0, KC)."""
+    if not block_merges(x, tome_info):
         return None
+    args = tome_info["args"]
     merge._check_metric(x)
     generator = module.generator
     fsize = x.shape[0] // args["batch_size"]                                 # patch.py:23
@@ -466,16 +482,32 @@ def make_diffusers_tome_block(block_class: Type[torch.nn.Module]) -> Type[torch.
             only_cross = getattr(self, "only_cross_attention", False)
             from . import attention as _attention
             ln1 = None
-            if (unmerged and hidden_states.is_cuda and hidden_states.dtype == torch.float16 and _attention.ENABLED
+            shared_items = None
+            if (hidden_states.is_cuda and hidden_states.dtype == torch.float16 and _attention.ENABLED
                     and not self.use_ada_layer_norm and not self.use_ada_layer_norm_zero and not only_cross
-                    and attention_mask is None and not cross_attention_kwargs and _plain_attention_module(self.attn1)):
+                    and attention_mask is None and not cross_attention_kwargs
+                    and (unmerged or (FUSE_UNMERGED_ATTENTION and not block_merges(hidden_states, self._tome_info)))
+                    and _plain_attention_module(self.attn1)):
                 ln1 = _fusable_layer_norm(self.norm1, hidden_states)
+                num_inputs = getattr(self.attn1, "_vtm_pnp", 0)
+                if ln1 is not None and num_inputs:
+                    from . import pnp as _pnp
+                    if _pnp.injection_active(self.attn1):             # never inside _unmerged_blocks()
+                        if hidden_states.shape[0] % num_inputs:
+                            ln1 = None                                # the module's forward, which fails as the reference's
+                        else:
+                            shared_items = hidden_states.shape[0] // num_inputs
             if ln1 is not None:
-                # unmerged (_unmerged_blocks): attn1(norm1(h)) + h, the add in the out projection of KD
+                # a block that does not merge (_unmerged_blocks, or FUSE_UNMERGED_ATTENTION): attn1(norm1(h)) + h, the
+                # add in the out projection of KD; with PnP injecting, item b takes the map of item b mod shared_items
                 shape = hidden_states.shape
                 hidden_states = hidden_states.contiguous()
                 n1 = ops.layer_norm(hidden_states.view(-1, shape[-1]), ln1).view(shape)
-                hidden_states = _attention.self_attention_residual(self.attn1, n1, hidden_states)
+                if shared_items is None:
+                    hidden_states = _attention.self_attention_residual(self.attn1, n1, hidden_states)
+                else:
+                    hidden_states = _attention.self_attention_residual(self.attn1, n1, hidden_states,
+                                                                       shared_items=shared_items)
             else:
                 if self.use_ada_layer_norm:                                       # patch.py:139-146
                     norm_hidden_states = self.norm1(hidden_states, timestep)
