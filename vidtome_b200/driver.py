@@ -66,6 +66,32 @@ def _check_depth(depth: torch.Tensor, x: torch.Tensor, model: torch.nn.Module):
                          f"channel")
 
 
+class _ControlNetServing:
+    """The lazy serving of an unpatched ControlNet shared by both drivers: at the first step that runs with
+    patch.FUSE_CONTROLNET_BLOCKS on, a ControlNet that apply_patch did not patch (the reference's default,
+    include_control=False) and that is not served yet is served (patch.serve_unmerged); close() unserves it again.  A
+    patched ControlNet, or one the caller served, is left as it is and close() leaves it alone."""
+
+    def __init__(self, controlnet: Optional[torch.nn.Module]):
+        self.controlnet = controlnet
+        self.decided = controlnet is None
+        self.served = False
+
+    def before_step(self):
+        if self.decided or not patch.FUSE_CONTROLNET_BLOCKS:
+            return
+        self.decided = True
+        if not patch.is_patched(self.controlnet) and not patch.is_served(self.controlnet):
+            patch.serve_unmerged(self.controlnet)
+            self.served = True
+
+    def close(self):
+        if self.served:
+            patch.unserve_unmerged(self.controlnet)
+        self.served = False
+        self.decided = self.controlnet is None
+
+
 class ChunkedDenoiser:
     """Chunked classifier-free-guidance DDIM sampling on a (patched) UNet, generate.py:205-311."""
 
@@ -129,6 +155,10 @@ class ChunkedDenoiser:
         from their own generators and keep their own global tokens, which every graph mode registers and resets like
         the UNet's.  The control images are a static input of every graph.  One control mode at a time: ControlNet
         and PnP (`source_latents`) are refused together, as the reference takes one (generate.py:61-68).
+        An unpatched ControlNet (the reference's default) runs its modules' own forwards; with
+        patch.FUSE_CONTROLNET_BLOCKS on, the first step serves it (patch.serve_unmerged), so that its blocks and
+        Transformer2DModel wrappers run in the library, never merged.  Its shapes are static, so graph keys do not
+        change; a graph replays the path it was captured with.  close() gives the ControlNet its own classes back.
 
         `depth` ([flen, 1, h, w], the reference's prepare_depth output: one depth map per frame at latent resolution,
         normalised to [-1, 1]) runs SD2-depth (stabilityai/stable-diffusion-2-depth, `sd_version: "depth"`), whose UNet
@@ -149,6 +179,7 @@ class ChunkedDenoiser:
         self.controlnet = controlnet
         self.control_images = control_images
         self.control_scale = control_scale
+        self._serving = _ControlNetServing(controlnet)
         self.unet = unet
         # shard=True: this process is one rank of a torch.distributed job and takes chunks i % world == rank of every
         # step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
@@ -548,6 +579,7 @@ class ChunkedDenoiser:
             if len(self.control_images) != len(x):
                 raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
             frames["ctrl"] = self.control_images.to(x)                      # prepare_data's .to(self.init_noise)
+            self._serving.before_step()
         if self.depth is not None:
             frames["depth"] = self.depth.to(x)                              # prepare_data's .to(self.init_noise)
         if self.chunk_graphs and self.merge_global and x.is_cuda and not self._stores:
@@ -580,6 +612,14 @@ class ChunkedDenoiser:
             x = self.step(x, i)
         return x
 
+    def close(self):
+        """Release the captured graphs and give a ControlNet this driver served its own classes back.  The driver may
+        step again afterwards: it then serves the ControlNet and captures anew."""
+        self._graph = None
+        self._chunk_graphs = {}
+        self._eager_steps = 0
+        self._serving.close()
+
 
 class ChunkedInverter:
     """DDIM inversion of source latents in frame batches, invert.py:117-211 (`Inverter.ddim_inversion`, `pred_noise`,
@@ -608,7 +648,11 @@ class ChunkedInverter:
     `depth` ([F, 1, h, w], the reference's prepare_depth output) inverts with SD2-depth's 5-channel UNet: every UNet call
     gets the batch's latents with its depth maps appended as a fifth channel, cast to the latents' dtype
     (invert.py:161-166), eagerly and in the captured step.  The update and the trajectory keep the 4 latent channels.
-    Depth with `controlnet` is refused, as in ChunkedDenoiser."""
+    Depth with `controlnet` is refused, as in ChunkedDenoiser.
+
+    An unpatched `controlnet` runs its modules' own forwards; with patch.FUSE_CONTROLNET_BLOCKS on, the first invert()
+    serves it (patch.serve_unmerged), so that its blocks and Transformer2DModel wrappers run in the library, unmerged,
+    as a patched model's do here.  close() gives it its own classes back."""
 
     def __init__(self, unet: torch.nn.Module, n_timesteps: int = 50, batch_size: int = 8,
                  save_steps: Optional[int] = None, save_intermediate: bool = True, cond: Optional[torch.Tensor] = None,
@@ -639,6 +683,7 @@ class ChunkedInverter:
         self.controlnet = controlnet
         self.control_images = control_images
         self.control_scale = control_scale
+        self._serving = _ControlNetServing(controlnet)
         self.cuda_graph = bool(cuda_graph)
         self.graph_warmup = int(graph_warmup)
         self.alphas_cumprod = ddim_alphas_cumprod()
@@ -726,6 +771,7 @@ class ChunkedInverter:
             if len(self.control_images) != len(x):
                 raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
             frames["ctrl"] = self.control_images.to(x)
+            self._serving.before_step()
         if self.depth is not None:
             _check_depth(self.depth, x, self.unet)
             frames["depth"] = self.depth.to(x)
@@ -772,6 +818,10 @@ class ChunkedInverter:
             graph.replay()
         torch.cuda.synchronize(x.device)
         del graph
+
+    def close(self):
+        """Give a ControlNet this inverter served its own classes back (invert() serves it again if called)."""
+        self._serving.close()
 
     def source_latents(self, frame_ids=None) -> Callable[[int], torch.Tensor]:
         """The callable ChunkedDenoiser(source_latents=...) takes: t -> the inverted latents at timestep t [flen, 4,

@@ -93,6 +93,15 @@ DEVICE_COIN = False
 # Read on every call, so it may be changed at any time.
 FUSE_UNMERGED_ATTENTION = False
 
+# Run the transformer blocks and Transformer2DModel wrappers of a model that apply_patch did not patch, and that
+# serve_unmerged served (the step driver and the inverter serve an unpatched ControlNet while this is on), through the
+# library, always unmerged: every block takes the path of a patched block inside _unmerged_blocks() (fused norm1 -> KD
+# with the residual in its out projection, norm2 -> cross-attention, norm3 -> GEGLU -> residual projection) and every
+# wrapper the library's entry and exit.  Off by default for the reason FUSE_UNMERGED_ATTENTION is: the flash kernel
+# takes its softmax in fp32, so results change within fp16 tolerance against the modules' own forwards.  Read on every
+# call; while it is off a served module runs its own forward.
+FUSE_CONTROLNET_BLOCKS = False
+
 # Depth of _unmerged_blocks() contexts: while > 0 every ToMeBlock runs as the reference's UNPATCHED block.
 _UNMERGED = 0
 
@@ -472,12 +481,14 @@ def make_diffusers_tome_block(block_class: Type[torch.nn.Module]) -> Type[torch.
     class ToMeBlock(block_class):
         # the original class, restored by remove_patch
         _parent = block_class
+        # True in the served class of serve_unmerged: the block never merges, as inside _unmerged_blocks()
+        _vtm_unmerged = False
 
         def forward(self, hidden_states, attention_mask=None, encoder_hidden_states=None,
                     encoder_attention_mask=None, timestep=None, cross_attention_kwargs=None,
                     class_labels=None) -> torch.Tensor:
             plan = None
-            unmerged = _UNMERGED > 0
+            unmerged = _UNMERGED > 0 or self._vtm_unmerged
             cross_attention_kwargs = cross_attention_kwargs if cross_attention_kwargs is not None else {}
             only_cross = getattr(self, "only_cross_attention", False)
             from . import attention as _attention
@@ -622,6 +633,121 @@ def make_library_transformer2d(wrapper_class: Type[torch.nn.Module]) -> Type[tor
             return super().forward(hidden_states, *args, **kwargs)
 
     return ToMeTransformer2D
+
+
+# the keyword arguments of BasicTransformerBlock.forward that ToMeBlock.forward restates
+SERVED_BLOCK_KWARGS = frozenset(("attention_mask", "encoder_hidden_states", "encoder_attention_mask", "timestep",
+                                 "cross_attention_kwargs", "class_labels"))
+# class names of the modules serve_unmerged swaps in
+_SERVED_CLASSES = ("UnmergedBlock", "UnmergedTransformer2D")
+
+
+def served_block_ineligibility(block: torch.nn.Module, hidden_states, args: tuple, kwargs: dict) -> Optional[str]:
+    """Why a call of a served block (serve_unmerged) runs the block class's own forward instead of the unmerged library
+    path, or None if it takes that path.  It takes it with FUSE_CONTROLNET_BLOCKS on, keyword arguments only and those
+    ToMeBlock.forward restates, no attention masks and no cross_attention_kwargs, the plain-LayerNorm block of the
+    diffusers releases the reference targets (use_ada_layer_norm / use_ada_layer_norm_zero present and false, not
+    only_cross_attention), no autograd, and a CUDA fp16 input.  Past this gate each stage keeps the rule it has inside
+    _unmerged_blocks(): attn1 through KD when _plain_attention_module and norm1 is _fusable_layer_norm, attn2 when
+    attention.cross_attention_eligible, the feed-forward when feedforward.geglu_parts; otherwise that stage's modules."""
+    if not FUSE_CONTROLNET_BLOCKS:
+        return "switch"
+    if args or not SERVED_BLOCK_KWARGS.issuperset(kwargs):
+        return "arguments"
+    if (kwargs.get("attention_mask") is not None or kwargs.get("encoder_attention_mask") is not None
+            or kwargs.get("cross_attention_kwargs")):
+        return "arguments"
+    if not (hasattr(block, "use_ada_layer_norm") and hasattr(block, "use_ada_layer_norm_zero")):
+        return "norm"
+    if block.use_ada_layer_norm or block.use_ada_layer_norm_zero or getattr(block, "only_cross_attention", False):
+        return "norm"
+    if block.training and torch.is_grad_enabled():
+        return "training"
+    if not isinstance(hidden_states, torch.Tensor) or not hidden_states.is_cuda or hidden_states.dtype != torch.float16:
+        return "device"
+    return None
+
+
+def make_unmerged_block(block_class: Type[torch.nn.Module]) -> Type[torch.nn.Module]:
+    """Served class for a BasicTransformerBlock of a model apply_patch did not patch (serve_unmerged): ToMeBlock's
+    forward in its unmerged state, which builds no merge plan and reads no `_tome_info`, `generator` or
+    `global_tokens`, while served_block_ineligibility passes; else the block class's own forward."""
+    tome = make_diffusers_tome_block(block_class)
+
+    class UnmergedBlock(tome):
+        # the original class, restored by unserve_unmerged
+        _parent = block_class
+        _vtm_unmerged = True
+
+        def forward(self, hidden_states, *args, **kwargs):
+            if served_block_ineligibility(self, hidden_states, args, kwargs) is None:
+                return tome.forward(self, hidden_states, **kwargs)
+            return block_class.forward(self, hidden_states, *args, **kwargs)
+
+    return UnmergedBlock
+
+
+def make_unmerged_transformer2d(wrapper_class: Type[torch.nn.Module]) -> Type[torch.nn.Module]:
+    """Served class for a Transformer2DModel of a model apply_patch did not patch (serve_unmerged): the patched class's
+    forward (the library's entry and exit under FUSE_TRANSFORMER_IO and transformer2d.ineligibility) while
+    FUSE_CONTROLNET_BLOCKS is on, else the wrapper class's own forward."""
+    library = make_library_transformer2d(wrapper_class)
+
+    class UnmergedTransformer2D(library):
+        # the original class, restored by unserve_unmerged
+        _parent = wrapper_class
+
+        def forward(self, hidden_states, *args, **kwargs):
+            if FUSE_CONTROLNET_BLOCKS:
+                return library.forward(self, hidden_states, *args, **kwargs)
+            return wrapper_class.forward(self, hidden_states, *args, **kwargs)
+
+    return UnmergedTransformer2D
+
+
+def is_patched(model: torch.nn.Module) -> bool:
+    """True if apply_patch patched `model` (or a module inside it) and remove_patch has not undone it: some module has
+    a patched class or the hooks of a `_tome_info`."""
+    return any(type(m).__name__ in ("ToMeBlock", "ToMeTransformer2D") or getattr(m, "_tome_info", {}).get("hooks")
+               for m in model.modules())
+
+
+def is_served(model: torch.nn.Module) -> bool:
+    """True if serve_unmerged served some module of `model`."""
+    return any(type(m).__name__ in _SERVED_CLASSES for m in model.modules())
+
+
+def serve_unmerged(model: torch.nn.Module) -> torch.nn.Module:
+    """Serve a model that apply_patch did not patch (the reference's unpatched ControlNet, generate.py:96-98) from the
+    library, always unmerged, while FUSE_CONTROLNET_BLOCKS is on: every BasicTransformerBlock gets the class of
+    make_unmerged_block and every Transformer2DModel that of make_unmerged_transformer2d.  Nothing else changes: no
+    `_tome_info`, no hooks (so no generator is forked and nothing is drawn), no `global_tokens`, no PnP, and the
+    parameters and buffers are the model's own.  A model patched by apply_patch is refused; serving a served model
+    again changes nothing.  unserve_unmerged undoes it.  Returns `model`."""
+    if is_patched(model):
+        raise ValueError("serve_unmerged: the model is patched by apply_patch, whose blocks already run in the library; "
+                         "serve only an unpatched model")
+    from . import _lib
+    _lib.load()   # fail here, loudly, if the CUDA library is missing
+    for module in model.modules():
+        if type(module).__name__ in _SERVED_CLASSES:
+            continue
+        if isinstance_str(module, "BasicTransformerBlock"):
+            module.__class__ = make_unmerged_block(module.__class__)
+        elif isinstance_str(module, "Transformer2DModel"):
+            module.__class__ = make_unmerged_transformer2d(module.__class__)
+    return model
+
+
+def unserve_unmerged(model: torch.nn.Module) -> torch.nn.Module:
+    """Undo serve_unmerged: every served module gets its original class back.  A model patched by apply_patch is
+    refused (remove_patch undoes apply_patch).  Returns `model`."""
+    if is_patched(model):
+        raise ValueError("unserve_unmerged: the model is patched by apply_patch; undo that with remove_patch")
+    for module in model.modules():
+        if type(module).__name__ in _SERVED_CLASSES:
+            module.__class__ = module._parent
+    return model
 
 
 def hook_tome_model(model: torch.nn.Module):
