@@ -501,7 +501,7 @@ def _attention_cases():
     lib = _lib.load
     out = {}
 
-    def self_case(entry, B, L, d, H, flags=0, name="random", length=None, lora=None, resid=False, f64=True):
+    def self_case(entry, B, L, d, H, flags=0, name="random", length=None, lora=None, resid=False, f64=True, items=1):
         x, w, wo, scale, g = _self_inputs(name, B, L, d, H, seed=B * L + d + flags)
         C = d * H
         if length is not None and length < L:
@@ -510,12 +510,12 @@ def _attention_cases():
         ws_bytes = lib().vtm_attention_lora_workspace_bytes(B, L, C, H, Rq, Ro)
         DP = _dp(d)
         ws_kept = None
-        if flags & 1 and B > 1:                         # q and k of samples 1..B-1 are left as they were
+        if flags & 1 and B > items:                     # q and k of samples items..B-1 are left as they were
             slab = B * H * L * DP
             ws_kept = torch.zeros(ws_bytes, dtype=torch.bool)
             per = H * L * DP * 2
             for j in range(2):
-                ws_kept[(j * slab * 2) + per:(j * slab * 2) + slab * 2] = True
+                ws_kept[(j * slab * 2) + per * items:(j * slab * 2) + slab * 2] = True
         unspec = None
         if length is not None:
             unspec = (torch.arange(L) >= length).repeat_interleave(C).repeat(B)
@@ -528,7 +528,7 @@ def _attention_cases():
         if lora:
             for k, (R, N) in (("q", (Rq, 3 * C)), ("o", (Ro, C))):
                 bufs["d" + k], bufs["u" + k] = Buf("in", _randn((R, C), g, 0.05)), Buf("in", _randn((N, R), g, 0.05))
-        what = f"{entry} {name} B={B} L={L} d={d} H={H} flags={flags} len={length} lora={lora}"
+        what = f"{entry} {name} B={B} L={L} d={d} H={H} flags={flags} items={items} len={length} lora={lora}"
         check = _attn_f64(x, w, H, scale, flags, what, rows=length) if f64 and not lora else None
 
         def los(b):
@@ -550,6 +550,12 @@ def _attention_cases():
                 return [b["x"], b["w"], b["wo"], None, _ref(lq), _ref(lo), B, L, C, H, scale, flags,
                         b["len"] if length is not None else None, b["y"], b["ws"], ws_bytes, _stream()]
             wsa, errs = 15, [(VTM_E_NULL, {14: None}), (VTM_E_SHAPE, {8: C + 4})]
+        elif entry == "vtm_attention_residual_ex":
+            def args(b):
+                lq, lo = los(b)
+                return [b["x"], b["w"], b["wo"], None, b["r"], _ref(lq), _ref(lo), B, L, C, H, scale, flags, items,
+                        b["y"], b["ws"], ws_bytes, _stream()]
+            wsa, errs = 16, [(VTM_E_NULL, {4: None}), (VTM_E_SHAPE, {12: 1, 13: B + 1})]
         else:
             def args(b):
                 lq, lo = los(b)
@@ -579,6 +585,12 @@ def _attention_cases():
                            (2, 65, 80, 2, (200, 8))]:
         reg("vtm_attention_residual", f"B={B} L={L} d={d} H={H} lora={lo}", B=B, L=L, d=d, H=H, resid=True, lora=lo,
             f64=lo is None)
+    # flags 0, then the map shared from one item and from 3 of 6 (which _attn_f64 does not model), and LoRA
+    for B, L, d, H, flags, items, lo in [(2, 193, 160, 2, 0, 1, None), (2, 65, 40, 2, 0, 1, None),
+                                         (3, 65, 40, 2, 1, 1, None), (6, 65, 80, 2, 1, 3, None),
+                                         (6, 193, 40, 2, 1, 3, (8, 16))]:
+        reg("vtm_attention_residual_ex", f"B={B} L={L} d={d} H={H} flags={flags} items={items} lora={lo}", B=B, L=L,
+            d=d, H=H, flags=flags, items=items, resid=True, lora=lo, f64=lo is None and items == 1)
 
     def cross_case(entry, B, Lq, Lk, d, H, lora=None, probe=False):
         import test_gpu_attention_core as core

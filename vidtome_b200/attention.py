@@ -32,6 +32,53 @@ def max_head_dim() -> int:
     return v
 
 
+# attention processors whose result is plain softmax(q k^T * scale) v (what KD computes)
+_PLAIN_PROCESSORS = ("AttnProcessor", "AttnProcessor2_0", "XFormersAttnProcessor")
+
+
+def stock_attention_parts(attn: torch.nn.Module):
+    """The lora.linear_parts of to_q, to_k, to_v and to_out[0] if `attn` is structurally a stock diffusers-style Attention
+    the library can run, else None: projections that are bare `torch.nn.Linear` or LoRA-adapted layers lora.linear_parts
+    reads (any other subclass or wrapper carries terms the library would miss), to_q / to_k / to_v without bias, to_out =
+    [Linear, Dropout(inactive)...], no forward hooks on the module or its projections (torch lists a hook registered
+    with_kwargs in `_forward_hooks` too), a default attention processor (or none), and none of the Attention options
+    that alter the math (group / spatial norm, norm_cross, residual connection, output rescale, added KV projections).
+    Instance-level forward overrides, shapes, dtypes and the head width are the callers' rules."""
+    if not all(hasattr(attn, n) for n in ("to_q", "to_k", "to_v", "to_out", "heads")):
+        return None
+    to_out = attn.to_out
+    if not isinstance(to_out, (torch.nn.ModuleList, torch.nn.Sequential)) or len(to_out) < 1:
+        return None
+    linears = (attn.to_q, attn.to_k, attn.to_v, to_out[0])
+    parts = [lora.linear_parts(m) for m in linears]
+    if any(p is None for p in parts) or any(p[1] is not None for p in parts[:3]):
+        return None
+    for m in (attn,) + linears + tuple(to_out[1:]):
+        if m._forward_hooks or m._forward_pre_hooks:
+            return None
+    for extra in to_out[1:]:
+        if not isinstance(extra, torch.nn.Dropout) or (extra.p > 0 and extra.training):
+            return None
+    proc = getattr(attn, "processor", None)
+    if proc is not None and type(proc).__name__ not in _PLAIN_PROCESSORS:
+        return None
+    if getattr(attn, "group_norm", None) is not None or getattr(attn, "spatial_norm", None) is not None:
+        return None
+    if getattr(attn, "norm_cross", None) or getattr(attn, "residual_connection", False):
+        return None
+    if getattr(attn, "rescale_output_factor", 1.0) != 1.0:
+        return None
+    if getattr(attn, "added_kv_proj_dim", None) is not None or getattr(attn, "add_k_proj", None) is not None:
+        return None
+    return parts
+
+
+def head_dim_fits(attn: torch.nn.Module, C: int) -> bool:
+    """Whether `attn`'s heads split C channels into heads the flash kernel runs: a multiple of 8 up to max_head_dim()."""
+    d = C // int(attn.heads)
+    return d * int(attn.heads) == C and d % 8 == 0 and d <= max_head_dim()
+
+
 def _packed(attn: torch.nn.Module, like: torch.Tensor):
     """(w_qkv, w_o, b_o, lora_qkv, lora_o): the tensors of _packed_weights and the LoRA packs (lora.pack) of the QKV GEMM
     and of to_out[0] (None without adapters) — cached on the module, refreshed when a weight or adapter tensor is replaced
@@ -76,7 +123,7 @@ def self_attention(attn: torch.nn.Module, x: torch.Tensor, shared_qk: bool = Fal
 def self_attention_residual(attn: torch.nn.Module, x: torch.Tensor, resid: torch.Tensor,
                             shared_items: Optional[int] = None) -> torch.Tensor:
     """attn(x) + resid for an unmerged block (vidtome/patch.py:157-169 with do_nothing merges) through
-    vtm_attention_residual: the same kernels as self_attention, the add in the out projection's epilogue.
+    vtm_attention_residual_ex: the same kernels as self_attention, the add in the out projection's epilogue.
     shared_items: PnP injection on the block's frame items (utils/pnp_utils.py:57-68,86-91, vtm_attention_residual_ex):
     item b uses the attention map of item b mod shared_items."""
     w_qkv, w_o, b_o, lora_qkv, lora_o = _packed(attn, x)
@@ -87,35 +134,13 @@ def self_attention_residual(attn: torch.nn.Module, x: torch.Tensor, resid: torch
 
 
 def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:
-    """True if `attn` is a stock diffusers-style cross-attention (to_q [C, C], to_k / to_v [C, Cctx] without bias,
-    to_out = [Linear, Dropout], default processor, no hooks / overrides / options that alter the math).  The projections
-    may be LoRA-adapted in any form lora.linear_parts reads."""
-    from .patch import _PLAIN_PROCESSORS
+    """True if `attn` is a stock cross-attention (stock_attention_parts) with no instance-level forward, to_q [C, C] fp16
+    on CUDA, to_k / to_v [C, Cctx] and to_out[0] [C, C], for a 3-D fp16 context `ctx` of Cctx % 8 == 0 channels, and
+    heads the flash kernel runs (head_dim_fits)."""
     if attn is None or "forward" in vars(attn) or not isinstance(ctx, torch.Tensor) or ctx.dim() != 3:
         return False
-    need = ("to_q", "to_k", "to_v", "to_out", "heads")
-    if not all(hasattr(attn, n) for n in need):
-        return False
-    to_out = attn.to_out
-    if not isinstance(to_out, (torch.nn.ModuleList, torch.nn.Sequential)) or len(to_out) < 1:
-        return False
-    linears = (attn.to_q, attn.to_k, attn.to_v, to_out[0])
-    parts = [lora.linear_parts(m) for m in linears]
-    if any(p is None for p in parts) or any(p[1] is not None for p in parts[:3]):
-        return False
-    for m in (attn,) + linears + tuple(to_out[1:]):
-        if m._forward_hooks or m._forward_pre_hooks:
-            return False
-    for extra in to_out[1:]:
-        if not isinstance(extra, torch.nn.Dropout) or (extra.p > 0 and extra.training):
-            return False
-    proc = getattr(attn, "processor", None)
-    if proc is not None and type(proc).__name__ not in _PLAIN_PROCESSORS:
-        return False
-    for name, bad in (("group_norm", None), ("spatial_norm", None), ("norm_cross", None), ("added_kv_proj_dim", None)):
-        if getattr(attn, name, None) not in (None, False):
-            return False
-    if getattr(attn, "residual_connection", False) or getattr(attn, "rescale_output_factor", 1.0) != 1.0:
+    parts = stock_attention_parts(attn)
+    if parts is None:
         return False
     wq, wk, wv, wo = (p[0] for p in parts)
     C = wq.shape[1]
@@ -126,12 +151,11 @@ def cross_attention_eligible(attn: torch.nn.Module, ctx: torch.Tensor) -> bool:
         return False
     if wq.dtype != torch.float16 or not wq.is_cuda or ctx.dtype != torch.float16:
         return False
-    d = C // int(attn.heads)
-    return d * int(attn.heads) == C and d % 8 == 0 and d <= max_head_dim()
+    return head_dim_fits(attn, C)
 
 
 def cross_attention_residual(attn: torch.nn.Module, x: torch.Tensor, ctx: torch.Tensor, resid: torch.Tensor) -> torch.Tensor:
-    """attn2(x, encoder_hidden_states=ctx) + resid (vidtome/patch.py:171-185) through vtm_cross_attention."""
+    """attn2(x, encoder_hidden_states=ctx) + resid (vidtome/patch.py:171-185) through vtm_cross_attention_lora."""
     parts = [lora.linear_parts(m) for m in (attn.to_q, attn.to_k, attn.to_v, attn.to_out[0])]
     tag = lora.tag(parts)
     cache = getattr(attn, "_vtm_packed_x", None)

@@ -1,4 +1,4 @@
-"""Thin torch-tensor wrappers over the C-ABI (one function per entry point of include/vidtome_b200.h).
+"""Thin torch-tensor wrappers over the C-ABI of include/vidtome_b200.h, one library call per op.
 
 torch is used here only for device memory and streams.  Every function requires CUDA fp16 / int32
 tensors and raises on anything else — there is no CPU or eager-PyTorch implementation behind these.
@@ -353,6 +353,14 @@ def _lora_ref(desc):
     return None if desc is None else C.byref(desc)
 
 
+def _lora_workspace(lib, M: int, R: int, device):
+    """(workspace tensor or None, its bytes) for the low-rank T of a LoRA projection of M rows; none without LoRA."""
+    if not R:
+        return None, 0
+    ws_bytes = lib.vtm_linear_lora_workspace_bytes(M, R)
+    return torch.empty(ws_bytes, dtype=torch.uint8, device=device), ws_bytes
+
+
 def linear(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
     """D = A W^T (+ bias) on the wgmma GEMM.  a [M, K], w [N, K] fp16."""
     _require(a, torch.float16, "a")
@@ -383,20 +391,12 @@ def linear_residual(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tenso
     if bias is not None:
         _require(bias, torch.float16, "bias")
     desc, R = _lora_arg(lora, K, N, "linear_residual")
-    if desc is not None:
-        lib = _lib.load()
-        ws_bytes = lib.vtm_linear_lora_workspace_bytes(M, R)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=a.device)
-        with _Timed("FF2", 2.0 * M * (N + R) * K + 2.0 * M * N * R, 2.0 * (M * K + N * K + 2 * M * N)):
-            check(lib.vtm_linear_lora_f16(a.data_ptr(), w.data_ptr(), _ptr(bias), resid.data_ptr(), N, C.byref(desc), M,
-                                          N, K, d.data_ptr(), N, ws.data_ptr(), ws_bytes, _stream()),
-                  "vtm_linear_lora_f16")
-        STATS.launches += 2
-        return d
-    with _Timed("FF2", 2.0 * M * N * K, 2.0 * (M * K + N * K + 2 * M * N)):
-        check(_lib.load().vtm_linear_residual_f16(a.data_ptr(), w.data_ptr(), _ptr(bias), resid.data_ptr(), N, M, N, K,
-                                                  d.data_ptr(), N, _stream()), "vtm_linear_residual_f16")
-    STATS.launches += 1
+    lib = _lib.load()
+    ws, ws_bytes = _lora_workspace(lib, M, R, a.device)
+    with _Timed("FF2", 2.0 * M * (N + R) * K + 2.0 * M * N * R, 2.0 * (M * K + N * K + 2 * M * N)):
+        check(lib.vtm_linear_lora_f16(a.data_ptr(), w.data_ptr(), _ptr(bias), resid.data_ptr(), N, _lora_ref(desc), M, N,
+                                      K, d.data_ptr(), N, _ptr(ws), ws_bytes, _stream()), "vtm_linear_lora_f16")
+    STATS.launches += 1 + (R > 0)
     return d
 
 
@@ -424,20 +424,13 @@ def linear_geglu(a: torch.Tensor, w_il: torch.Tensor, bias_il: Optional[torch.Te
     if bias_il is not None:
         _require(bias_il, torch.float16, "bias_il")
     desc, R = _lora_arg(lora, K, N, "linear_geglu")
-    if desc is not None:
-        lib = _lib.load()
-        ws_bytes = lib.vtm_linear_lora_workspace_bytes(M, R)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=a.device)
-        with _Timed("FF1", 2.0 * M * (N + R) * K + 2.0 * M * N * R, 2.0 * (M * K + N * K + M * N // 2)):
-            check(lib.vtm_linear_geglu_lora_f16(a.data_ptr(), w_il.data_ptr(), _ptr(bias_il), C.byref(desc), M, N, K,
-                                                d.data_ptr(), N // 2, ws.data_ptr(), ws_bytes, _stream()),
-                  "vtm_linear_geglu_lora_f16")
-        STATS.launches += 2
-        return d
-    with _Timed("FF1", 2.0 * M * N * K, 2.0 * (M * K + N * K + M * N // 2)):
-        check(_lib.load().vtm_linear_geglu_f16(a.data_ptr(), w_il.data_ptr(), _ptr(bias_il), M, N, K, d.data_ptr(), N // 2,
-                                               _stream()), "vtm_linear_geglu_f16")
-    STATS.launches += 1
+    lib = _lib.load()
+    ws, ws_bytes = _lora_workspace(lib, M, R, a.device)
+    with _Timed("FF1", 2.0 * M * (N + R) * K + 2.0 * M * N * R, 2.0 * (M * K + N * K + M * N // 2)):
+        check(lib.vtm_linear_geglu_lora_f16(a.data_ptr(), w_il.data_ptr(), _ptr(bias_il), _lora_ref(desc), M, N, K,
+                                            d.data_ptr(), N // 2, _ptr(ws), ws_bytes, _stream()),
+              "vtm_linear_geglu_lora_f16")
+    STATS.launches += 1 + (R > 0)
     return d
 
 
@@ -458,39 +451,20 @@ def attention(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, b_o: Opti
     _require(w_qkv, torch.float16, "w_qkv")
     _require(w_o, torch.float16, "w_o")
     B, L, Cc = x.shape
-    lib = _lib.load()
-    if lora_qkv is not None or lora_o is not None:
-        dq, rq = _lora_arg(lora_qkv, Cc, 3 * Cc, "attention qkv")
-        do, ro = _lora_arg(lora_o, Cc, Cc, "attention out")
-        ws_bytes = lib.vtm_attention_lora_workspace_bytes(B, L, Cc, heads, rq, ro)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        y = torch.empty_like(x)
-        if seq_len is not None:
-            _require(seq_len, torch.int32, "seq_len")
-        flops = 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc + 8.0 * B * L * Cc * (rq + ro)
-        with _Timed("KD", flops, 4.0 * B * L * Cc + 8.0 * Cc * Cc):
-            check(lib.vtm_attention_lora(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), _lora_ref(dq),
-                                         _lora_ref(do), B, L, Cc, heads, float(scale), 1 if shared_qk else 0,
-                                         _ptr(seq_len), y.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
-                  "vtm_attention_lora")
-        STATS.launches += 3 + (rq > 0) + (ro > 0)
-        return y
-    ws_bytes = lib.vtm_attention_workspace_bytes(B, L, Cc, heads)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-    y = torch.empty_like(x)
     if seq_len is not None:
         _require(seq_len, torch.int32, "seq_len")
-        with _Timed("KD", 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc, 4.0 * B * L * Cc + 8.0 * Cc * Cc):
-            check(lib.vtm_attention_dev(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), B, L, Cc, heads,
-                                        float(scale), 1 if shared_qk else 0, seq_len.data_ptr(), y.data_ptr(),
-                                        ws.data_ptr(), ws_bytes, _stream()), "vtm_attention_dev")
-        STATS.launches += 3
-        return y
-    with _Timed("KD", 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc, 4.0 * B * L * Cc + 8.0 * Cc * Cc):
-        check(lib.vtm_attention_ex(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), B, L, Cc, heads,
-                                   float(scale), 1 if shared_qk else 0, y.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
-              "vtm_attention_ex")
-    STATS.launches += 3
+    lib = _lib.load()
+    dq, rq = _lora_arg(lora_qkv, Cc, 3 * Cc, "attention qkv")
+    do, ro = _lora_arg(lora_o, Cc, Cc, "attention out")
+    ws_bytes = lib.vtm_attention_lora_workspace_bytes(B, L, Cc, heads, rq, ro)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+    y = torch.empty_like(x)
+    flops = 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc + 8.0 * B * L * Cc * (rq + ro)
+    with _Timed("KD", flops, 4.0 * B * L * Cc + 8.0 * Cc * Cc):
+        check(lib.vtm_attention_lora(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), _lora_ref(dq),
+                                     _lora_ref(do), B, L, Cc, heads, float(scale), 1 if shared_qk else 0, _ptr(seq_len),
+                                     y.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "vtm_attention_lora")
+    STATS.launches += 3 + (rq > 0) + (ro > 0)
     return y
 
 
@@ -521,17 +495,12 @@ def attention_residual(x: torch.Tensor, w_qkv: torch.Tensor, w_o: torch.Tensor, 
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
     y = torch.empty_like(x)
     flops = 4.0 * B * L * L * Cc + 8.0 * B * L * Cc * Cc + 8.0 * B * L * Cc * (rq + ro)
+    flags, qk_items = (0, 1) if shared_items is None else (1, int(shared_items))
     with _Timed("KD", flops, 6.0 * B * L * Cc + 8.0 * Cc * Cc):
-        if shared_items is None:
-            check(lib.vtm_attention_residual(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o),
-                                             resid.data_ptr(), _lora_ref(dq), _lora_ref(do), B, L, Cc, heads,
-                                             float(scale), y.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
-                  "vtm_attention_residual")
-        else:
-            check(lib.vtm_attention_residual_ex(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o),
-                                                resid.data_ptr(), _lora_ref(dq), _lora_ref(do), B, L, Cc, heads,
-                                                float(scale), 1, int(shared_items), y.data_ptr(), ws.data_ptr(),
-                                                ws_bytes, _stream()), "vtm_attention_residual_ex")
+        check(lib.vtm_attention_residual_ex(x.data_ptr(), w_qkv.data_ptr(), w_o.data_ptr(), _ptr(b_o), resid.data_ptr(),
+                                            _lora_ref(dq), _lora_ref(do), B, L, Cc, heads, float(scale), flags, qk_items,
+                                            y.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
+              "vtm_attention_residual_ex")
     STATS.launches += 3 + (rq > 0) + (ro > 0)
     return y
 
@@ -587,30 +556,20 @@ def cross_attention(x: torch.Tensor, ctx: torch.Tensor, w_q: torch.Tensor, w_kv:
     if resid is not None:
         _require(resid, torch.float16, "resid")
     lib = _lib.load()
-    flops = 4.0 * B * Lq * Lk * Cc + 4.0 * B * Lq * Cc * Cc + 4.0 * B * Lk * Cctx * Cc
-    if lora_q is not None or lora_kv is not None or lora_o is not None:
-        dq, rq = _lora_arg(lora_q, Cc, Cc, "cross_attention q")
-        dkv, rkv = _lora_arg(lora_kv, Cctx, 2 * Cc, "cross_attention kv")
-        do, ro = _lora_arg(lora_o, Cc, Cc, "cross_attention out")
-        ws_bytes = lib.vtm_cross_attention_lora_workspace_bytes(B, Lq, Lk, Cc, heads, rq, rkv, ro)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-        y = torch.empty_like(x)
-        flops += 4.0 * B * Lq * Cc * (rq + ro) + 2.0 * B * Lk * (Cctx + 2 * Cc) * rkv
-        with _Timed("XA", flops, 2.0 * B * Lq * Cc * (3 if resid is not None else 2)):
-            check(lib.vtm_cross_attention_lora(x.data_ptr(), ctx.data_ptr(), w_q.data_ptr(), w_kv.data_ptr(),
-                                               w_o.data_ptr(), _ptr(b_o), _ptr(resid), _lora_ref(dq), _lora_ref(dkv),
-                                               _lora_ref(do), B, Lq, Lk, Cc, Cctx, heads, float(scale), y.data_ptr(),
-                                               ws.data_ptr(), ws_bytes, _stream()), "vtm_cross_attention_lora")
-        STATS.launches += 4 + (rq > 0) + (rkv > 0) + (ro > 0)
-        return y
-    ws_bytes = lib.vtm_cross_attention_workspace_bytes(B, Lq, Lk, Cc, heads)
+    dq, rq = _lora_arg(lora_q, Cc, Cc, "cross_attention q")
+    dkv, rkv = _lora_arg(lora_kv, Cctx, 2 * Cc, "cross_attention kv")
+    do, ro = _lora_arg(lora_o, Cc, Cc, "cross_attention out")
+    ws_bytes = lib.vtm_cross_attention_lora_workspace_bytes(B, Lq, Lk, Cc, heads, rq, rkv, ro)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
     y = torch.empty_like(x)
+    flops = (4.0 * B * Lq * Lk * Cc + 4.0 * B * Lq * Cc * Cc + 4.0 * B * Lk * Cctx * Cc
+             + (4.0 * B * Lq * Cc * (rq + ro) + 2.0 * B * Lk * (Cctx + 2 * Cc) * rkv))
     with _Timed("XA", flops, 2.0 * B * Lq * Cc * (3 if resid is not None else 2)):
-        check(lib.vtm_cross_attention(x.data_ptr(), ctx.data_ptr(), w_q.data_ptr(), w_kv.data_ptr(), w_o.data_ptr(), _ptr(b_o),
-                                      _ptr(resid), B, Lq, Lk, Cc, Cctx, heads, float(scale), y.data_ptr(), ws.data_ptr(),
-                                      ws_bytes, _stream()), "vtm_cross_attention")
-    STATS.launches += 4
+        check(lib.vtm_cross_attention_lora(x.data_ptr(), ctx.data_ptr(), w_q.data_ptr(), w_kv.data_ptr(), w_o.data_ptr(),
+                                           _ptr(b_o), _ptr(resid), _lora_ref(dq), _lora_ref(dkv), _lora_ref(do), B, Lq,
+                                           Lk, Cc, Cctx, heads, float(scale), y.data_ptr(), ws.data_ptr(), ws_bytes,
+                                           _stream()), "vtm_cross_attention_lora")
+    STATS.launches += 4 + (rq > 0) + (rkv > 0) + (ro > 0)
     return y
 
 

@@ -21,9 +21,8 @@ from typing import Any, Callable, Dict, List, Optional, Tuple, Type
 
 import torch
 
-from . import merge, ops
+from . import attention, feedforward, merge, ops
 from ._lib import VtmSplit
-from .lora import linear_parts
 from .utils import (draw_coin, draw_randf, func_warper, init_generator, isinstance_str, join_frame, join_warper,
                     split_frame, split_warper)
 
@@ -112,7 +111,7 @@ def _unmerged_blocks():
     first, on the unpatched UNet; SURVEY App. C.13).  Inside, a ToMeBlock builds no merge plan (nothing is drawn,
     `global_tokens` is left alone), its pre-hook forks no generator, and no PnP injection runs whatever `t` the marked
     modules hold (pnp.injection_active).  attn1 of a stock module (_plain_attention_module) runs as norm1 -> KD with the
-    residual in its out projection (vtm_attention_residual), PnP-marked modules included; any other attn1 runs its own
+    residual in its out projection (vtm_attention_residual_ex), PnP-marked modules included; any other attn1 runs its own
     forward.  attn2 and ff go through the library as they do outside."""
     global _UNMERGED
     _UNMERGED += 1
@@ -411,50 +410,17 @@ def compute_merge(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[str,
     return m, u, merged
 
 
-# attention processors whose result is plain softmax(q k^T * scale) v (what KD computes)
-_PLAIN_PROCESSORS = ("AttnProcessor", "AttnProcessor2_0", "XFormersAttnProcessor")
-
-
 def _plain_attention_module(attn: torch.nn.Module) -> bool:
-    """True only if replacing `attn.forward` by KD cannot change the result: `attn` is a stock diffusers-style
-    Attention whose projections are bare `torch.nn.Linear` or LoRA-adapted layers that lora.linear_parts reads (their
-    low-rank terms then run as extra K steps of KD's projection GEMMs; any other subclass or wrapper carries terms KD
-    would miss), to_q/to_k/to_v without bias, to_out = [Linear, Dropout(inactive)],
-    no instance-level forward override (PnP installs one, utils/pnp_utils.py:99-101), no forward hooks, a default
-    attention processor (or none), and none of the Attention options that alter the math (group / spatial norm,
-    residual connection, output rescale, added KV projections).  Anything else goes through `self.attn1(...)`
-    exactly as the reference does (patch.py:157-162), e.g. after `pipe.load_lora_weights` (generate.py:93-94)."""
+    """True only if replacing `attn.forward` by KD cannot change the result: `attn` is a stock Attention
+    (attention.stock_attention_parts; LoRA-adapted projections run as extra K steps of KD's projection GEMMs) with no
+    instance-level forward override other than PnP's (utils/pnp_utils.py:99-101), to_q / to_k / to_v / to_out[0] all
+    [C, C], and heads KD runs (attention.head_dim_fits).  Anything else goes through `self.attn1(...)` exactly as the
+    reference does (patch.py:157-162), e.g. after `pipe.load_lora_weights` (generate.py:93-94)."""
     override = vars(attn).get("forward")
     if override is not None and not getattr(override, "_vtm_pnp_forward", False):
         return False                       # someone else's replaced forward (e.g. the reference's own PnP closure)
-    need = ("to_q", "to_k", "to_v", "to_out", "heads")
-    if not all(hasattr(attn, n) for n in need):
-        return False
-    to_out = attn.to_out
-    if not isinstance(to_out, (torch.nn.ModuleList, torch.nn.Sequential)) or len(to_out) < 1:
-        return False
-    linears = (attn.to_q, attn.to_k, attn.to_v, to_out[0])
-    parts = [linear_parts(m) for m in linears]
-    if any(p is None for p in parts):
-        return False
-    if any(p[1] is not None for p in parts[:3]):
-        return False
-    for m in (attn,) + linears + tuple(to_out[1:]):
-        if m._forward_hooks or m._forward_pre_hooks or getattr(m, "_forward_hooks_with_kwargs", None):
-            return False
-    for extra in to_out[1:]:
-        if not isinstance(extra, torch.nn.Dropout) or (extra.p > 0 and extra.training):
-            return False
-    proc = getattr(attn, "processor", None)
-    if proc is not None and type(proc).__name__ not in _PLAIN_PROCESSORS:
-        return False
-    if getattr(attn, "group_norm", None) is not None or getattr(attn, "spatial_norm", None) is not None:
-        return False
-    if getattr(attn, "norm_cross", None) or getattr(attn, "residual_connection", False):
-        return False
-    if getattr(attn, "rescale_output_factor", 1.0) != 1.0:
-        return False
-    if getattr(attn, "added_kv_proj_dim", None) is not None or getattr(attn, "add_k_proj", None) is not None:
+    parts = attention.stock_attention_parts(attn)
+    if parts is None:
         return False
     wq, wk, wv, wo = (p[0] for p in parts)
     C = wq.shape[1]
@@ -462,9 +428,134 @@ def _plain_attention_module(attn: torch.nn.Module) -> bool:
         return False                       # inner dim != query dim or cross-attention shaped K/V
     if wv.shape != wq.shape or wo.shape != (C, C):
         return False
-    from .attention import max_head_dim
-    head_dim = C // int(attn.heads)
-    return head_dim * int(attn.heads) == C and head_dim % 8 == 0 and head_dim <= max_head_dim()   # KD's enabled range
+    return attention.head_dim_fits(attn, C)
+
+
+def _pnp_shared_items(attn: torch.nn.Module, batch: int) -> Optional[int]:
+    """While PnP injects into `attn` (pnp.injection_active; the batch is num_inputs runs of [source | uncond | cond]
+    items): how many items lead, item b taking the attention map of item b mod that count (batch / num_inputs), or 0 if
+    the batch is not a whole number of runs.  None when nothing is injected."""
+    num_inputs = getattr(attn, "_vtm_pnp", 0)
+    if not num_inputs:
+        return None
+    from . import pnp
+    if not pnp.injection_active(attn):                                    # never inside _unmerged_blocks()
+        return None
+    return 0 if batch % num_inputs else batch // num_inputs
+
+
+def _self_attention_stage(block, hidden_states, attention_mask, encoder_hidden_states, timestep, class_labels,
+                          cross_attention_kwargs):
+    """norm1 -> [merge] -> attn1 -> [unmerge] + residual (patch.py:139-169).  Returns the hidden states and, for an
+    AdaNorm-zero norm1, its (shift_mlp, scale_mlp, gate_mlp) for the feed-forward, else None."""
+    unmerged = _UNMERGED > 0 or block._vtm_unmerged
+    only_cross = getattr(block, "only_cross_attention", False)
+
+    def library_attn1(route) -> bool:
+        # attn1 runs in the library (KD): no mask, no kwargs, a stock module; `route()` is the route's own condition
+        return (attention.ENABLED and not only_cross and attention_mask is None and not cross_attention_kwargs
+                and route() and _plain_attention_module(block.attn1))
+
+    if (hidden_states.is_cuda and hidden_states.dtype == torch.float16 and not block.use_ada_layer_norm
+            and not block.use_ada_layer_norm_zero
+            and library_attn1(lambda: unmerged or (FUSE_UNMERGED_ATTENTION
+                                                   and not block_merges(hidden_states, block._tome_info)))):
+        ln1 = _fusable_layer_norm(block.norm1, hidden_states)
+        shared_items = None if ln1 is None else _pnp_shared_items(block.attn1, hidden_states.shape[0])
+        if ln1 is not None and shared_items != 0:   # else the module's forward, which fails as the reference's
+            # a block that does not merge (_unmerged_blocks, or FUSE_UNMERGED_ATTENTION): attn1(norm1(h)) + h, the add
+            # in the out projection of KD; with PnP injecting, item b takes the map of item b mod shared_items
+            shape = hidden_states.shape
+            hidden_states = hidden_states.contiguous()
+            n1 = ops.layer_norm(hidden_states.view(-1, shape[-1]), ln1).view(shape)
+            return attention.self_attention_residual(block.attn1, n1, hidden_states, shared_items=shared_items), None
+
+    plan = None
+    mlp_terms = None
+    if block.use_ada_layer_norm:                                                  # patch.py:139-146
+        norm_hidden_states = block.norm1(hidden_states, timestep)
+    elif block.use_ada_layer_norm_zero:
+        norm_hidden_states, gate_msa, *mlp_terms = block.norm1(hidden_states, timestep, class_labels,
+                                                               hidden_dtype=hidden_states.dtype)
+    else:
+        ln = _fusable_layer_norm(block.norm1, hidden_states) if hidden_states.is_cuda and not unmerged else None
+        if ln is not None:
+            # norm1 fused into the merge kernels: only the kept rows are ever normalised
+            plan = build_merge_plan(block, hidden_states, block._tome_info, ln=ln)
+        norm_hidden_states = None if plan is not None else block.norm1(hidden_states)
+
+    if plan is None and not unmerged:
+        plan = build_merge_plan(block, norm_hidden_states, block._tome_info)   # patch.py:149-150
+    if plan is not None:
+        norm_hidden_states = plan.merged_tokens
+
+    # 1. Self-Attention (patch.py:154-162)
+    if library_attn1(lambda: plan is not None):
+        # KD; with PnP control registered (pnp.py) and the timestep inside the injection schedule, the attention map of
+        # the source sample is applied to every sample's values (utils/pnp_utils.py:57-68, 87-91)
+        shared_items = _pnp_shared_items(block.attn1, norm_hidden_states.shape[0])
+        if shared_items not in (None, 1):
+            raise RuntimeError("PnP injection needs one merged token set per input (batch_size == num_inputs)")
+        attn_output = attention.self_attention(block.attn1, norm_hidden_states, shared_qk=shared_items == 1,
+                                               seq_len=plan.seq_len)                                      # KD
+    elif plan is not None and plan.seq_len is not None:
+        raise RuntimeError("GlobalTokenStore: the merged tokens are sized for capacity with their length on the device, "
+                           "which only the library's self-attention (KD) reads; this block's attn1 runs its own forward")
+    else:
+        attn_output = block.attn1(norm_hidden_states, encoder_hidden_states=encoder_hidden_states if only_cross else None,
+                                  attention_mask=attention_mask, **cross_attention_kwargs)
+    if block.use_ada_layer_norm_zero:
+        attn_output = gate_msa.unsqueeze(1) * attn_output                        # patch.py:164-165
+
+    # Unmerge + residual (patch.py:168-169), fused into one pass
+    if plan is not None:
+        return plan.unmerge_add(attn_output, hidden_states), mlp_terms
+    return attn_output + hidden_states, mlp_terms
+
+
+def _cross_attention_stage(block, hidden_states, encoder_hidden_states, encoder_attention_mask, timestep,
+                           cross_attention_kwargs):
+    """norm2 -> attn2 + residual (patch.py:171-185)."""
+    attn2 = getattr(block, "attn2", None)
+    if attn2 is None:
+        return hidden_states
+    if (FUSE_CROSS_ATTENTION and hidden_states.is_cuda and not block.use_ada_layer_norm
+            and encoder_attention_mask is None and not cross_attention_kwargs
+            and attention.cross_attention_eligible(attn2, encoder_hidden_states)
+            and encoder_hidden_states.shape[0] == hidden_states.shape[0]):
+        ln2 = _fusable_layer_norm(block.norm2, hidden_states)
+        if ln2 is not None:
+            # norm2 -> q / kv projections (head-major) -> flash attention over the context -> out projection with bias
+            # and residual fused, all in the CUDA library
+            shape = hidden_states.shape
+            n2 = ops.layer_norm(hidden_states.contiguous().view(-1, shape[-1]), ln2).view(shape)
+            return attention.cross_attention_residual(attn2, n2, encoder_hidden_states, hidden_states)
+    norm_hidden_states = block.norm2(hidden_states, timestep) if block.use_ada_layer_norm else block.norm2(hidden_states)
+    attn_output = attn2(norm_hidden_states, encoder_hidden_states=encoder_hidden_states,
+                        attention_mask=encoder_attention_mask, **cross_attention_kwargs)
+    return attn_output + hidden_states
+
+
+def _feed_forward_stage(block, hidden_states, mlp_terms):
+    """norm3 -> ff + residual (patch.py:187-199), with AdaNorm-zero's (shift_mlp, scale_mlp, gate_mlp) or None.  A block
+    without `ff` (the hot-path skeleton used by bench.py) stops after the earlier stages."""
+    ff = getattr(block, "ff", None)
+    if ff is None:
+        return hidden_states
+    if FUSE_FEED_FORWARD and hidden_states.is_cuda and not block.use_ada_layer_norm_zero:
+        parts = feedforward.geglu_parts(ff)
+        ln3 = _fusable_layer_norm(block.norm3, hidden_states) if parts is not None else None
+        if ln3 is not None:
+            # norm3 -> GEGLU projection (gate fused) -> output projection (+ bias + residual), wgmma
+            return feedforward.feed_forward_residual(ff, parts, ln3, hidden_states)
+    norm_hidden_states = block.norm3(hidden_states)
+    if mlp_terms is not None:
+        shift_mlp, scale_mlp, gate_mlp = mlp_terms
+        norm_hidden_states = norm_hidden_states * (1 + scale_mlp[:, None]) + shift_mlp[:, None]
+    ff_output = ff(norm_hidden_states)
+    if mlp_terms is not None:
+        ff_output = gate_mlp.unsqueeze(1) * ff_output
+    return ff_output + hidden_states
 
 
 def make_tome_block(block_class: Type[torch.nn.Module]) -> Type[torch.nn.Module]:
@@ -487,129 +578,12 @@ def make_diffusers_tome_block(block_class: Type[torch.nn.Module]) -> Type[torch.
         def forward(self, hidden_states, attention_mask=None, encoder_hidden_states=None,
                     encoder_attention_mask=None, timestep=None, cross_attention_kwargs=None,
                     class_labels=None) -> torch.Tensor:
-            plan = None
-            unmerged = _UNMERGED > 0 or self._vtm_unmerged
             cross_attention_kwargs = cross_attention_kwargs if cross_attention_kwargs is not None else {}
-            only_cross = getattr(self, "only_cross_attention", False)
-            from . import attention as _attention
-            ln1 = None
-            shared_items = None
-            if (hidden_states.is_cuda and hidden_states.dtype == torch.float16 and _attention.ENABLED
-                    and not self.use_ada_layer_norm and not self.use_ada_layer_norm_zero and not only_cross
-                    and attention_mask is None and not cross_attention_kwargs
-                    and (unmerged or (FUSE_UNMERGED_ATTENTION and not block_merges(hidden_states, self._tome_info)))
-                    and _plain_attention_module(self.attn1)):
-                ln1 = _fusable_layer_norm(self.norm1, hidden_states)
-                num_inputs = getattr(self.attn1, "_vtm_pnp", 0)
-                if ln1 is not None and num_inputs:
-                    from . import pnp as _pnp
-                    if _pnp.injection_active(self.attn1):             # never inside _unmerged_blocks()
-                        if hidden_states.shape[0] % num_inputs:
-                            ln1 = None                                # the module's forward, which fails as the reference's
-                        else:
-                            shared_items = hidden_states.shape[0] // num_inputs
-            if ln1 is not None:
-                # a block that does not merge (_unmerged_blocks, or FUSE_UNMERGED_ATTENTION): attn1(norm1(h)) + h, the
-                # add in the out projection of KD; with PnP injecting, item b takes the map of item b mod shared_items
-                shape = hidden_states.shape
-                hidden_states = hidden_states.contiguous()
-                n1 = ops.layer_norm(hidden_states.view(-1, shape[-1]), ln1).view(shape)
-                if shared_items is None:
-                    hidden_states = _attention.self_attention_residual(self.attn1, n1, hidden_states)
-                else:
-                    hidden_states = _attention.self_attention_residual(self.attn1, n1, hidden_states,
-                                                                       shared_items=shared_items)
-            else:
-                if self.use_ada_layer_norm:                                       # patch.py:139-146
-                    norm_hidden_states = self.norm1(hidden_states, timestep)
-                elif self.use_ada_layer_norm_zero:
-                    norm_hidden_states, gate_msa, shift_mlp, scale_mlp, gate_mlp = self.norm1(
-                        hidden_states, timestep, class_labels, hidden_dtype=hidden_states.dtype)
-                else:
-                    ln = (_fusable_layer_norm(self.norm1, hidden_states) if hidden_states.is_cuda and not unmerged
-                          else None)
-                    if ln is not None:
-                        # norm1 fused into the merge kernels: only the kept rows are ever normalised
-                        plan = build_merge_plan(self, hidden_states, self._tome_info, ln=ln)
-                    norm_hidden_states = None if plan is not None else self.norm1(hidden_states)
-
-                if plan is None and not unmerged:
-                    plan = build_merge_plan(self, norm_hidden_states, self._tome_info)  # patch.py:149-150
-                if plan is not None:
-                    norm_hidden_states = plan.merged_tokens
-
-                # 1. Self-Attention (patch.py:154-162)
-                if (plan is not None and _attention.ENABLED and not only_cross and attention_mask is None
-                        and not cross_attention_kwargs and _plain_attention_module(self.attn1)):
-                    # KD; with PnP control registered (pnp.py) and the timestep inside the injection schedule, the
-                    # attention map of the source sample is applied to every sample's values (utils/pnp_utils.py:57-68,
-                    # 87-91)
-                    shared = False
-                    if getattr(self.attn1, "_vtm_pnp", 0):
-                        from . import pnp as _pnp
-                        shared = _pnp.injection_active(self.attn1)
-                        if shared and norm_hidden_states.shape[0] != self.attn1._vtm_pnp:
-                            raise RuntimeError("PnP injection needs one merged token set per input "
-                                               "(batch_size == num_inputs)")
-                    attn_output = _attention.self_attention(self.attn1, norm_hidden_states, shared_qk=shared,
-                                                            seq_len=plan.seq_len)                             # KD
-                elif plan is not None and plan.seq_len is not None:
-                    raise RuntimeError("GlobalTokenStore: the merged tokens are sized for capacity with their length on "
-                                       "the device, which only the library's self-attention (KD) reads; this block's "
-                                       "attn1 runs its own forward")
-                else:
-                    attn_output = self.attn1(
-                        norm_hidden_states,
-                        encoder_hidden_states=encoder_hidden_states if only_cross else None,
-                        attention_mask=attention_mask, **cross_attention_kwargs)
-                if self.use_ada_layer_norm_zero:
-                    attn_output = gate_msa.unsqueeze(1) * attn_output            # patch.py:164-165
-
-                # Unmerge + residual (patch.py:168-169), fused into one pass
-                if plan is not None:
-                    hidden_states = plan.unmerge_add(attn_output, hidden_states)
-                else:
-                    hidden_states = attn_output + hidden_states
-
-            attn2 = getattr(self, "attn2", None)
-            if (attn2 is not None and FUSE_CROSS_ATTENTION and hidden_states.is_cuda and not self.use_ada_layer_norm
-                    and encoder_attention_mask is None and not cross_attention_kwargs
-                    and _attention.cross_attention_eligible(attn2, encoder_hidden_states)
-                    and encoder_hidden_states.shape[0] == hidden_states.shape[0]):
-                ln2 = _fusable_layer_norm(self.norm2, hidden_states)
-                if ln2 is not None:
-                    # norm2 -> q / kv projections (head-major) -> flash attention over the context -> out projection
-                    # with bias and residual fused (patch.py:171-185), all in the CUDA library
-                    shape = hidden_states.shape
-                    n2 = ops.layer_norm(hidden_states.contiguous().view(-1, shape[-1]), ln2).view(shape)
-                    hidden_states = _attention.cross_attention_residual(attn2, n2, encoder_hidden_states, hidden_states)
-                    attn2 = None
-            if attn2 is not None:                                            # patch.py:171-185
-                norm_hidden_states = (self.norm2(hidden_states, timestep) if self.use_ada_layer_norm
-                                      else self.norm2(hidden_states))
-                attn_output = self.attn2(norm_hidden_states, encoder_hidden_states=encoder_hidden_states,
-                                         attention_mask=encoder_attention_mask, **cross_attention_kwargs)
-                hidden_states = attn_output + hidden_states
-
-            # 3. Feed-forward (patch.py:187-199).  A block without `ff` (the hot-path skeleton used by
-            # bench.py) stops after the self-attention section.
-            ff = getattr(self, "ff", None)
-            if ff is not None and FUSE_FEED_FORWARD and hidden_states.is_cuda and not self.use_ada_layer_norm_zero:
-                from . import feedforward as _ff
-                parts = _ff.geglu_parts(ff)
-                ln3 = _fusable_layer_norm(self.norm3, hidden_states) if parts is not None else None
-                if ln3 is not None:
-                    # norm3 -> GEGLU projection (gate fused) -> output projection (+ bias + residual), wgmma
-                    return _ff.feed_forward_residual(ff, parts, ln3, hidden_states)
-            if ff is not None:
-                norm_hidden_states = self.norm3(hidden_states)
-                if self.use_ada_layer_norm_zero:
-                    norm_hidden_states = norm_hidden_states * (1 + scale_mlp[:, None]) + shift_mlp[:, None]
-                ff_output = self.ff(norm_hidden_states)
-                if self.use_ada_layer_norm_zero:
-                    ff_output = gate_mlp.unsqueeze(1) * ff_output
-                hidden_states = ff_output + hidden_states
-            return hidden_states
+            hidden_states, mlp_terms = _self_attention_stage(self, hidden_states, attention_mask, encoder_hidden_states,
+                                                             timestep, class_labels, cross_attention_kwargs)
+            hidden_states = _cross_attention_stage(self, hidden_states, encoder_hidden_states, encoder_attention_mask,
+                                                   timestep, cross_attention_kwargs)
+            return _feed_forward_stage(self, hidden_states, mlp_terms)
 
     return ToMeBlock
 

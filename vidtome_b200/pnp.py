@@ -9,7 +9,7 @@ cfg`) the merged token sets of the samples are aligned, so this is well defined 
 
 `register_attention_control(model, injection_schedule, num_inputs)` here has the reference's name and arguments.  It
 installs (i) an equivalent torch forward for every call that does not come through a merged ToMeBlock, and (ii) a marker
-(`attn._vtm_pnp`) that lets ToMeBlock run the same computation through KD (`vtm_attention_ex`, flag
+(`attn._vtm_pnp`) that lets ToMeBlock run the same computation through KD (`vtm_attention_lora`, flag
 VTM_ATTN_SHARED_QK: every sample reads the queries and keys of sample 0 and its own values).  `register_time(model, t)`
 sets `attn.t` on every marked module.
 
