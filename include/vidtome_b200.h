@@ -479,6 +479,27 @@ int vtm_ddim_update_f16(void* x_dev, const void* eps_dev, int64_t n, const float
                         const int32_t* step_dev, int32_t n_steps, void* traj_dev, int32_t n_slots, void* stream);
 
 /*
+ * KS — the sampling step's classifier-free guidance combine and DDIM update in one pass, for one chunk
+ * (generate.py:274-279, the guidance combine of pred_noise, and generate.py:281-311, pred_next_x with inversion=False):
+ *   u = eps[(samples - 2) n ..],  c = eps[(samples - 1) n ..]      (eps.chunk(samples)[-2:])
+ *   e = u + guidance * (c - u)
+ *   s = *step_dev;  (a, r, k, d) = coef_dev[4 s .. 4 s + 3];  out <- k * ((x - a * e) * r) + d * e
+ * with a = sigma, r = 1 / mu, k = mu_prev, d = sigma_prev (the rows ops.ddim_table builds).  A step outside
+ * [0, n_steps) writes nothing.
+ *   x_dev [n] fp16, the chunk's latents; eps_dev [samples, n] fp16, the UNet output of the chunk, samples 2
+ *   ([uncond | cond]) or 3 (PnP's [source | uncond | cond]); out_dev [n] fp16, either x_dev itself or a buffer that
+ *   overlaps neither x nor eps (VTM_E_SHAPE); any n >= 1; all three 2-byte aligned (VTM_E_SHAPE); coef_dev
+ *   [n_steps, 4] fp32, 16-byte aligned; step_dev int32, 4-byte aligned.  NULL pointers: VTM_E_NULL.
+ * Rounding is torch's, op for op: the guidance sub, mul and add each round to fp16, with `guidance` the fp32 value of
+ * the caller's python float (the opmath scalar of torch's half mul); then KI's five roundings.  NaN and inf propagate
+ * as through those torch ops.  16-byte vectors wherever x, u, c and out share their offset from a 16-byte boundary.
+ * No allocation, no synchronisation: capturable in a CUDA graph, where one capture serves every step.
+ */
+int vtm_cfg_ddim_update_f16(const void* x_dev, const void* eps_dev, int64_t n, int32_t samples, float guidance,
+                            const float* coef_dev, const int32_t* step_dev, int32_t n_steps, void* out_dev,
+                            void* stream);
+
+/*
  * KG1 / KG2 / NchwEpi — the entry and exit of diffusers' Transformer2DModel.forward, the module that owns every
  * BasicTransformerBlock of the UNet and works on NCHW activations (third-party code, not part of the reference; its
  * arithmetic is torch's):

@@ -68,5 +68,16 @@ y = ops.cross_attention(xq, ctx, wq, wkv, wq, torch.zeros(320, device="cuda").ha
 assert torch.isfinite(y).all()
 y = ops.attention(xq, torch.cat([wq, wq, wq], 0).contiguous(), wq, None, 8, 40 ** -0.5, shared_qk=True)
 assert torch.isfinite(y).all()
+# KS: the sampling step's guidance combine and DDIM update, vector path and element path (n % 8 != 0), in place
+coef = ops.ddim_table([(0.5, 0.9, 0.95, 0.3)] * 4).cuda()
+step = torch.full((1,), 2, dtype=torch.int32, device="cuda")
+for n, samples in [(4 * 64 * 64, 2), (3 * 4 * 15 * 15, 3)]:
+    xs = torch.randn((n + 1,), generator=g, device="cuda").half()
+    es = torch.randn((samples * n,), generator=g, device="cuda").half()
+    for x_ in (xs[:n], xs[1:]):
+        out = torch.empty_like(x_)
+        ops.cfg_ddim_update(x_, es, samples, 7.5, coef, step, out)
+        ops.cfg_ddim_update(x_, es, samples, 7.5, coef, step, x_)
+        assert torch.isfinite(out).all()
 torch.cuda.synchronize()
 print("sanitize_small: ok")

@@ -146,6 +146,7 @@ SIGNATURES = {
     "vtm_attention_residual_ex": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _LORA, _LORA, _i32, _i32, _i32, _i32, C.c_float,
                                             _i32, _i32, _vp, _vp, _sz, _vp]),
     "vtm_ddim_update_f16": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp, _i32, _vp, _i32, _vp]),
+    "vtm_cfg_ddim_update_f16": (C.c_int, [_vp, _vp, _i64, _i32, C.c_float, _vp, _vp, _i32, _vp, _vp]),
     "vtm_group_norm_stats_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
     "vtm_group_norm_stats_f16": (C.c_int, [_vp, _i32, _i32, _i32, _i32, C.c_float, _vp, _vp, _sz, _vp]),
     "vtm_group_norm_tokens_f16": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),

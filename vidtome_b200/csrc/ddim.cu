@@ -14,6 +14,10 @@
 // The pass streams 16-byte vectors; the elements before x's first 16-byte boundary and after its last one are done one
 // by one, and when eps or the trajectory slot sits at another offset from a 16-byte boundary (possible when n % 8 != 0)
 // the whole pass is element by element.
+//
+// KS (vtm_cfg_ddim_update_f16) is KI's sampling sibling: it takes a chunk's raw UNet output, forms the classifier-free
+// guidance combine in the same pass (three more fp16 roundings, generate.py:274-279) and writes x_{t-1} (generate.py:
+// 281-311) to `out`, which may be x itself.  No trajectory; the same vectors, head, tail and fallback as KI.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -95,8 +99,108 @@ ddim_update_kernel(__half* __restrict__ x, const __half* __restrict__ eps, long 
   }
 }
 
+// KS: the sampling step's guidance combine and DDIM update, out <- c * ((x - a * e) * r) + d * e with
+//   e = u + g * (c_eps - u)                         generate.py:274-279 (noise_pred_uncond, noise_pred_cond)
+//   a = sigma, r = 1 / mu, c = mu_prev, d = sigma_prev   generate.py:281-311 (inversion=False)
+// u and c_eps are the last two of the `samples` blocks of the UNet output.  The three guidance ops round to fp16 as
+// torch's half sub / mul / add do; g is float(guidance), the opmath value torch takes a python scalar at.
+__device__ __forceinline__ float cfg_ddim_value(float x, float u, float c, float g, const DdimCoef& k) {
+  const float diff = rh(__fsub_rn(c, u));        // cond - uncond
+  const float gd = rh(__fmul_rn(g, diff));       // guidance * (cond - uncond)
+  const float e = rh(__fadd_rn(u, gd));          // uncond + ...
+  return ddim_value(x, e, k);
+}
+
+__device__ __forceinline__ void cfg_ddim_elem(const __half* x, const __half* u, const __half* c, __half* out,
+                                              long long i, float g, const DdimCoef& k) {
+  out[i] = __float2half_rn(cfg_ddim_value(__half2float(x[i]), __half2float(u[i]), __half2float(c[i]), g, k));
+}
+
+// x and out may be the same buffer (every element is read by the thread that writes it), so neither is __restrict__
+// and x is not read through the non-coherent path.
+__global__ void __launch_bounds__(DDIM_THREADS)
+cfg_ddim_update_kernel(const __half* x, const __half* __restrict__ u, const __half* __restrict__ c, long long n,
+                       float g, const float* __restrict__ coef, const int32_t* __restrict__ step_dev, int32_t n_steps,
+                       __half* out) {
+  const int step = *step_dev;
+  if (step < 0 || step >= n_steps) return;
+  const float4 raw = reinterpret_cast<const float4*>(coef)[step];
+  const DdimCoef k{raw.x, raw.y, raw.z, raw.w};
+
+  const long long tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long nthreads = static_cast<long long>(gridDim.x) * blockDim.x;
+  // elements before out's first 16-byte boundary (pointers are 2-byte aligned)
+  long long head = ((16 - (reinterpret_cast<uintptr_t>(out) & 15)) & 15) >> 1;
+  if (head > n) head = n;
+  const uintptr_t others = reinterpret_cast<uintptr_t>(x + head) | reinterpret_cast<uintptr_t>(u + head) |
+                           reinterpret_cast<uintptr_t>(c + head);
+  if ((others & 15) != 0) {
+    for (long long i = tid; i < n; i += nthreads) cfg_ddim_elem(x, u, c, out, i, g, k);
+    return;
+  }
+  const long long nv = (n - head) >> 3;
+  const long long tail0 = head + (nv << 3);
+  if (tid < head) cfg_ddim_elem(x, u, c, out, tid, g, k);
+  if (tid < n - tail0) cfg_ddim_elem(x, u, c, out, tail0 + tid, g, k);
+  const uint4* xv = reinterpret_cast<const uint4*>(x + head);
+  const __half* uv = u + head;
+  const __half* cv = c + head;
+  uint4* ov = reinterpret_cast<uint4*>(out + head);
+  for (long long v = tid; v < nv; v += nthreads) {
+    uint4 a = xv[v];
+    const uint4 p = ld_nc_16(uv + (v << 3));
+    const uint4 q = ld_nc_16(cv + (v << 3));
+    __half2* a2 = reinterpret_cast<__half2*>(&a);
+    const __half2* p2 = reinterpret_cast<const __half2*>(&p);
+    const __half2* q2 = reinterpret_cast<const __half2*>(&q);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 xf = __half22float2(a2[e]), uf = __half22float2(p2[e]), cf = __half22float2(q2[e]);
+      a2[e] = __floats2half2_rn(cfg_ddim_value(xf.x, uf.x, cf.x, g, k), cfg_ddim_value(xf.y, uf.y, cf.y, g, k));
+    }
+    ov[v] = a;
+  }
+}
+
+bool overlaps(const void* a, long long a_bytes, const void* b, long long b_bytes) {
+  const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
+  return pa < pb + static_cast<uintptr_t>(b_bytes) && pb < pa + static_cast<uintptr_t>(a_bytes);
+}
+
+unsigned ddim_blocks(long long n, int sms) {
+  long long blocks = (n + 8LL * DDIM_THREADS - 1) / (8LL * DDIM_THREADS);
+  const long long cap = static_cast<long long>(sms) * (2048 / DDIM_THREADS);
+  if (blocks > cap) blocks = cap;
+  if (blocks < 1) blocks = 1;
+  return static_cast<unsigned>(blocks);
+}
+
 }  // namespace
 }  // namespace vtm
+
+extern "C" int vtm_cfg_ddim_update_f16(const void* x_dev, const void* eps_dev, int64_t n, int32_t samples,
+                                       float guidance, const float* coef_dev, const int32_t* step_dev, int32_t n_steps,
+                                       void* out_dev, void* stream_) {
+  using namespace vtm;
+  if (!x_dev || !eps_dev || !coef_dev || !step_dev || !out_dev) return VTM_E_NULL;
+  if (n <= 0 || n_steps <= 0 || (samples != 2 && samples != 3) || n > INT64_MAX / 2 / samples) return VTM_E_SHAPE;
+  if (((reinterpret_cast<uintptr_t>(x_dev) | reinterpret_cast<uintptr_t>(eps_dev) |
+        reinterpret_cast<uintptr_t>(out_dev)) & 1) != 0)
+    return VTM_E_SHAPE;                                             // fp16 tensors are 2-byte aligned
+  if ((reinterpret_cast<uintptr_t>(coef_dev) & 15) != 0 || (reinterpret_cast<uintptr_t>(step_dev) & 3) != 0)
+    return VTM_E_SHAPE;                                             // the table is read as one float4 per step
+  const long long bytes = 2LL * n;
+  if ((out_dev != x_dev && overlaps(out_dev, bytes, x_dev, bytes)) || overlaps(out_dev, bytes, eps_dev, samples * bytes))
+    return VTM_E_SHAPE;                                             // out is x itself or apart from x and eps
+  int sms = 0;
+  int rc = cached_sm_count(&sms);
+  if (rc) return rc;
+  const __half* eps = static_cast<const __half*>(eps_dev);
+  cfg_ddim_update_kernel<<<ddim_blocks(n, sms), DDIM_THREADS, 0, static_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const __half*>(x_dev), eps + (samples - 2) * n, eps + (samples - 1) * n, n, guidance, coef_dev,
+      step_dev, n_steps, static_cast<__half*>(out_dev));
+  return launch_rc();
+}
 
 extern "C" int vtm_ddim_update_f16(void* x_dev, const void* eps_dev, int64_t n, const float* coef_dev,
                                    const int32_t* slot_dev, const int32_t* step_dev, int32_t n_steps, void* traj_dev,

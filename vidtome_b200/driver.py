@@ -26,6 +26,13 @@ import torch
 
 from . import patch, pnp
 
+# On CUDA fp16 latents (shard=False), every chunk of a ChunkedDenoiser step ends with KS (ops.cfg_ddim_update): the
+# guidance combine and the DDIM update of the chunk's rows in one kernel, its coefficients read from a device table at a
+# device step index, so that a captured step includes the update.  Bit-identical to pred_noise's combine followed by
+# pred_next_x.  Off: the step takes those torch ops.  Read at every eager step and at capture; a graph replays the path
+# it was captured with.
+FUSE_STEP_UPDATE = True
+
 
 def ddim_alphas_cumprod(num_train_timesteps: int = 1000, beta_start: float = 0.00085,
                         beta_end: float = 0.012) -> torch.Tensor:
@@ -106,10 +113,11 @@ class ChunkedDenoiser:
                  pnp_conv_modules: Optional[Iterable[torch.nn.Module]] = None, depth: Optional[torch.Tensor] = None):
         """`cuda_graph=True`: after `graph_warmup` eager steps, the noise prediction of a whole step (every chunk:
         CFG batch, UNet forward with the merge path, guidance combine) is captured once into a CUDA graph and
-        replayed; per step the host then issues one graph launch plus the DDIM update instead of ~250 kernel
-        launches.  The frame draws of the local matcher stay on the device (utils.draw_randf) and come from the
-        blocks' generators, which are registered with the graph, so replays produce the same sequence of draws —
-        and bit-identical latents — as eager stepping.  Needs static shapes: `randomize_chunks=False`, frame counts
+        replayed; per step the host then issues one graph launch instead of ~250 kernel launches.  On CUDA fp16
+        latents the DDIM update is inside the graph too (FUSE_STEP_UPDATE: KS ends every chunk); otherwise it follows
+        the replay in torch ops.  The frame draws of the local matcher stay on the device (utils.draw_randf) and come
+        from the blocks' generators, which are registered with the graph, so replays produce the same sequence of
+        draws — and bit-identical latents — as eager stepping.  Needs static shapes: `randomize_chunks=False`, frame counts
         divisible by the target stride, and local merging only (`merge_global=False`) unless `capture_global=True`.
 
         `capture_global=True` (with `merge_global=True, cuda_graph=True`) captures global merging too.  The graph runs
@@ -187,8 +195,8 @@ class ChunkedDenoiser:
         self.shard = bool(shard)
         self.cuda_graph = bool(cuda_graph)
         self.graph_warmup = int(graph_warmup)
-        self._graph = None          # (CUDAGraph, static x, static timestep, static noise, key[, slot index state],
-                                    #  static per-frame inputs)
+        self._graph = None          # (CUDAGraph, static x, static timestep, static noise or x_{t-1}, key[, slot
+                                    #  index state], static per-frame inputs, fused update)
         self._eager_steps = 0
         self.capture_global = bool(capture_global)
         self.chunk_graphs = bool(chunk_graphs)
@@ -205,11 +213,12 @@ class ChunkedDenoiser:
             raise ValueError("cuda_graph=True needs merge_global=False and randomize_chunks=False (static work)")
         if self.capture_global and self.shard:
             raise ValueError("capture_global=True does not capture the cross-rank exchange of shard=True")
-        # (chunk length, first in step, frame shape, PnP injection[, PnP conv injection when pnp_f_t is set])
-        #   -> (CUDAGraph, static x, static noise, static per-frame inputs {"src" | "ctrl" | "depth": tensor})
+        # (chunk length, first in step, frame shape, PnP injection[, PnP conv injection when pnp_f_t is set], fused
+        #   update) -> (CUDAGraph, static x, static noise or x_{t-1}, static per-frame inputs {"src" | "ctrl" | "depth"})
         self._chunk_graphs = {}
         self._chunk_t = None        # the UNet's timestep input shared by the chunk graphs
         self._stores = []           # patch.GlobalTokenStore of every block (chunk_graphs with merge_global)
+        self._tables = {}           # device -> (KS's coefficient table, its step index), made on first use
         self.chunk_size = chunk_size
         self.guidance_scale = guidance_scale
         self.merge_global = merge_global
@@ -302,6 +311,19 @@ class ChunkedDenoiser:
                    ctrl: Optional[torch.Tensor] = None, depth: Optional[torch.Tensor] = None) -> torch.Tensor:
         """`src`: the source latents of the chunk (PnP), prepended to the batch.  `ctrl`: the control images of the
         chunk (ControlNet).  `depth`: the depth maps of the chunk (SD2-depth), appended to every sample as a channel."""
+        return self.guide(*self.unet_output(x, t, src, ctrl, depth))
+
+    # generate.py:274-279
+    def guide(self, eps: torch.Tensor, batch_size: int) -> torch.Tensor:
+        """Classifier-free guidance on the raw UNet output of `batch_size` samples."""
+        noise_pred_uncond, noise_pred_cond = eps.chunk(batch_size)[-2:]
+        return noise_pred_uncond + self.guidance_scale * (noise_pred_cond - noise_pred_uncond)
+
+    # generate.py:238-273
+    def unet_output(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None,
+                    ctrl: Optional[torch.Tensor] = None, depth: Optional[torch.Tensor] = None):
+        """The raw UNet output of the chunk's batch ([source |] uncond | cond, each len(x) frames) and its number of
+        samples, before the guidance combine of pred_noise."""
         flen = len(x)
         text = None if self.cond is None else self.cond.repeat_interleave(flen, dim=0)
         latent_model_input = torch.cat([x, x])                                # classifier-free guidance
@@ -320,8 +342,7 @@ class ChunkedDenoiser:
             mid *= self.control_scale
             kwargs = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
         eps = self.unet(latent_model_input, t, encoder_hidden_states=text, **kwargs).sample
-        noise_pred_uncond, noise_pred_cond = eps.chunk(batch_size)[-2:]
-        return noise_pred_uncond + self.guidance_scale * (noise_pred_cond - noise_pred_uncond)
+        return eps, batch_size
 
     # generate.py:281-311 (inversion=False branch)
     def pred_next_x(self, x: torch.Tensor, eps: torch.Tensor, i: int) -> torch.Tensor:
@@ -333,6 +354,54 @@ class ChunkedDenoiser:
         mu_prev, sigma_prev = float(alpha_prod_t_prev ** 0.5), float((1 - alpha_prod_t_prev) ** 0.5)
         pred_x0 = (x - sigma * eps) / mu
         return mu_prev * pred_x0 + sigma_prev * eps
+
+    def coefficients(self, i: int):
+        """(a, b, c, d) of step i for x <- c * ((x - a * eps) / b) + d * eps: (sigma, mu, mu_prev, sigma_prev), the
+        floats pred_next_x takes (generate.py:281-311, inversion=False)."""
+        t = self.timesteps[i]
+        alpha_prod_t = self.alphas_cumprod[t]
+        alpha_prod_t_prev = (self.alphas_cumprod[self.timesteps[i + 1]] if i < len(self.timesteps) - 1
+                             else self.final_alpha_cumprod)
+        mu, sigma = float(alpha_prod_t ** 0.5), float((1 - alpha_prod_t) ** 0.5)
+        mu_prev, sigma_prev = float(alpha_prod_t_prev ** 0.5), float((1 - alpha_prod_t_prev) ** 0.5)
+        return sigma, mu, mu_prev, sigma_prev
+
+    def step_tables(self, device: torch.device):
+        """KS's coefficient table ([n_steps, 4] fp32, ops.ddim_table of `coefficients`) and its step index (one int32,
+        which every step sets) on `device`, made once: captured graphs hold their addresses."""
+        device = torch.device(device)
+        if device not in self._tables:
+            from . import ops
+            coef = ops.ddim_table(self.coefficients(i) for i in range(len(self.timesteps))).to(device)
+            self._tables[device] = (coef, torch.zeros(1, dtype=torch.int32, device=device))
+        return self._tables[device]
+
+    def _fuses_update(self, x: torch.Tensor) -> bool:
+        """Whether a step on `x` that starts (or is captured) now ends each chunk with KS."""
+        return (FUSE_STEP_UPDATE and not self.shard and x.is_cuda and x.dtype == torch.float16
+                and x.is_contiguous())
+
+    def _next_x_rows(self, x: torch.Tensor, t, frames: dict, out: torch.Tensor):
+        """x_{t-1} of one chunk (`x`, with its rows of the per-frame inputs) into `out`, by KS at the step index that
+        step() set.  UNet output of another dtype gets pred_noise's guidance combine in torch, rounded to the
+        latents' dtype as the torch path stores it, and KI's update of the same step."""
+        from . import ops
+        coef, step = self.step_tables(x.device)
+        eps, samples = self.unet_output(x, t, **frames)
+        if eps.dtype == torch.float16:
+            ops.cfg_ddim_update(x, eps.contiguous(), samples, self.guidance_scale, coef, step, out)
+            return
+        noise = self.guide(eps, samples).to(x.dtype)
+        out.copy_(x)
+        ops.ddim_update(out, noise.contiguous(), coef, step)
+
+    def _all_next_x(self, x: torch.Tensor, t, frames: dict, out: torch.Tensor) -> torch.Tensor:
+        """The step's x_{t-1} of every frame into `out`, chunk by chunk (the fused form of _all_noises + pred_next_x;
+        shard=False, so the chunks cover every frame)."""
+        for chunk in self.get_chunks(len(x)):
+            lo, hi = int(chunk[0]), int(chunk[-1]) + 1
+            self._next_x_rows(x[lo:hi], t, _rows(frames, lo, hi), out[lo:hi])
+        return out
 
     def _step_chunks(self, flen: int) -> List[torch.Tensor]:
         chunks = self.get_chunks(flen)
@@ -378,20 +447,23 @@ class ChunkedDenoiser:
         return tuple(x.shape), self.injecting(t), self.conv_injecting(t)
 
     def _capture(self, x: torch.Tensor, t: int, frames: dict):
-        """Capture `_all_noises` for inputs shaped like `x` (called after the eager warm-up steps, so that every
+        """Capture the step for inputs shaped like `x`: `_all_next_x` (every chunk's x_{t-1}) when the update is fused
+        (_fuses_update), else `_all_noises` (called after the eager warm-up steps, so that every
         lazily created piece of state — generators forked by the hook, cached packed weights, the library handle,
         allocator pools — already exists)."""
         self._graph = None                                                   # release the previous graph first
         gx = x.clone()
         gframes = {k: v.clone() for k, v in frames.items()}                # the per-frame inputs, set per replay
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)      # the UNet's timestep input, set per replay
+        fused = self._fuses_update(x)
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = self._all_noises(gx, gt, gframes)
-        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gframes)
+            # gn: the step's x_{t-1} with the fused update, else its noise prediction
+            gn = self._all_next_x(gx, gt, gframes, torch.empty_like(gx)) if fused else self._all_noises(gx, gt, gframes)
+        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gframes, fused)
 
     @staticmethod
     def slot_index(chunks: List[torch.Tensor], flen: int) -> torch.Tensor:
@@ -424,18 +496,25 @@ class ChunkedDenoiser:
             graph.register_generator_state(g)
         for model in self._models():                                        # slot 0 starts the recurrence afresh
             patch.update_patch(model, global_tokens=None)
+        fused = self._fuses_update(x)
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = torch.zeros_like(gx)
+            # gn, in slot order: the step's x_{t-1} with the fused update, else its noise prediction
+            gn = torch.empty_like(gx) if fused else torch.zeros_like(gx)
             for k in range(flen // cs):
                 lo, hi = k * cs, (k + 1) * cs
-                gn[lo:hi] = self.pred_noise(gx[lo:hi], gt, **_rows(gframes, lo, hi))
+                if fused:
+                    self._next_x_rows(gx[lo:hi], gt, _rows(gframes, lo, hi), gn[lo:hi])
+                else:
+                    gn[lo:hi] = self.pred_noise(gx[lo:hi], gt, **_rows(gframes, lo, hi))
         idx_dev = torch.empty((2, flen), dtype=torch.int64, device=x.device)
         idx_host = torch.empty((2, flen), dtype=torch.int64).pin_memory()
         copied = torch.cuda.Event()          # the pinned buffer is rewritten only after its last upload has run
-        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), idx_dev, idx_host, copied, gframes)
+        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), idx_dev, idx_host, copied, gframes, fused)
 
-    def _slot_noises(self, x: torch.Tensor, t: int, frames: dict) -> torch.Tensor:
+    def _slot_noises(self, x: torch.Tensor, t: int, frames: dict):
+        """Replay the slot graph of the step; returns (its output in frame order, whether it is x_{t-1} rather than
+        the noise prediction)."""
         flen = len(x)
         if flen % self.chunk_size != 0:
             raise RuntimeError(f"capture_global=True needs a frame count divisible by chunk_size (got {flen} frames, "
@@ -443,7 +522,7 @@ class ChunkedDenoiser:
         order = self.slot_index(self.get_chunks(flen), flen)        # the same host draws as eager stepping
         if self._graph is None or self._graph[4] != self._graph_key(x, t):
             self._capture_slots(x, t, frames)
-        graph, gx, gt, gn, _, idx_dev, idx_host, copied, gframes = self._graph
+        graph, gx, gt, gn, _, idx_dev, idx_host, copied, gframes, fused = self._graph
         copied.synchronize()
         idx_host.copy_(order)
         idx_dev.copy_(idx_host, non_blocking=True)
@@ -453,7 +532,7 @@ class ChunkedDenoiser:
             torch.index_select(frames[k], 0, idx_dev[0], out=g)
         gt.fill_(int(t))
         graph.replay()
-        return torch.index_select(gn, 0, idx_dev[1])                # slots -> frames
+        return torch.index_select(gn, 0, idx_dev[1]), fused         # slots -> frames
 
     @staticmethod
     def draw_dependent_lengths(chunk_size: int, target_stride: int) -> List[int]:
@@ -517,8 +596,9 @@ class ChunkedDenoiser:
                 patch.update_patch(model, global_tokens=None)
 
     def _capture_chunk(self, key, x: torch.Tensor, frames: dict):
-        """Capture the noise prediction of one chunk shaped like `x` (with the chunk's rows of the per-frame inputs);
-        `key[1]` says whether it is the first chunk of a step, i.e. whether the blocks' stores are empty when it runs."""
+        """Capture the noise prediction of one chunk shaped like `x` (with the chunk's rows of the per-frame inputs), or
+        with `key[-1]` (the fused update) its x_{t-1}; `key[1]` says whether it is the first chunk of a step, i.e.
+        whether the blocks' stores are empty when it runs."""
         gx = x.clone()
         gframes = {k: v.clone() for k, v in frames.items()}
         graph = torch.cuda.CUDAGraph()
@@ -526,13 +606,21 @@ class ChunkedDenoiser:
             graph.register_generator_state(g)
         for st in self._stores:
             st.filled = not key[1]
+        fused = key[-1]
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph):
-            gn = self.pred_noise(gx, self._chunk_t, **gframes)
+            # gn: the chunk's x_{t-1} with the fused update, else its noise prediction
+            if fused:
+                gn = torch.empty_like(gx)
+                self._next_x_rows(gx, self._chunk_t, gframes, gn)
+            else:
+                gn = self.pred_noise(gx, self._chunk_t, **gframes)
         self._chunk_graphs[key] = (graph, gx, gn, gframes)
         return self._chunk_graphs[key]
 
-    def _chunk_graph_noises(self, x: torch.Tensor, t: int, frames: dict) -> torch.Tensor:
+    def _chunk_graph_step(self, x: torch.Tensor, t: int, i: int, frames: dict) -> torch.Tensor:
+        """Replay every chunk's graph; returns the step's x_{t-1}.  The graphs are keyed by whether the step fuses the
+        update (_fuses_update): those captured without it give the noise prediction, which pred_next_x then takes."""
         flen = len(x)
         chunks = self.get_chunks(flen)                                      # the same host draws as eager stepping
         if not self._chunk_graphs:
@@ -548,12 +636,14 @@ class ChunkedDenoiser:
         if self._chunk_t is None:
             self._chunk_t = torch.tensor(int(t), device=x.device, dtype=torch.long)
         self._chunk_t.fill_(int(t))
-        noises = torch.empty_like(x)
+        fused = self._fuses_update(x)
+        out = torch.empty_like(x)                       # x_{t-1} with the fused update, else the noise prediction
         for k, chunk in enumerate(chunks):
             lo, hi = int(chunk[0]), int(chunk[-1]) + 1
             key = (hi - lo, self.merge_global and k == 0, tuple(x.shape[1:]), inject)
             if self.pnp_f_t is not None:
                 key = key + (conv,)
+            key = key + (fused,)
             entry = self._chunk_graphs.get(key)
             if entry is None:
                 entry = self._capture_chunk(key, x[lo:hi], _rows(frames, lo, hi))
@@ -562,8 +652,8 @@ class ChunkedDenoiser:
             for name, g in gframes.items():
                 g.copy_(frames[name][lo:hi])
             graph.replay()
-            noises[lo:hi].copy_(gn)
-        return noises
+            out[lo:hi].copy_(gn)
+        return out if fused else self.pred_next_x(x, out, i)
 
     # one iteration of generate.py:211-224
     @torch.no_grad()
@@ -584,24 +674,29 @@ class ChunkedDenoiser:
             frames["depth"] = self.depth.to(x)                              # prepare_data's .to(self.init_noise)
         if self.chunk_graphs and self.merge_global and x.is_cuda and not self._stores:
             self._install_stores()
+        if self._fuses_update(x) or x.device in self._tables:             # KS's step index, read on the device
+            self.step_tables(x.device)[1].fill_(i)
         if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.chunk_graphs:
-            noises = self._chunk_graph_noises(x, t, frames)
+            x = self._chunk_graph_step(x, t, i, frames)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.capture_global:
-            noises = self._slot_noises(x, t, frames)
+            out, fused = self._slot_noises(x, t, frames)
+            x = out if fused else self.pred_next_x(x, out, i)
         elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup:
             if self._graph is None or self._graph[4] != self._graph_key(x, t):
                 self._capture(x, t, frames)
-            graph, gx, gt, gn, _, gframes = self._graph
+            graph, gx, gt, gn, _, gframes, fused = self._graph
             gx.copy_(x, non_blocking=True)
             for k, g in gframes.items():
                 g.copy_(frames[k], non_blocking=True)
             gt.fill_(int(t))
             graph.replay()
-            noises = gn
+            x = gn.clone() if fused else self.pred_next_x(x, gn, i)     # the next replay rewrites gn
         else:
             self._eager_steps += 1
-            noises = self._all_noises(x, t, frames)
-        x = self.pred_next_x(x, noises, i)
+            if self._fuses_update(x):
+                x = self._all_next_x(x, t, frames, torch.empty_like(x))
+            else:
+                x = self.pred_next_x(x, self._all_noises(x, t, frames), i)
         if self.merge_global:
             self._reset_global()
         return x

@@ -538,6 +538,36 @@ def ddim_update(x: torch.Tensor, eps: torch.Tensor, coef: torch.Tensor, step: to
     return x
 
 
+def cfg_ddim_update(x: torch.Tensor, eps: torch.Tensor, samples: int, guidance: float, coef: torch.Tensor,
+                    step: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """KS: the sampling step of one chunk from its raw UNet output.  With u, c = eps.chunk(samples)[-2:],
+    e = u + guidance * (c - u) and (a, r, k, d) = coef[step[0]] (a = sigma, r = 1 / mu, k = mu_prev, d = sigma_prev):
+    out <- k * ((x - a * e) * r) + d * e, bit for bit as torch's half ops on python floats compute
+    `pred_next_x(x, pred_noise(...))`.  x, out fp16 of one shape (out may be x itself, else apart from x and eps);
+    eps fp16 [samples * x.shape[0], *x.shape[1:]] with samples 2 or 3; coef [n_steps, 4] fp32 (ddim_table); step a
+    1-element int32 tensor read on the device.  A step outside [0, n_steps) leaves out as it was."""
+    _require(x, torch.float16, "x")
+    _require(eps, torch.float16, "eps")
+    _require(out, torch.float16, "out")
+    _require(coef, torch.float32, "coef")
+    _require(step, torch.int32, "step")
+    if x.dim() < 1 or eps.shape[1:] != x.shape[1:] or eps.shape[0] != samples * x.shape[0]:
+        raise RuntimeError(f"cfg_ddim_update: eps {tuple(eps.shape)} must be {samples} samples shaped like x "
+                           f"{tuple(x.shape)}")
+    if out.shape != x.shape:
+        raise RuntimeError(f"cfg_ddim_update: out {tuple(out.shape)} must be shaped like x {tuple(x.shape)}")
+    if coef.dim() != 2 or coef.shape[1] != 4 or step.numel() != 1:
+        raise RuntimeError("cfg_ddim_update: coef must be [n_steps, 4] and step a 1-element tensor")
+    n = x.numel()
+    with _Timed("KS", 11.0 * n, 2.0 * n * 4):                      # x, u, c read; out written
+        check(_lib.load().vtm_cfg_ddim_update_f16(x.data_ptr(), eps.data_ptr(), n, int(samples), float(guidance),
+                                                  coef.data_ptr(), step.data_ptr(), coef.shape[0], out.data_ptr(),
+                                                  _stream()),
+              "vtm_cfg_ddim_update_f16")
+    STATS.launches += 1
+    return out
+
+
 def cross_attention(x: torch.Tensor, ctx: torch.Tensor, w_q: torch.Tensor, w_kv: torch.Tensor, w_o: torch.Tensor,
                     b_o: Optional[torch.Tensor], heads: int, scale: float, resid: Optional[torch.Tensor] = None,
                     lora_q=None, lora_kv=None, lora_o=None) -> torch.Tensor:
