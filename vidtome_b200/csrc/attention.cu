@@ -223,10 +223,14 @@ constexpr bool fa_moves_registers(int KS) { return KS >= 9; }
 // maxima, l_r the rescaled row sums with this tile's P added, alpha the factor O must be rescaled by before P V of this
 // tile is added to it.  MASK (the last tile only) sets keys at or past `kvalid` to -inf.  The roundings are spelled
 // out: scale as a separate multiply, then ex2 of a subtraction, and l = fma(l, alpha, p0 + p1) for the first pair.
+// A row whose scores so far are all -inf (every key of its first tiles -inf, e.g. a K channel that overflowed to +inf
+// against a negative query component) keeps m_r = -inf: it subtracts 0 instead, as FlashAttention-2 does, so those
+// keys get p = 0 and alpha = 0 rather than ex2(-inf - -inf) = NaN.  Finite rows subtract their maximum unchanged.
+// A row whose every key scores -inf ends with l = 0 and O = 0 (see the store).
 template <bool MASK>
 __device__ __forceinline__ void fa_softmax(float (&s)[32], float (&m_r)[2], float (&l_r)[2], float (&alpha)[2],
                                            float scale_log2, int kvalid, int lane) {
-  float mx[2] = {-INFINITY, -INFINITY};
+  float mx[2] = {-INFINITY, -INFINITY}, m_safe[2];
 #pragma unroll
   for (int n = 0; n < 8; ++n) {
 #pragma unroll
@@ -244,14 +248,16 @@ __device__ __forceinline__ void fa_softmax(float (&s)[32], float (&m_r)[2], floa
   for (int r = 0; r < 2; ++r) {
     mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
     mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-    const float m_new = fmaxf(m_r[r], mx[r]);   // finite: every tile holds at least one valid key
-    alpha[r] = ex2_approx(__fsub_rn(m_r[r], m_new));
+    const float m_new = fmaxf(m_r[r], mx[r]);   // -inf while every score of the row so far is -inf
+    const float m_sub = m_new == -INFINITY ? 0.f : m_new;
+    alpha[r] = ex2_approx(__fsub_rn(m_r[r], m_sub));
     m_r[r] = m_new;
+    m_safe[r] = m_sub;
   }
 #pragma unroll
   for (int n = 0; n < 8; ++n) {
-    const float p0 = ex2_approx(__fsub_rn(s[4 * n], m_r[0])), p1 = ex2_approx(__fsub_rn(s[4 * n + 1], m_r[0]));
-    const float p2 = ex2_approx(__fsub_rn(s[4 * n + 2], m_r[1])), p3 = ex2_approx(__fsub_rn(s[4 * n + 3], m_r[1]));
+    const float p0 = ex2_approx(__fsub_rn(s[4 * n], m_safe[0])), p1 = ex2_approx(__fsub_rn(s[4 * n + 1], m_safe[0]));
+    const float p2 = ex2_approx(__fsub_rn(s[4 * n + 2], m_safe[1])), p3 = ex2_approx(__fsub_rn(s[4 * n + 3], m_safe[1]));
     if (n == 0) {
       l_r[0] = __fmaf_rn(l_r[0], alpha[0], __fadd_rn(p0, p1));
       l_r[1] = __fmaf_rn(l_r[1], alpha[1], __fadd_rn(p2, p3));
@@ -470,7 +476,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constan
     float l = l_r[r];
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
-    const float inv = 1.f / l;
+    // l = 0 only when every key of the row scored -inf: O = 0 then, as torch's attention and FlashAttention-2 return
+    // (IEEE's 0 / 0 would be NaN); a NaN l still gives NaN
+    const float inv = l == 0.f ? 1.f : 1.f / l;
     const int row = q0 + cg * 64 + wq * 16 + (lane >> 2) + 8 * r;
     if (row >= q_valid) continue;
 #pragma unroll

@@ -203,8 +203,10 @@ struct NchwEpi {
 // (its leading coefficient is negative and it is monotonic up to 65504, with no fp32 overflow), so |g| h < 2^-26 and
 // g h rounds to -0 in fp16 as gelu does, and ex2 flushes h to 0 once p < -126.  Holding h at its value at a clamp instead
 // would let g h grow with |g|.  Then gelu(g) = g (1 - h) for g >= 0 and g h for g < 0: over every finite fp16 gate the
-// fp16 result is within one ulp of the correctly rounded gelu, and zero wherever that is (+0 at g = -0).  Two values at
-// a time, their Horner steps interleaved.
+// fp16 result is within one ulp of the correctly rounded gelu, and zero wherever that is (+0 at g = -0).  At g = +inf
+// p = -inf and h = 0, so g h = inf 0 = NaN: wherever h is 0 the positive branch returns g itself (the same bits for
+// every finite g, since g - g 0 = g), which makes gelu(+inf) = +inf as torch's erf form gives; gelu(-inf) = -inf 0 and
+// gelu(NaN) stay NaN, as there.  Two values at a time, their Horner steps interleaved.
 __device__ __forceinline__ void gelu_x2(float g0, float g1, float& y0, float& y1) {
   const float t0 = fabsf(g0), t1 = fabsf(g1);
   const float lead = -1.79155074e-06f;
@@ -222,8 +224,8 @@ __device__ __forceinline__ void gelu_x2(float g0, float g1, float& y0, float& y1
   horner(-1.f);                                   // p(t) - 1
   const float h0 = ex2_approx(p0), h1 = ex2_approx(p1);                 // erfc(t / sqrt 2) / 2
   const float gh0 = g0 * h0, gh1 = g1 * h1;
-  y0 = g0 >= 0.f ? g0 - gh0 : gh0;
-  y1 = g1 >= 0.f ? g1 - gh1 : gh1;
+  y0 = g0 >= 0.f ? (h0 == 0.f ? g0 : g0 - gh0) : gh0;
+  y1 = g1 >= 0.f ? (h1 == 0.f ? g1 : g1 - gh1) : gh1;
 }
 
 struct GegluEpi {
