@@ -14,21 +14,28 @@ tests).  Two cases:
   north-star variant, a semantic variant of the recurrence (it reproduces one step of it with "previous chunk's
   local tokens" in place of the running set); parity is defined against the reference's own `_2s` matcher fed
   the same global tokens (the attribute is public, patch.py:60).
+
+DDIM inversion and reconstruction (driver.ChunkedInverter(shard=True)) shard the frame batches (`shard_batches`):
+nothing crosses GPUs during the steps, and one all-gather at the end (`gather_batches`) gives every rank all frames.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
 
 
+def initialized() -> bool:
+    return dist.is_available() and dist.is_initialized()
+
+
 def world() -> int:
-    return dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+    return dist.get_world_size() if initialized() else 1
 
 
 def rank() -> int:
-    return dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
+    return dist.get_rank() if initialized() else 0
 
 
 def shard_chunks(chunks: Sequence, rank_: Optional[int] = None, world_: Optional[int] = None) -> List:
@@ -42,6 +49,41 @@ def shard_chunks(chunks: Sequence, rank_: Optional[int] = None, world_: Optional
     r = rank() if rank_ is None else rank_
     w = world() if world_ is None else world_
     return [c for i, c in enumerate(chunks) if i % w == r]
+
+
+def shard_batches(flen: int, batch_size: int, rank_: Optional[int] = None,
+                  world_: Optional[int] = None) -> List[Tuple[int, int]]:
+    """The frame ranges [lo, hi) of the inversion batches this rank runs: the batches of `batch_size` frames of the
+    unsharded run (the last one may be ragged, invert.py:124-129), batch k -> rank k % world.  Batch shapes do not
+    change, so every frame is computed exactly as without sharding.  A rank may get no batch (world > batch count)."""
+    r = rank() if rank_ is None else rank_
+    w = world() if world_ is None else world_
+    return [(lo, min(lo + batch_size, flen)) for k, lo in enumerate(range(0, flen, batch_size)) if k % w == r]
+
+
+def gather_batches(local: torch.Tensor, flen: int, batch_size: int, frame_dim: int = 0, group=None) -> torch.Tensor:
+    """Assemble every rank's `local` frames (its shard_batches, concatenated in order along `frame_dim`) into the
+    full [.., flen, ..] tensor, in frame order, on every rank: one all-gather of equal-size slabs, each padded to
+    ceil(n_batches / world) batches, then each rank's batches put back at their frame ranges.  Without sharding
+    (world 1) `local` is returned as it is."""
+    w = world()
+    if w == 1:
+        return local
+    n_batches = -(-flen // batch_size)
+    slab = -(-n_batches // w) * batch_size
+    shape = list(local.shape)
+    shape[frame_dim] = slab
+    padded = local.new_zeros(shape)
+    padded.narrow(frame_dim, 0, local.shape[frame_dim]).copy_(local)
+    out = torch.empty((w * shape[0],) + tuple(shape[1:]), dtype=local.dtype, device=local.device)
+    dist.all_gather_into_tensor(out, padded, group=group)                 # rank-major concatenation
+    out = out.view([w] + shape)
+    shape[frame_dim] = flen
+    full = local.new_empty(shape)
+    for r in range(w):
+        for j, (lo, hi) in enumerate(shard_batches(flen, batch_size, r, w)):
+            full.narrow(frame_dim, lo, hi - lo).copy_(out[r].narrow(frame_dim, j * batch_size, hi - lo))
+    return full
 
 
 def check_step_lockstep(local_chunk_lens: Sequence[int], group=None) -> bool:

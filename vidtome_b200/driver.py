@@ -12,8 +12,9 @@ Restates, on synthetic latents, the parts of the reference's Generator that sit 
   SD2-depth       generate.py:131-132,255-262 (each frame's depth map appended to the UNet input, with `depth`)
 and, in ChunkedInverter, the reference's Inverter around its hot path:
   ddim_inversion  invert.py:117-140     (reversed timesteps, frame batches, the kept latents)
+  ddim_sample     invert.py:142-157     (`recon`: the inverted latents sampled back, reconstruct())
   pred_noise      invert.py:159-179     (UNet forward, optional depth channel, optional ControlNet residuals)
-  pred_next_x     invert.py:182-211     (inversion=True branch)
+  pred_next_x     invert.py:182-211     (inversion=True and, for reconstruct(), inversion=False)
 Text conditioning, VAE, ControlNet and depth preprocessing and file IO are outside the hot path and not restated.
 """
 from __future__ import annotations
@@ -747,13 +748,26 @@ class ChunkedInverter:
 
     An unpatched `controlnet` runs its modules' own forwards; with patch.FUSE_CONTROLNET_BLOCKS on, the first invert()
     serves it (patch.serve_unmerged), so that its blocks and Transformer2DModel wrappers run in the library, unmerged,
-    as a patched model's do here.  close() gives it its own classes back."""
+    as a patched model's do here.  close() gives it its own classes back.
+
+    reconstruct() samples the inverted latents back to clean latents (the reference's `recon`, invert.py:142-157): the
+    same batches and per-frame inputs over the forward timesteps, with the sampling update, eagerly or from one CUDA
+    graph per step as above.
+
+    `shard=True`: this process is one rank of an initialised torch.distributed job.  No op of the unmerged UNet mixes
+    frames, so every batch is independent of the others for all steps: rank r runs the batches k with k % world == r
+    (dist.shard_batches) on compact local latents, per-frame inputs and cond rows, and captures only those batches.
+    invert() and reconstruct() end with one all-gather (dist.gather_batches, outside any graph) that gives every rank
+    the whole result in frame order.  Batch shapes are those of the unsharded run, so every frame is computed as there:
+    bit-identical to it whenever the UNet computes a batch the same way in every process, as the library does (torch's
+    SDPA, which runs attention above attention.MAX_HEAD_DIM, may differ between processes in the last bits).  A rank
+    without a batch still joins the gather.  Nothing crosses ranks during the steps."""
 
     def __init__(self, unet: torch.nn.Module, n_timesteps: int = 50, batch_size: int = 8,
                  save_steps: Optional[int] = None, save_intermediate: bool = True, cond: Optional[torch.Tensor] = None,
                  controlnet: Optional[torch.nn.Module] = None, control_images: Optional[torch.Tensor] = None,
                  control_scale: float = 1.0, cuda_graph: bool = False, graph_warmup: int = 2,
-                 depth: Optional[torch.Tensor] = None):
+                 depth: Optional[torch.Tensor] = None, shard: bool = False):
         if not isinstance(n_timesteps, int) or n_timesteps <= 0:
             raise ValueError(f"n_timesteps must be a positive int (got {n_timesteps!r})")
         if not isinstance(batch_size, int) or batch_size <= 0:
@@ -771,6 +785,10 @@ class ChunkedInverter:
             raise ValueError(f"cuda_graph=True needs graph_warmup >= 1 (got {graph_warmup!r}): the modules' packed "
                              f"weights are created by an eager step, outside the graph's memory pool")
         _check_depth_arg(depth, controlnet)
+        from . import dist as _dist
+        if shard and not _dist.initialized():
+            raise ValueError("shard=True needs an initialised torch.distributed process group (one rank per process)")
+        self.shard = bool(shard)
         self.depth = depth
         self.unet = unet
         self.batch_size = batch_size
@@ -784,6 +802,7 @@ class ChunkedInverter:
         self.alphas_cumprod = ddim_alphas_cumprod()
         self.final_alpha_cumprod = self.alphas_cumprod[0]     # set_alpha_to_one=False in SD's config
         self.timesteps = ddim_timesteps(n_timesteps)[::-1]    # invert.py:120: reversed(scheduler.timesteps)
+        self.sample_timesteps = ddim_timesteps(n_timesteps)   # invert.py:145: reconstruct() runs forward
         to_save = set(ddim_timesteps(save_steps)) if save_intermediate else set()
         saved = [t for t in self.timesteps if t in to_save]   # invert.py:132
         if self.timesteps[-1] not in saved:                   # invert.py:137-138: the final latents
@@ -829,36 +848,49 @@ class ChunkedInverter:
             kwargs = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
         return self.unet(x, t, encoder_hidden_states=cond, **kwargs).sample
 
-    def _batch_cond(self, lo: int, hi: int, flen: int) -> Optional[torch.Tensor]:
-        if self.cond is None:
-            return None
-        if self.cond.shape[0] == 1:
-            return self.cond.expand(hi - lo, -1, -1)
-        if self.cond.shape[0] != flen:
-            raise ValueError(f"cond has {self.cond.shape[0]} rows for {flen} frames (one per frame, or one for all)")
-        return self.cond[lo:hi]
+    # invert.py:142-157 (ddim_sample) and 182-211 (inversion=False branch)
+    def sample_coefficients(self, i: int):
+        """(a, b, c, d) of reconstruction step i for x <- c * ((x - a * eps) / b) + d * eps: (sigma, mu, mu_prev,
+        sigma_prev) over the forward timesteps `sample_timesteps`, final_alpha_cumprod at the last step; the floats
+        ChunkedDenoiser.coefficients gives for the same schedule."""
+        ts = self.sample_timesteps
+        alpha_prod_t = self.alphas_cumprod[ts[i]]
+        alpha_prod_t_prev = self.alphas_cumprod[ts[i + 1]] if i < len(ts) - 1 else self.final_alpha_cumprod
+        mu, sigma = float(alpha_prod_t ** 0.5), float((1 - alpha_prod_t) ** 0.5)
+        mu_prev, sigma_prev = float(alpha_prod_t_prev ** 0.5), float((1 - alpha_prod_t_prev) ** 0.5)
+        return sigma, mu, mu_prev, sigma_prev
 
-    def _all_noises(self, x: torch.Tensor, t, frames: dict, out: Optional[torch.Tensor] = None):
-        """`frames`: the per-frame inputs besides the latents, {"ctrl" | "depth": [F, ...]} (those in use)."""
+    def sample_next_x(self, x: torch.Tensor, eps: torch.Tensor, i: int) -> torch.Tensor:
+        """Reconstruction step i in torch ops (invert.py:182-211 with inversion=False)."""
+        sigma, mu, mu_prev, sigma_prev = self.sample_coefficients(i)
+        pred_x0 = (x - sigma * eps) / mu
+        return mu_prev * pred_x0 + sigma_prev * eps
+
+    def _check_cond(self, flen: int):
+        if self.cond is not None and self.cond.shape[0] not in (1, flen):
+            raise ValueError(f"cond has {self.cond.shape[0]} rows for {flen} frames (one per frame, or one for all)")
+
+    @staticmethod
+    def _batch_cond(cond: Optional[torch.Tensor], lo: int, hi: int) -> Optional[torch.Tensor]:
+        """Frames lo..hi-1 of `cond`: its rows, or its one row for every frame."""
+        if cond is None:
+            return None
+        return cond.expand(hi - lo, -1, -1) if cond.shape[0] == 1 else cond[lo:hi]
+
+    def _all_noises(self, x: torch.Tensor, t, frames: dict, cond: Optional[torch.Tensor],
+                    out: Optional[torch.Tensor] = None):
+        """`frames`: the per-frame inputs besides the latents, {"ctrl" | "depth": [F, ...]} (those in use), and `cond`
+        the text embeddings ([F | 1, 77, D] or None), both for the frames of `x`."""
         flen = len(x)
         noises = torch.empty_like(x) if out is None else out
         for lo in range(0, flen, self.batch_size):                         # invert.py:124-129
             hi = min(lo + self.batch_size, flen)
-            noises[lo:hi] = self.pred_noise(x[lo:hi], self._batch_cond(lo, hi, flen), t, **_rows(frames, lo, hi))
+            noises[lo:hi] = self.pred_noise(x[lo:hi], self._batch_cond(cond, lo, hi), t, **_rows(frames, lo, hi))
         return noises
 
-    def _device_tables(self, x: torch.Tensor):
-        from . import ops
-        coef = ops.ddim_table(self.coefficients(i) for i in range(len(self.timesteps))).to(x.device)
-        slots = torch.tensor(self.slots, dtype=torch.int32, device=x.device)
-        ts = torch.tensor(self.timesteps, dtype=torch.int64, device=x.device)
-        step = torch.zeros(1, dtype=torch.int32, device=x.device)
-        return coef, slots, ts, step
-
-    @torch.no_grad()
-    def invert(self, x: torch.Tensor) -> torch.Tensor:
-        """Invert the clean latents x [F, 4, h, w] (invert.py:117-140).  Returns the final latents (the last entry of
-        `trajectory`); `x` itself is not modified."""
+    def _inputs(self, x: torch.Tensor):
+        """Check the latents x [F, 4, h, w] against the per-frame inputs; returns this process's frames of x (a copy)
+        and of {"ctrl" | "depth"} and cond (all frames unless shard=True), and whether KI updates them."""
         if x.dim() != 4:
             raise ValueError(f"latents must be [F, 4, h, w] (got {tuple(x.shape)})")
         frames = {}
@@ -870,34 +902,98 @@ class ChunkedInverter:
         if self.depth is not None:
             _check_depth(self.depth, x, self.unet)
             frames["depth"] = self.depth.to(x)
-        if self.cond is not None:
-            self._batch_cond(0, 0, len(x))                                 # check the row count up front
+        self._check_cond(len(x))                                             # the row count, up front
         kernel = x.is_cuda and x.dtype == torch.float16
         if self.cuda_graph and not kernel:
             raise ValueError("cuda_graph=True needs CUDA fp16 latents: the captured step updates them with KI")
-        x = x.clone()
+        if not self.shard:
+            return x.clone(), frames, self.cond, kernel
+        # the rank's whole batches, back to back: the local batches keep the unsharded run's boundaries and shapes
+        from . import dist as _dist
+        idx = [f for lo, hi in _dist.shard_batches(len(x), self.batch_size) for f in range(lo, hi)]
+        idx = torch.tensor(idx, dtype=torch.int64, device=x.device)
+        frames = {k: v.index_select(0, idx) for k, v in frames.items()}
+        cond = self.cond
+        if cond is not None and cond.shape[0] != 1:
+            cond = cond.index_select(0, idx.to(cond.device))
+        return x.index_select(0, idx), frames, cond, kernel
+
+    def _gather(self, local: torch.Tensor, flen: int, frame_dim: int) -> torch.Tensor:
+        if not self.shard:
+            return local
+        from . import dist as _dist
+        return _dist.gather_batches(local, flen, self.batch_size, frame_dim)
+
+    @torch.no_grad()
+    def invert(self, x: torch.Tensor) -> torch.Tensor:
+        """Invert the clean latents x [F, 4, h, w] (invert.py:117-140).  Returns the final latents (the last entry of
+        `trajectory`); `x` itself is not modified.  With shard=True every rank runs its batches
+        (dist.shard_batches) and one all-gather at the end gives every rank the whole trajectory, bit-identical to
+        the unsharded run's (see the class's note on sharding)."""
+        flen = len(x) if x.dim() == 4 else 0
+        x, frames, cond, kernel = self._inputs(x)
         traj = torch.empty((len(self.saved_timesteps),) + tuple(x.shape), dtype=x.dtype, device=x.device)
         scope = patch._unmerged_blocks() if self._patched() else contextlib.nullcontext()
         with scope:
-            if kernel:
-                self._invert_device(x, frames, traj)
+            if len(x) == 0:                                                 # a rank without a batch
+                pass
+            elif kernel:
+                coefficients = [self.coefficients(i) for i in range(len(self.timesteps))]
+                self._run_device(x, frames, cond, coefficients, self.timesteps, self.slots, traj)
             else:
                 with torch.autocast(x.device.type, dtype=torch.float16, enabled=x.is_cuda):
                     for i, t in enumerate(self.timesteps):
-                        x = self.pred_next_x(x, self._all_noises(x, t, frames), i)
+                        x = self.pred_next_x(x, self._all_noises(x, t, frames, cond), i)
                         if self.slots[i] >= 0:
                             traj[self.slots[i]] = x
-        self.trajectory = traj
-        return traj[-1]
+        self.trajectory = self._gather(traj, flen, 1)
+        return self.trajectory[-1]
 
-    def _invert_device(self, x: torch.Tensor, frames: dict, traj: torch.Tensor):
+    @torch.no_grad()
+    def reconstruct(self, x: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Sample the inverted latents back to clean latents (the reference's `recon`, Inverter.ddim_sample,
+        invert.py:142-157 and 272-273): over the forward DDIM timesteps, every batch's noise prediction with its rows
+        of cond and of the ControlNet or depth inputs, as in invert() (no CFG), then x <- mu_prev * (x - sigma * eps) /
+        mu + sigma_prev * eps.  `x` [F, 4, h, w] defaults to the last entry of `trajectory`; it is not modified.
+        Returns [F, 4, h, w].  On CUDA fp16 the update is KI with the sampling coefficients and no trajectory, and
+        with cuda_graph=True each step after the `graph_warmup` eager ones is one replay; elsewhere it is
+        sample_next_x.  With shard=True the ranks split the batches as in invert() and gather the result once."""
+        if x is None:
+            if self.trajectory is None:
+                raise RuntimeError("reconstruct: call invert() first or pass the latents")
+            x = self.trajectory[-1]
+        flen = len(x) if x.dim() == 4 else 0
+        x, frames, cond, kernel = self._inputs(x)
+        scope = patch._unmerged_blocks() if self._patched() else contextlib.nullcontext()
+        with scope:
+            if len(x) == 0:
+                pass
+            elif kernel:
+                coefficients = [self.sample_coefficients(i) for i in range(len(self.sample_timesteps))]
+                self._run_device(x, frames, cond, coefficients, self.sample_timesteps)
+            else:
+                with torch.autocast(x.device.type, dtype=torch.float16, enabled=x.is_cuda):
+                    for i, t in enumerate(self.sample_timesteps):
+                        x = self.sample_next_x(x, self._all_noises(x, t, frames, cond), i)
+        return self._gather(x, flen, 0)
+
+    def _run_device(self, x: torch.Tensor, frames: dict, cond: Optional[torch.Tensor], coefficients,
+                    timesteps: List[int], slots: Optional[List[int]] = None, traj: Optional[torch.Tensor] = None):
+        """Every step of `timesteps` on x in place, each ending with KI on the step's `coefficients` (a, b, c, d), and
+        with `slots` its store of x into `traj`: `graph_warmup` eager steps, then, with cuda_graph=True, one replay
+        per step of a graph that reads the UNet's timestep, KI's coefficients and its slot at a device step counter and
+        advances it."""
         from . import ops
-        coef, slots, ts, step = self._device_tables(x)
-        n = len(self.timesteps)
+        coef = ops.ddim_table(coefficients).to(x.device)
+        ts = torch.tensor(timesteps, dtype=torch.int64, device=x.device)
+        step = torch.zeros(1, dtype=torch.int32, device=x.device)
+        if slots is not None:
+            slots = torch.tensor(slots, dtype=torch.int32, device=x.device)
+        n = len(timesteps)
         eager = n if not self.cuda_graph else min(self.graph_warmup, n)
         with torch.autocast("cuda", dtype=torch.float16):
             for i in range(eager):
-                eps = self._all_noises(x, self.timesteps[i], frames)
+                eps = self._all_noises(x, timesteps[i], frames, cond)
                 ops.ddim_update(x, eps, coef, step, slots, traj)
                 step.add_(1)
         if eager == n:
@@ -906,7 +1002,7 @@ class ChunkedInverter:
         torch.cuda.synchronize(x.device)
         with torch.cuda.graph(graph), torch.autocast("cuda", dtype=torch.float16, cache_enabled=False):
             gt = torch.index_select(ts, 0, step)                          # the UNet's timestep input, [1]
-            eps = self._all_noises(x, gt, frames)
+            eps = self._all_noises(x, gt, frames, cond)
             ops.ddim_update(x, eps, coef, step, slots, traj)
             step.add_(1)
         for _ in range(eager, n):
