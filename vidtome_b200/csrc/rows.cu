@@ -45,8 +45,8 @@ struct LnParams {
 };
 
 // In-register LayerNorm of one row held as P vectors per lane by a G-lane group (torch half semantics: fp32
-// statistics, y = gamma * (rstd * (x - mean)) + beta in fp32, rounded to fp16).  The kernels that fuse it are bound by
-// instruction issue, not by HBM, so the row is converted to fp32 ONCE and kept in registers through both statistics
+// statistics, y = gamma * (rstd * (x - mean)) + beta in fp32, rounded to fp16).  To keep the instruction count of the
+// kernels that fuse it down, the row is converted to fp32 ONCE and kept in registers through both statistics
 // passes and the affine step, and gamma / beta are read as fp32 from shared memory (staged once per CTA by
 // stage_ln_params) instead of two 16-byte global loads + 16 conversions per data vector.
 constexpr int LN_MAX_C = 2048;
@@ -116,9 +116,9 @@ __device__ __forceinline__ void layer_norm_row(uint4 (&v)[P], int sub, int vecs,
 // merge.py:84 `metric = metric / metric.norm(dim=-1, keepdim=True)`; merge.py:76-85 split().
 // torch half semantics: norm accumulates in fp32 and is rounded to fp16; the division is carried out
 // in fp32 on the fp16-rounded norm and rounded to fp16.
-// K0 is bound by instruction issue, not by HBM (ncu: 866 warp instructions per two rows of 640 values, issue slots 54 %,
-// DRAM 19 %): FULL (see layer_norm_row) removes the per-vector range tests and the two division variants run as separate
-// loops instead of a test per value pair.
+// FULL (see layer_norm_row) removes the per-vector range tests, and the two division variants run as separate loops
+// instead of a test per value pair.  Neither loop may index v at run time (see the slow one): the row must stay in
+// registers, or K0 stops streaming at HBM rate.
 // DC: device-count (mode 2) split, src / dst rows at the capacity's row stride (vtm_split_t mode 2)
 template <int G, int P, bool LN, bool FULL = false, bool DC = false>
 __global__ void __launch_bounds__(ROW_THREADS, LN ? 3 : 4)
@@ -212,7 +212,10 @@ normalize_split_kernel(const __half* __restrict__ x, long long x_bs, const int* 
         }
       }
     } else {
-#pragma unroll 1
+      // Unrolled like the fast path.  A loop here would index v at run time, which puts v in local memory, and then
+      // every row, slow or not, stores its vectors there (ptxas reports that frame as stack, not as spill).  With such
+      // a loop K0 ran at 1.2-1.7 TB/s on H100; without it, 2.5-3.2 TB/s.
+#pragma unroll
       for (int i = 0; i < P; ++i) {
         if (live && (FULL || sub + G * i < vecs)) {
           __half2* h = reinterpret_cast<__half2*>(&v[i]);
