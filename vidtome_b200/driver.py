@@ -34,6 +34,35 @@ from . import patch, pnp
 # it was captured with.
 FUSE_STEP_UPDATE = True
 
+# A step captured into one CUDA graph (cuda_graph=True with local merging, or capture_global=True) issues chunk k on
+# side stream ("lane") k % LANES, forked from the capture stream and joined back into it, so the graph runs the chunks
+# concurrently.  With local merging nothing links two chunks; with global merging the one edge is the global-token
+# recurrence, per merged block (patch.LaneEdges).  Each captured draw has a fixed Philox offset, so the latents are those
+# of one stream, bit for bit.  A step of one chunk, or shard=True, captures on the capture stream alone.  DESIGN §5 and
+# §7 give the reasons for the count.
+LANES = 3
+
+
+def run_on_lanes(n: int, lanes: list, body: Callable[[int], None], edges=None) -> None:
+    """body(k) for k in range(n), inside a capture: on the current stream when fewer than two lanes are given, else
+    chunk k on lanes[k % len(lanes)], every lane forked from the current stream first and joined into it at the end,
+    with `edges` (patch.LaneEdges, or None) installed for the global stages."""
+    if len(lanes) < 2:
+        for k in range(n):
+            body(k)
+        return
+    main = torch.cuda.current_stream()
+    for lane in lanes:
+        lane.wait_stream(main)
+    try:
+        with patch.lane_edges(edges):
+            for k in range(n):
+                with torch.cuda.stream(lanes[k % len(lanes)]):
+                    body(k)
+    finally:
+        for lane in lanes:
+            main.wait_stream(lane)
+
 
 def ddim_alphas_cumprod(num_train_timesteps: int = 1000, beta_start: float = 0.00085,
                         beta_end: float = 0.012) -> torch.Tensor:
@@ -220,6 +249,8 @@ class ChunkedDenoiser:
         self._chunk_t = None        # the UNet's timestep input shared by the chunk graphs
         self._stores = []           # patch.GlobalTokenStore of every block (chunk_graphs with merge_global)
         self._tables = {}           # device -> (KS's coefficient table, its step index), made on first use
+        self._lane_count = LANES    # streams of a captured step (LANES; fewer when the KB1 sorts would not fit)
+        self._lanes = {}            # device -> its lane streams, made before the first capture
         self.chunk_size = chunk_size
         self.guidance_scale = guidance_scale
         self.merge_global = merge_global
@@ -447,23 +478,63 @@ class ChunkedDenoiser:
             return tuple(x.shape), self.injecting(t)
         return tuple(x.shape), self.injecting(t), self.conv_injecting(t)
 
+    def _lane_streams(self, device: torch.device, n_chunks: int) -> list:
+        """The lanes of a capture of `n_chunks` chunks: min(_lane_count, n_chunks) streams of `device`, made once per
+        driver (before any capture).  None with shard=True, or before any eager step: then the state that the first
+        call of a module creates (packed weights, generators) would be made on one lane and read on another."""
+        n = 0 if self.shard or self._eager_steps < 1 else min(self._lane_count, n_chunks)
+        lanes = self._lanes.setdefault(device, [])
+        while n > 1 and len(lanes) < n:
+            lanes.append(torch.cuda.Stream(device))
+        return lanes[:n] if n > 1 else []
+
+    def _lane_edges(self, lanes: list):
+        """patch.LaneEdges over every merged block of the models, for a capture on `lanes` (None on one stream)."""
+        if not lanes:
+            return None
+        return patch.LaneEdges(m for model in self._models() for m in model.modules()
+                               if type(m).__name__ == "ToMeBlock")
+
+    def _lanes_fit(self, lanes: list, grids: List[int], device) -> bool:
+        """Whether the KB1 sorts of a capture on `lanes` (their CTA counts `grids`) can all be resident together:
+        a sort of at most ops.sort_co_resident CTAs is one launch whose CTAs wait for each other at spin barriers, so
+        the sorts that several lanes may run at once must fit on the device side by side."""
+        from . import ops
+        cap = ops.sort_co_resident(device)
+        return len(lanes) * max([c for c in grids if c <= cap], default=0) <= cap
+
     def _capture(self, x: torch.Tensor, t: int, frames: dict):
-        """Capture the step for inputs shaped like `x`: `_all_next_x` (every chunk's x_{t-1}) when the update is fused
-        (_fuses_update), else `_all_noises` (called after the eager warm-up steps, so that every
-        lazily created piece of state — generators forked by the hook, cached packed weights, the library handle,
-        allocator pools — already exists)."""
+        """Capture the step for inputs shaped like `x`: every chunk's x_{t-1} (_next_x_rows, as `_all_next_x`) when the
+        update is fused (_fuses_update), else every chunk's noise prediction (as `_all_noises`), chunk k on lane
+        k % LANES (run_on_lanes).  Called after the eager warm-up steps, so that every lazily created piece of state —
+        generators forked by the hook, cached packed weights, the library handle, allocator pools — already exists."""
+        from . import ops
         self._graph = None                                                   # release the previous graph first
         gx = x.clone()
         gframes = {k: v.clone() for k, v in frames.items()}                # the per-frame inputs, set per replay
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)      # the UNet's timestep input, set per replay
         fused = self._fuses_update(x)
+        lanes = self._lane_streams(x.device, len(self.get_chunks(len(x))))
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
         torch.cuda.synchronize(x.device)
-        with torch.cuda.graph(graph):
+        with ops.recording_sort_grids() as grids, torch.cuda.graph(graph):
             # gn: the step's x_{t-1} with the fused update, else its noise prediction
-            gn = self._all_next_x(gx, gt, gframes, torch.empty_like(gx)) if fused else self._all_noises(gx, gt, gframes)
+            gn = torch.empty_like(gx) if fused else torch.zeros_like(gx)
+            spans = [(int(c[0]), int(c[-1]) + 1) for c in (self.get_chunks(len(gx)) if fused
+                                                              else self._step_chunks(len(gx)))]
+
+            def chunk(k):
+                lo, hi = spans[k]
+                if fused:
+                    self._next_x_rows(gx[lo:hi], gt, _rows(gframes, lo, hi), gn[lo:hi])
+                else:
+                    gn[lo:hi] = self.pred_noise(gx[lo:hi], gt, **_rows(gframes, lo, hi))
+            run_on_lanes(len(spans), lanes, chunk, self._lane_edges(lanes))
+        if not self._lanes_fit(lanes, grids, x.device):
+            self._lane_count = 1
+            return self._capture(x, t, frames)
         self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gframes, fused)
 
     @staticmethod
@@ -498,16 +569,23 @@ class ChunkedDenoiser:
         for model in self._models():                                        # slot 0 starts the recurrence afresh
             patch.update_patch(model, global_tokens=None)
         fused = self._fuses_update(x)
+        lanes = self._lane_streams(x.device, flen // cs)
         torch.cuda.synchronize(x.device)
-        with torch.cuda.graph(graph):
+        from . import ops
+        with ops.recording_sort_grids() as grids, torch.cuda.graph(graph):
             # gn, in slot order: the step's x_{t-1} with the fused update, else its noise prediction
             gn = torch.empty_like(gx) if fused else torch.zeros_like(gx)
-            for k in range(flen // cs):
+
+            def slot(k):
                 lo, hi = k * cs, (k + 1) * cs
                 if fused:
                     self._next_x_rows(gx[lo:hi], gt, _rows(gframes, lo, hi), gn[lo:hi])
                 else:
                     gn[lo:hi] = self.pred_noise(gx[lo:hi], gt, **_rows(gframes, lo, hi))
+            run_on_lanes(flen // cs, lanes, slot, self._lane_edges(lanes))
+        if not self._lanes_fit(lanes, grids, x.device):
+            self._lane_count = 1
+            return self._capture_slots(x, t, frames)
         idx_dev = torch.empty((2, flen), dtype=torch.int64, device=x.device)
         idx_host = torch.empty((2, flen), dtype=torch.int64).pin_memory()
         copied = torch.cuda.Event()          # the pinned buffer is rewritten only after its last upload has run

@@ -5,6 +5,7 @@ tensors and raises on anything else — there is no CPU or eager-PyTorch impleme
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from typing import Sequence, Optional, Tuple
 
@@ -149,6 +150,32 @@ def sim_argmax(a: torch.Tensor, b: torch.Tensor, align_batch: bool, simt: bool =
     return keys
 
 
+# While a list is installed here (recording_sort_grids), topr_sort appends the CTA count of every sort it issues.
+_SORT_GRIDS = None
+
+
+def sort_ctas(Bp: int, Ns: int) -> int:
+    """CTAs of KB1's grid for keys [Bp, Ns]: one 1024-key tile per CTA and row."""
+    return ((Ns + 1023) // 1024) * Bp
+
+
+def sort_co_resident(device) -> int:
+    """CTAs of KB1's single-launch sort that fit on `device` at once (2 per SM: 1024 threads of 32 registers, 44 KiB of
+    shared memory).  A sort of at most this many CTAs runs as that one launch, whose phases meet at spin barriers."""
+    return 2 * torch.cuda.get_device_properties(device).multi_processor_count
+
+
+@contextlib.contextmanager
+def recording_sort_grids():
+    """Collect the CTA counts (sort_ctas) of the KB1 sorts issued inside, in a list it yields."""
+    global _SORT_GRIDS
+    prev, _SORT_GRIDS = _SORT_GRIDS, []
+    try:
+        yield _SORT_GRIDS
+    finally:
+        _SORT_GRIDS = prev
+
+
 def topr_sort(keys: torch.Tensor, counts: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """KB1.  keys [Bp, Ns] -> (edge [Bp, Ns] int32, rank [Bp, Ns] int32).  With `counts` (device counts), Ns is the
     capacity and only the first counts[0] entries of each row are sorted."""
@@ -168,7 +195,9 @@ def topr_sort(keys: torch.Tensor, counts: Optional[torch.Tensor] = None) -> Tupl
             check(lib.vtm_topr_sort(keys.data_ptr(), Bp, Ns, edge.data_ptr(), rank.data_ptr(), ws.data_ptr(),
                                     ws_bytes, _stream()), "vtm_topr_sort")
     # one cooperative launch when all (tiles x Bp) CTAs are co-resident (2 per SM), else 6 small launches
-    STATS.launches += 1 if ((Ns + 1023) // 1024) * Bp <= 2 * torch.cuda.get_device_properties(keys.device).multi_processor_count else 6
+    STATS.launches += 1 if sort_ctas(Bp, Ns) <= sort_co_resident(keys.device) else 6
+    if _SORT_GRIDS is not None:
+        _SORT_GRIDS.append(sort_ctas(Bp, Ns))
     return edge, rank
 
 

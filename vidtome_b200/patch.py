@@ -17,7 +17,7 @@ from __future__ import annotations
 import contextlib
 import math
 from dataclasses import dataclass, field
-from typing import Any, Callable, Dict, List, Optional, Tuple, Type
+from typing import Any, Callable, Dict, Iterable, List, Optional, Tuple, Type
 
 import torch
 
@@ -103,6 +103,66 @@ FUSE_CONTROLNET_BLOCKS = False
 
 # Depth of _unmerged_blocks() contexts: while > 0 every ToMeBlock runs as the reference's UNPATCHED block.
 _UNMERGED = 0
+
+# The LaneEdges of the lane capture in progress (lane_edges), else None.
+_LANE_EDGES = None
+
+
+class LaneEdges:
+    """The global-token recurrence as the only edge between the chunks of a step captured on several streams ("lanes",
+    driver.LANES).  One event per merged block module: before a block's global stage reads the global tokens that the
+    previous chunk left (patch.py:59-82), the current stream waits on the block's event (`wait`); after the stage has
+    stored its own, it records the event on the current stream (`record`).  The reader also marks the tokens as used by
+    its stream (record_stream), so that the caching allocator does not give their memory to a later allocation on the
+    writer's stream while the reader may still copy them.  `event` and `current_stream` are the CUDA ones; they can be
+    replaced by stand-ins."""
+
+    def __init__(self, modules: Iterable[torch.nn.Module], event: Callable = None, current_stream: Callable = None):
+        self._event = event or torch.cuda.Event
+        self._current_stream = current_stream or torch.cuda.current_stream
+        self.events: Dict[int, Any] = {}
+        self.recorded = set()                  # ids of the modules whose event some chunk has recorded
+        for m in modules:
+            if id(m) not in self.events:
+                self.events[id(m)] = self._event()
+
+    def _of(self, module):
+        ev = self.events.get(id(module))
+        if ev is None:
+            raise RuntimeError(f"lane capture: {type(module).__name__} has no recurrence event; every merged block of "
+                               f"the captured models must be given one")
+        return ev
+
+    def wait(self, module, tokens) -> None:
+        """Before `module` reads `tokens`, its stored global tokens: order the read after the previous chunk's store."""
+        ev = self._of(module)
+        stream = self._current_stream()
+        if id(module) in self.recorded:
+            stream.wait_event(ev)
+        tokens.record_stream(stream)
+
+    def record(self, module) -> None:
+        """After `module` stored its global tokens: the next chunk's read of them waits on this."""
+        self._of(module).record(self._current_stream())
+        self.recorded.add(id(module))
+
+
+@contextlib.contextmanager
+def lane_edges(edges: Optional[LaneEdges]):
+    """Install `edges` for the global stages run inside (None: none; not nested)."""
+    global _LANE_EDGES
+    if _LANE_EDGES is not None and edges is not None:
+        raise RuntimeError("lane_edges: a lane capture is already in progress")
+    prev, _LANE_EDGES = _LANE_EDGES, edges
+    try:
+        yield edges
+    finally:
+        _LANE_EDGES = prev
+
+
+def active_lane_edges() -> Optional[LaneEdges]:
+    """The LaneEdges installed by lane_edges, else None (every call outside a lane capture)."""
+    return _LANE_EDGES
 
 
 @contextlib.contextmanager
@@ -246,6 +306,9 @@ def _global_stage_device_coin(module, table, mu, pi, g, ln, args, levels):
         raise ValueError("not enough values to unpack (expected 3, got 2)")  # as the host-coin path
     cat = torch.empty((B, 2 * L, C), dtype=torch.float16, device=table.device)
     ops.gather_rows(table, mu, ln=ln, out=cat[:, :L])                       # merged local tokens, straight into cat
+    edges = _LANE_EDGES
+    if edges is not None:                                                   # lane capture: after the previous store
+        edges.wait(module, g)
     cat[:, L:].copy_(g)                                                     # the stored global tokens
     split = VtmSplit.prefix_coin(L, coin, args["global_rand"])
     m = merge.match_level(cat, None, split, gratio, bool(args["align_batch"]))   # patch.py:73-74
@@ -255,6 +318,8 @@ def _global_stage_device_coin(module, table, mu, pi, g, ln, args, levels):
     merged_tokens = ops.gather_rows(cat, mu_g)                               # patch.py:75
     # patch.py:80: global_tokens <- u(merged_tokens), the local half after unmerging (kept on the device)
     module.global_tokens = ops.unmerge_add(merged_tokens, tau[:, :L], None)
+    if edges is not None:
+        edges.record(module)
     # compose with the local unmerge: pi_total[p] = tau[pi[p]]
     if pi.shape[0] != tau.shape[0]:
         pi = pi.expand(tau.shape[0], -1).contiguous()
@@ -387,6 +452,8 @@ def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[s
         else:
             merged_tokens = local_tokens
             module.global_tokens = local_tokens.detach().clone()            # patch.py:82
+            if _LANE_EDGES is not None:                                     # the first chunk of a lane capture
+                _LANE_EDGES.record(module)
     else:
         merged_tokens = ops.gather_rows(table, mu, ln=ln)                    # patch.py:50,56 composed
     return MergePlan(fsize=fsize, N0=N0, merged_tokens=merged_tokens, pi=pi, levels=levels, randf=randfs,
