@@ -99,7 +99,7 @@ def _pnp(graph, frames):
     for i in range(PNP_STEPS):
         x = den.step(x, i)
         xs.append(x.clone())
-        keys.append(den._graph[4] if graph and den._graph is not None else None)
+        keys.append(den._graph.key if graph and den._graph is not None else None)
     torch.cuda.synchronize()
     return xs, keys, den
 
@@ -289,7 +289,7 @@ def _dump(monkeypatch, tmp_path, lanes, make, tag):
         _, den = make()
     assert den._graph is not None and den._lane_count == lanes
     path = str(tmp_path / f"{tag}_{lanes}.dot")
-    den._graph[0].debug_dump(path)
+    den._graph.graph.debug_dump(path)
     with open(path) as f:
         return Dot(f.read())
 

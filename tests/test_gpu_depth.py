@@ -89,7 +89,7 @@ def test_pnp_with_depth_bit_identical_to_eager():
     eager, den_e = _run("eager_plain", pnp=True)
     assert den_e.pnp_schedule == den_e.timesteps[:3] and den_e.pnp_conv_schedule == den_e.timesteps[:4]
     graph, den = _run("step_graph", pnp=True)
-    assert den._graph[4] == (tuple(graph[0].shape), False, False)       # the last step's key: neither injection
+    assert den._graph.key == (tuple(graph[0].shape), False, False)       # the last step's key: neither injection
     _assert_identical(eager, graph)
 
 

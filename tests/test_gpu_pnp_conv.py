@@ -225,7 +225,7 @@ def _run(mode, pnp_f_t=0.75, frames=8, size=16):
         x = den.step(x, i)
         xs.append(x.clone())
         keys.append(sorted(den._chunk_graphs) if mode == "chunk_graphs" else
-                    (den._graph[4] if graph and den._graph is not None else None))
+                    (den._graph.key if graph and den._graph is not None else None))
     torch.cuda.synchronize()
     return xs, keys, den
 

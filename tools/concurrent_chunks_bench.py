@@ -128,7 +128,7 @@ def run(workload: str, lanes, rounds: int, steps: int, check_steps: int):
         out[str(n)] = {"lane_count": ch.den._lane_count,
                        "steps_per_s_median": r[len(r) // 2], "min": r[0], "max": r[-1], "all": rates[n],
                        "pool_MiB": None}
-        size = pool_bytes(ch.den._graph[0])
+        size = pool_bytes(ch.den._graph.graph)
         if size is not None:
             out[str(n)]["pool_MiB"] = round(size / 2 ** 20, 1)
     base = out["1"]["steps_per_s_median"]

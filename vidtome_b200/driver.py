@@ -20,7 +20,7 @@ Text conditioning, VAE, ControlNet and depth preprocessing and file IO are outsi
 from __future__ import annotations
 
 import contextlib
-from typing import Callable, Iterable, List, Optional
+from typing import Callable, Iterable, List, NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -77,30 +77,44 @@ def ddim_timesteps(n_timesteps: int, num_train_timesteps: int = 1000) -> List[in
     return [int(t) + 1 for t in (np.arange(0, n_timesteps) * ratio).round()[::-1]]
 
 
+def ddim_coefficients(alpha_from: torch.Tensor, alpha_to: torch.Tensor):
+    """(a, b, c, d) = (sigma_from, mu_from, mu_to, sigma_to) of the DDIM step from cumulative alpha `alpha_from` to
+    `alpha_to` (mu = alpha ** 0.5, sigma = (1 - alpha) ** 0.5), the floats ddim_step and ops.ddim_table take."""
+    return (float((1 - alpha_from) ** 0.5), float(alpha_from ** 0.5), float(alpha_to ** 0.5),
+            float((1 - alpha_to) ** 0.5))
+
+
+def ddim_step(x: torch.Tensor, eps: torch.Tensor, coefficients) -> torch.Tensor:
+    """x <- c * ((x - a * eps) / b) + d * eps: the predicted x0 moved to the other timestep (generate.py:281-311,
+    invert.py:182-211)."""
+    a, b, c, d = coefficients
+    return c * ((x - a * eps) / b) + d * eps
+
+
 def _rows(frames: dict, lo: int, hi: int) -> dict:
     """Frames lo..hi-1 of every per-frame input ({"src" | "ctrl" | "depth": [flen, ...]}) of a step."""
     return {k: v[lo:hi] for k, v in frames.items()}
 
 
-def _check_depth_arg(depth: Optional[torch.Tensor], controlnet: Optional[torch.nn.Module]):
-    if depth is None:
-        return
-    if depth.dim() != 4 or depth.shape[1] != 1:
-        raise ValueError(f"depth must be [flen, 1, h, w] (got {tuple(depth.shape)})")
-    if controlnet is not None:
-        raise ValueError("depth and controlnet are exclusive: the reference's ControlNets are SD1.5 models with a "
-                         "4-channel input, and its configs use no control with the depth model")
+def _spans(chunks: List[torch.Tensor]) -> List[tuple]:
+    """(lo, hi) of every chunk: chunks are contiguous frame ranges (possibly visited in another order), so a step slices
+    instead of indexing with a host tensor, which would cost a synchronous host->device copy per chunk per step."""
+    return [(int(c[0]), int(c[-1]) + 1) for c in chunks]
 
 
-def _check_depth(depth: torch.Tensor, x: torch.Tensor, model: torch.nn.Module):
-    """One depth map per frame at the latents' resolution, for a model that takes the latent channels + 1."""
-    if len(depth) != len(x) or depth.shape[2:] != x.shape[2:]:
-        raise ValueError(f"depth is {tuple(depth.shape)}, the latents {tuple(x.shape)}: it needs one map per frame at "
-                         f"the latents' resolution")
-    n = getattr(getattr(model, "config", None), "in_channels", getattr(model, "in_channels", None))
-    if isinstance(n, int) and n != x.shape[1] + 1:
-        raise ValueError(f"depth: the model takes {n} input channels, not the latents' {x.shape[1]} and one depth "
-                         f"channel")
+class _Graph(NamedTuple):
+    """A captured step or chunk: `graph` reads the static inputs `x`, `t` and `frames` ({"src" | "ctrl" | "depth"})
+    and writes `out`, x_{t-1} when `fused` (KS ends every chunk), else the noise prediction.  The first five fields
+    keep the positions the driver's graph tuples always had (graph, x, t, out, key), for code that indexes them."""
+    graph: torch.cuda.CUDAGraph
+    x: torch.Tensor
+    t: torch.Tensor
+    out: torch.Tensor
+    key: tuple                      # _graph_key for a step graph, the chunk key for a chunk graph
+    frames: dict
+    fused: bool
+    phase: tuple                    # the PnP injections it was captured with (_phase)
+    slots: Optional[tuple] = None   # capture_global: (slot index on the device, its pinned host copy, upload event)
 
 
 class _ControlNetServing:
@@ -129,7 +143,64 @@ class _ControlNetServing:
         self.decided = self.controlnet is None
 
 
-class ChunkedDenoiser:
+class _Driver:
+    """What both drivers share: the UNet, the optional ControlNet with its control images or the optional depth maps,
+    and the DDIM schedule."""
+
+    def __init__(self, unet: torch.nn.Module, controlnet: Optional[torch.nn.Module],
+                 control_images: Optional[torch.Tensor], control_scale: float, depth: Optional[torch.Tensor],
+                 source_latents: Optional[Callable[[int], torch.Tensor]] = None):
+        if depth is not None and (depth.dim() != 4 or depth.shape[1] != 1):
+            raise ValueError(f"depth must be [flen, 1, h, w] (got {tuple(depth.shape)})")
+        if depth is not None and controlnet is not None:
+            raise ValueError("depth and controlnet are exclusive: the reference's ControlNets are SD1.5 models with a "
+                             "4-channel input, and its configs use no control with the depth model")
+        if controlnet is not None and source_latents is not None:
+            raise ValueError("controlnet and source_latents (PnP) are exclusive: the reference runs one control mode "
+                             "(generate.py:61-68)")
+        if (controlnet is None) != (control_images is None):
+            raise ValueError("controlnet and control_images go together")
+        if control_images is not None and (control_images.dim() != 4 or control_images.shape[1] != 3):
+            raise ValueError(f"control_images must be [flen, 3, H, W] (got {tuple(control_images.shape)})")
+        self.unet = unet
+        self.controlnet = controlnet
+        self.control_images = control_images
+        self.control_scale = control_scale
+        self.depth = depth
+        self._serving = _ControlNetServing(controlnet)
+        self.alphas_cumprod = ddim_alphas_cumprod()
+        self.final_alpha_cumprod = self.alphas_cumprod[0]     # set_alpha_to_one=False in SD's config
+
+    def _models(self) -> List[torch.nn.Module]:
+        """The UNet and, with ControlNet control, the ControlNet: the models whose blocks the driver serves."""
+        return [self.unet] + ([self.controlnet] if self.controlnet is not None else [])
+
+    def _alpha(self, timesteps: List[int], k: int) -> torch.Tensor:
+        """The cumulative alpha at timesteps[k]; final_alpha_cumprod before the first and after the last one."""
+        return self.alphas_cumprod[timesteps[k]] if 0 <= k < len(timesteps) else self.final_alpha_cumprod
+
+    def _frames(self, x: torch.Tensor, frames: dict) -> dict:
+        """`frames` with the control images ("ctrl") or the depth maps ("depth") of the latents x added, checked against
+        x and cast to its dtype (prepare_data's .to(self.init_noise)).  An unpatched ControlNet is served here."""
+        if self.controlnet is not None:
+            if len(self.control_images) != len(x):
+                raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
+            frames["ctrl"] = self.control_images.to(x)
+            self._serving.before_step()
+        if self.depth is not None:
+            # one depth map per frame at the latents' resolution, for a model that takes the latent channels + 1
+            if len(self.depth) != len(x) or self.depth.shape[2:] != x.shape[2:]:
+                raise ValueError(f"depth is {tuple(self.depth.shape)}, the latents {tuple(x.shape)}: it needs one map "
+                                 f"per frame at the latents' resolution")
+            n = getattr(getattr(self.unet, "config", None), "in_channels", getattr(self.unet, "in_channels", None))
+            if isinstance(n, int) and n != x.shape[1] + 1:
+                raise ValueError(f"depth: the model takes {n} input channels, not the latents' {x.shape[1]} and one "
+                                 f"depth channel")
+            frames["depth"] = self.depth.to(x)
+        return frames
+
+
+class ChunkedDenoiser(_Driver):
     """Chunked classifier-free-guidance DDIM sampling on a (patched) UNet, generate.py:205-311."""
 
     def __init__(self, unet: torch.nn.Module, n_timesteps: int = 50, chunk_size: int = 16,
@@ -205,28 +276,14 @@ class ChunkedDenoiser:
         (generate.py:255-262).  Depth combines with PnP (the reference's default `control: "pnp"`) and with every graph
         mode, in each of which the depth maps are a static input like the control images; graph keys do not change.
         Depth with `controlnet` is refused: the reference's ControlNets are SD1.5 models with a 4-channel input."""
-        _check_depth_arg(depth, controlnet)
-        self.depth = depth
-        if controlnet is not None and source_latents is not None:
-            raise ValueError("controlnet and source_latents (PnP) are exclusive: the reference runs one control mode "
-                             "(generate.py:61-68)")
-        if (controlnet is None) != (control_images is None):
-            raise ValueError("controlnet and control_images go together")
-        if control_images is not None and (control_images.dim() != 4 or control_images.shape[1] != 3):
-            raise ValueError(f"control_images must be [flen, 3, H, W] (got {tuple(control_images.shape)})")
-        self.controlnet = controlnet
-        self.control_images = control_images
-        self.control_scale = control_scale
-        self._serving = _ControlNetServing(controlnet)
-        self.unet = unet
+        super().__init__(unet, controlnet, control_images, control_scale, depth, source_latents)
         # shard=True: this process is one rank of a torch.distributed job and takes chunks i % world == rank of every
         # step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
         # lock-step once per step (dist.check_step_lockstep)
         self.shard = bool(shard)
         self.cuda_graph = bool(cuda_graph)
         self.graph_warmup = int(graph_warmup)
-        self._graph = None          # (CUDAGraph, static x, static timestep, static noise or x_{t-1}, key[, slot
-                                    #  index state], static per-frame inputs, fused update)
+        self._graph: Optional[_Graph] = None     # the step graph of cuda_graph=True or capture_global=True
         self._eager_steps = 0
         self.capture_global = bool(capture_global)
         self.chunk_graphs = bool(chunk_graphs)
@@ -243,8 +300,7 @@ class ChunkedDenoiser:
             raise ValueError("cuda_graph=True needs merge_global=False and randomize_chunks=False (static work)")
         if self.capture_global and self.shard:
             raise ValueError("capture_global=True does not capture the cross-rank exchange of shard=True")
-        # (chunk length, first in step, frame shape, PnP injection[, PnP conv injection when pnp_f_t is set], fused
-        #   update) -> (CUDAGraph, static x, static noise or x_{t-1}, static per-frame inputs {"src" | "ctrl" | "depth"})
+        # (chunk length, first in step, frame shape) + _phase + (fused update,) -> _Graph
         self._chunk_graphs = {}
         self._chunk_t = None        # the UNet's timestep input shared by the chunk graphs
         self._stores = []           # patch.GlobalTokenStore of every block (chunk_graphs with merge_global)
@@ -261,8 +317,6 @@ class ChunkedDenoiser:
         self.chunk_ord, self.perm_div = chunk_ord, perm_div
         self.randomize_chunks = randomize_chunks
         self.cond = cond                      # [2, 77, D] (uncond, cond) text embeddings, may be None
-        self.alphas_cumprod = ddim_alphas_cumprod()
-        self.final_alpha_cumprod = self.alphas_cumprod[0]     # set_alpha_to_one=False in SD's config
         self.timesteps = ddim_timesteps(n_timesteps)
         self.source_latents = source_latents
         self.pnp_schedule: List[int] = []
@@ -378,25 +432,12 @@ class ChunkedDenoiser:
 
     # generate.py:281-311 (inversion=False branch)
     def pred_next_x(self, x: torch.Tensor, eps: torch.Tensor, i: int) -> torch.Tensor:
-        t = self.timesteps[i]
-        alpha_prod_t = self.alphas_cumprod[t]
-        alpha_prod_t_prev = (self.alphas_cumprod[self.timesteps[i + 1]] if i < len(self.timesteps) - 1
-                             else self.final_alpha_cumprod)
-        mu, sigma = float(alpha_prod_t ** 0.5), float((1 - alpha_prod_t) ** 0.5)
-        mu_prev, sigma_prev = float(alpha_prod_t_prev ** 0.5), float((1 - alpha_prod_t_prev) ** 0.5)
-        pred_x0 = (x - sigma * eps) / mu
-        return mu_prev * pred_x0 + sigma_prev * eps
+        return ddim_step(x, eps, self.coefficients(i))
 
     def coefficients(self, i: int):
         """(a, b, c, d) of step i for x <- c * ((x - a * eps) / b) + d * eps: (sigma, mu, mu_prev, sigma_prev), the
         floats pred_next_x takes (generate.py:281-311, inversion=False)."""
-        t = self.timesteps[i]
-        alpha_prod_t = self.alphas_cumprod[t]
-        alpha_prod_t_prev = (self.alphas_cumprod[self.timesteps[i + 1]] if i < len(self.timesteps) - 1
-                             else self.final_alpha_cumprod)
-        mu, sigma = float(alpha_prod_t ** 0.5), float((1 - alpha_prod_t) ** 0.5)
-        mu_prev, sigma_prev = float(alpha_prod_t_prev ** 0.5), float((1 - alpha_prod_t_prev) ** 0.5)
-        return sigma, mu, mu_prev, sigma_prev
+        return ddim_coefficients(self._alpha(self.timesteps, i), self._alpha(self.timesteps, i + 1))
 
     def step_tables(self, device: torch.device):
         """KS's coefficient table ([n_steps, 4] fp32, ops.ddim_table of `coefficients`) and its step index (one int32,
@@ -413,10 +454,15 @@ class ChunkedDenoiser:
         return (FUSE_STEP_UPDATE and not self.shard and x.is_cuda and x.dtype == torch.float16
                 and x.is_contiguous())
 
-    def _next_x_rows(self, x: torch.Tensor, t, frames: dict, out: torch.Tensor):
-        """x_{t-1} of one chunk (`x`, with its rows of the per-frame inputs) into `out`, by KS at the step index that
-        step() set.  UNet output of another dtype gets pred_noise's guidance combine in torch, rounded to the
-        latents' dtype as the torch path stores it, and KI's update of the same step."""
+    def _chunk_into(self, x: torch.Tensor, t, frames: dict, out: torch.Tensor, lo: int, hi: int, fused: bool):
+        """The chunk of frames lo..hi-1 of `x` (with those rows of the per-frame inputs `frames`) into the same rows of
+        `out`: with `fused` its x_{t-1} by KS at the step index that step() set, else its noise prediction
+        (pred_noise).  Fused, a UNet output of another dtype gets pred_noise's guidance combine in torch, rounded to
+        the latents' dtype as the torch path stores it, and KI's update of the same step."""
+        x, frames, out = x[lo:hi], _rows(frames, lo, hi), out[lo:hi]
+        if not fused:
+            out.copy_(self.pred_noise(x, t, **frames))
+            return
         from . import ops
         coef, step = self.step_tables(x.device)
         eps, samples = self.unet_output(x, t, **frames)
@@ -426,14 +472,6 @@ class ChunkedDenoiser:
         noise = self.guide(eps, samples).to(x.dtype)
         out.copy_(x)
         ops.ddim_update(out, noise.contiguous(), coef, step)
-
-    def _all_next_x(self, x: torch.Tensor, t, frames: dict, out: torch.Tensor) -> torch.Tensor:
-        """The step's x_{t-1} of every frame into `out`, chunk by chunk (the fused form of _all_noises + pred_next_x;
-        shard=False, so the chunks cover every frame)."""
-        for chunk in self.get_chunks(len(x)):
-            lo, hi = int(chunk[0]), int(chunk[-1]) + 1
-            self._next_x_rows(x[lo:hi], t, _rows(frames, lo, hi), out[lo:hi])
-        return out
 
     def _step_chunks(self, flen: int) -> List[torch.Tensor]:
         chunks = self.get_chunks(flen)
@@ -448,21 +486,6 @@ class ChunkedDenoiser:
                                    "use 'allgather' for ragged chunks")
         return chunks
 
-    def _all_noises(self, x: torch.Tensor, t, frames: dict) -> torch.Tensor:
-        """`frames`: the step's per-frame inputs besides the latents, {"src" | "ctrl" | "depth": [flen, ...]} (those in
-        use), passed to pred_noise under these names."""
-        noises = torch.zeros_like(x)
-        for chunk in self._step_chunks(len(x)):
-            # chunks are contiguous frame ranges (possibly visited in another order): slice instead of indexing with
-            # a host tensor, which would cost a synchronous host->device copy per chunk per step
-            lo, hi = int(chunk[0]), int(chunk[-1]) + 1
-            noises[lo:hi] = self.pred_noise(x[lo:hi], t, **_rows(frames, lo, hi))
-        return noises
-
-    def _models(self) -> List[torch.nn.Module]:
-        """The UNet and, with ControlNet control, the ControlNet: the models whose blocks the driver serves."""
-        return [self.unet] + ([self.controlnet] if self.controlnet is not None else [])
-
     def _block_generators(self) -> List[torch.Generator]:
         seen, gens = set(), []
         for model in self._models():
@@ -473,10 +496,13 @@ class ChunkedDenoiser:
                     gens.append(g)
         return gens
 
+    def _phase(self, t: int) -> tuple:
+        """The PnP injections of step t, decided on the host when a graph is captured: attention, and conv when
+        pnp_f_t is set."""
+        return (self.injecting(t),) if self.pnp_f_t is None else (self.injecting(t), self.conv_injecting(t))
+
     def _graph_key(self, x: torch.Tensor, t: int):
-        if self.pnp_f_t is None:
-            return tuple(x.shape), self.injecting(t)
-        return tuple(x.shape), self.injecting(t), self.conv_injecting(t)
+        return (tuple(x.shape),) + self._phase(t)
 
     def _lane_streams(self, device: torch.device, n_chunks: int) -> list:
         """The lanes of a capture of `n_chunks` chunks: min(_lane_count, n_chunks) streams of `device`, made once per
@@ -503,39 +529,56 @@ class ChunkedDenoiser:
         cap = ops.sort_co_resident(device)
         return len(lanes) * max([c for c in grids if c <= cap], default=0) <= cap
 
-    def _capture(self, x: torch.Tensor, t: int, frames: dict):
-        """Capture the step for inputs shaped like `x`: every chunk's x_{t-1} (_next_x_rows, as `_all_next_x`) when the
-        update is fused (_fuses_update), else every chunk's noise prediction (as `_all_noises`), chunk k on lane
-        k % LANES (run_on_lanes).  Called after the eager warm-up steps, so that every lazily created piece of state —
-        generators forked by the hook, cached packed weights, the library handle, allocator pools — already exists."""
+    def _record(self, x: torch.Tensor, t: torch.Tensor, frames: dict, spans: List[tuple], *, fused: bool,
+                first: bool, key: tuple, phase: tuple) -> _Graph:
+        """Capture the chunks `spans` ((lo, hi) rows) of inputs shaped like `x`, with its per-frame inputs `frames` and
+        the UNet's timestep input `t`, into one graph: chunk k by _chunk_into on lane k % LANES (run_on_lanes).  The
+        global tokens start as at the first chunk of a step (`first`: none) or at a later one (the stores' tokens).
+        When the KB1 sorts of the lanes would not fit on the device together, it captures again on one stream.  Called
+        after the eager warm-up steps, so that every lazily created piece of state — generators forked by the hook,
+        cached packed weights, the library handle, allocator pools — already exists."""
         from . import ops
-        self._graph = None                                                   # release the previous graph first
         gx = x.clone()
         gframes = {k: v.clone() for k, v in frames.items()}                # the per-frame inputs, set per replay
-        gt = torch.tensor(int(t), device=x.device, dtype=torch.long)      # the UNet's timestep input, set per replay
-        fused = self._fuses_update(x)
-        lanes = self._lane_streams(x.device, len(self.get_chunks(len(x))))
+        lanes = self._lane_streams(x.device, len(spans))
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
+        if self.merge_global:                                               # host state only
+            self._reset_global()
+            for st in self._stores:
+                st.filled = not first
         torch.cuda.synchronize(x.device)
         with ops.recording_sort_grids() as grids, torch.cuda.graph(graph):
-            # gn: the step's x_{t-1} with the fused update, else its noise prediction
-            gn = torch.empty_like(gx) if fused else torch.zeros_like(gx)
-            spans = [(int(c[0]), int(c[-1]) + 1) for c in (self.get_chunks(len(gx)) if fused
-                                                              else self._step_chunks(len(gx)))]
-
-            def chunk(k):
-                lo, hi = spans[k]
-                if fused:
-                    self._next_x_rows(gx[lo:hi], gt, _rows(gframes, lo, hi), gn[lo:hi])
-                else:
-                    gn[lo:hi] = self.pred_noise(gx[lo:hi], gt, **_rows(gframes, lo, hi))
-            run_on_lanes(len(spans), lanes, chunk, self._lane_edges(lanes))
+            out = torch.empty_like(gx) if fused else torch.zeros_like(gx)
+            run_on_lanes(len(spans), lanes, lambda k: self._chunk_into(gx, t, gframes, out, *spans[k], fused),
+                         self._lane_edges(lanes))
         if not self._lanes_fit(lanes, grids, x.device):
             self._lane_count = 1
-            return self._capture(x, t, frames)
-        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), gframes, fused)
+            return self._record(x, t, frames, spans, fused=fused, first=first, key=key, phase=phase)
+        return _Graph(graph=graph, x=gx, t=t, out=out, key=key, frames=gframes, fused=fused, phase=phase)
+
+    def _capture(self, x: torch.Tensor, t: int, frames: dict):
+        """Capture the step graph for inputs shaped like `x`: the chunks of _step_chunks or, with capture_global, chunk
+        slots (slot k runs rows [k * chunk_size, (k + 1) * chunk_size) of the step's visiting order, which _replay
+        applies as data).  Neither draws from the host RNG: fixed chunking with local merging draws nothing, and the
+        slots need no chunk list."""
+        if self.capture_global and patch.GLOBAL_EXCHANGE != "recurrence":
+            raise RuntimeError(f"capture_global=True needs patch.GLOBAL_EXCHANGE='recurrence' (got "
+                               f"{patch.GLOBAL_EXCHANGE!r}): the cross-rank exchange is not captured")
+        self._graph = None                                                   # release the previous graph first
+        cs = self.chunk_size
+        spans = ([(lo, lo + cs) for lo in range(0, len(x), cs)] if self.capture_global
+                 else _spans(self._step_chunks(len(x))))
+        gt = torch.tensor(int(t), device=x.device, dtype=torch.long)      # the UNet's timestep input, set per replay
+        graph = self._record(x, gt, frames, spans, fused=self._fuses_update(x), first=True,
+                             key=self._graph_key(x, t), phase=self._phase(t))
+        if self.capture_global:
+            # the pinned buffer is rewritten only after its last upload has run (the event)
+            graph = graph._replace(slots=(torch.empty((2, len(x)), dtype=torch.int64, device=x.device),
+                                          torch.empty((2, len(x)), dtype=torch.int64).pin_memory(),
+                                          torch.cuda.Event()))
+        self._graph = graph
 
     @staticmethod
     def slot_index(chunks: List[torch.Tensor], flen: int) -> torch.Tensor:
@@ -551,67 +594,39 @@ class ChunkedDenoiser:
             raise RuntimeError("slot_index: the chunks must cover every frame exactly once")
         return torch.stack([fwd, inv])
 
-    def _capture_slots(self, x: torch.Tensor, t: int, frames: dict):
-        """Capture the noise prediction of one step over chunk slots (capture_global=True): slot k runs chunk k of the
-        step's visiting order on gx[k * chunk_size:(k + 1) * chunk_size].  get_chunks is not called here, so capturing
-        consumes no draw of the host RNG that eager stepping would not."""
-        flen, cs = len(x), self.chunk_size
-        if patch.GLOBAL_EXCHANGE != "recurrence":
-            raise RuntimeError(f"capture_global=True needs patch.GLOBAL_EXCHANGE='recurrence' (got "
-                               f"{patch.GLOBAL_EXCHANGE!r}): the cross-rank exchange is not captured")
-        self._graph = None                                                   # release the previous graph first
-        gx = x.clone()
-        gframes = {k: v.clone() for k, v in frames.items()}                # the per-frame inputs in slot order
-        gt = torch.tensor(int(t), device=x.device, dtype=torch.long)
-        graph = torch.cuda.CUDAGraph()
-        for g in self._block_generators():
-            graph.register_generator_state(g)
-        for model in self._models():                                        # slot 0 starts the recurrence afresh
-            patch.update_patch(model, global_tokens=None)
-        fused = self._fuses_update(x)
-        lanes = self._lane_streams(x.device, flen // cs)
-        torch.cuda.synchronize(x.device)
-        from . import ops
-        with ops.recording_sort_grids() as grids, torch.cuda.graph(graph):
-            # gn, in slot order: the step's x_{t-1} with the fused update, else its noise prediction
-            gn = torch.empty_like(gx) if fused else torch.zeros_like(gx)
-
-            def slot(k):
-                lo, hi = k * cs, (k + 1) * cs
-                if fused:
-                    self._next_x_rows(gx[lo:hi], gt, _rows(gframes, lo, hi), gn[lo:hi])
-                else:
-                    gn[lo:hi] = self.pred_noise(gx[lo:hi], gt, **_rows(gframes, lo, hi))
-            run_on_lanes(flen // cs, lanes, slot, self._lane_edges(lanes))
-        if not self._lanes_fit(lanes, grids, x.device):
-            self._lane_count = 1
-            return self._capture_slots(x, t, frames)
-        idx_dev = torch.empty((2, flen), dtype=torch.int64, device=x.device)
-        idx_host = torch.empty((2, flen), dtype=torch.int64).pin_memory()
-        copied = torch.cuda.Event()          # the pinned buffer is rewritten only after its last upload has run
-        self._graph = (graph, gx, gt, gn, self._graph_key(x, t), idx_dev, idx_host, copied, gframes, fused)
-
-    def _slot_noises(self, x: torch.Tensor, t: int, frames: dict):
-        """Replay the slot graph of the step; returns (its output in frame order, whether it is x_{t-1} rather than
-        the noise prediction)."""
+    def _replay(self, x: torch.Tensor, t: int, frames: dict):
+        """Replay the step graph, capturing it first when the step's key is new; returns its output in frame order and
+        whether that is x_{t-1} rather than the noise prediction (a graph replays the path it was captured with).
+        With capture_global the step still draws its chunk order on the host with get_chunks, as eager stepping does,
+        and applies it as data: one index_select of the inputs into the slots, one of the output back."""
         flen = len(x)
-        if flen % self.chunk_size != 0:
-            raise RuntimeError(f"capture_global=True needs a frame count divisible by chunk_size (got {flen} frames, "
-                               f"chunk_size {self.chunk_size}): chunks of unequal length cannot share one graph")
-        order = self.slot_index(self.get_chunks(flen), flen)        # the same host draws as eager stepping
-        if self._graph is None or self._graph[4] != self._graph_key(x, t):
-            self._capture_slots(x, t, frames)
-        graph, gx, gt, gn, _, idx_dev, idx_host, copied, gframes, fused = self._graph
-        copied.synchronize()
-        idx_host.copy_(order)
-        idx_dev.copy_(idx_host, non_blocking=True)
-        copied.record()
-        torch.index_select(x, 0, idx_dev[0], out=gx)                # latents -> slots
-        for k, g in gframes.items():
-            torch.index_select(frames[k], 0, idx_dev[0], out=g)
-        gt.fill_(int(t))
-        graph.replay()
-        return torch.index_select(gn, 0, idx_dev[1]), fused         # slots -> frames
+        if self.capture_global:
+            if flen % self.chunk_size != 0:
+                raise RuntimeError(f"capture_global=True needs a frame count divisible by chunk_size (got {flen} "
+                                   f"frames, chunk_size {self.chunk_size}): chunks of unequal length cannot share one "
+                                   f"graph")
+            order = self.slot_index(self.get_chunks(flen), flen)    # the same host draws as eager stepping
+        if self._graph is None or self._graph.key != self._graph_key(x, t):
+            self._capture(x, t, frames)
+        g = self._graph
+        if g.slots is None:
+            g.x.copy_(x, non_blocking=True)
+            for k, v in g.frames.items():
+                v.copy_(frames[k], non_blocking=True)
+        else:
+            index, index_host, copied = g.slots
+            copied.synchronize()
+            index_host.copy_(order)
+            index.copy_(index_host, non_blocking=True)
+            copied.record()
+            torch.index_select(x, 0, index[0], out=g.x)                # latents -> slots
+            for k, v in g.frames.items():
+                torch.index_select(frames[k], 0, index[0], out=v)
+        g.t.fill_(int(t))
+        g.graph.replay()
+        if g.slots is not None:
+            return torch.index_select(g.out, 0, index[1]), g.fused     # slots -> frames
+        return (g.out.clone() if g.fused else g.out), g.fused           # the next replay rewrites out
 
     @staticmethod
     def draw_dependent_lengths(chunk_size: int, target_stride: int) -> List[int]:
@@ -674,108 +689,61 @@ class ChunkedDenoiser:
             for model in self._models():
                 patch.update_patch(model, global_tokens=None)
 
-    def _capture_chunk(self, key, x: torch.Tensor, frames: dict):
-        """Capture the noise prediction of one chunk shaped like `x` (with the chunk's rows of the per-frame inputs), or
-        with `key[-1]` (the fused update) its x_{t-1}; `key[1]` says whether it is the first chunk of a step, i.e.
-        whether the blocks' stores are empty when it runs."""
-        gx = x.clone()
-        gframes = {k: v.clone() for k, v in frames.items()}
-        graph = torch.cuda.CUDAGraph()
-        for g in self._block_generators():
-            graph.register_generator_state(g)
-        for st in self._stores:
-            st.filled = not key[1]
-        fused = key[-1]
-        torch.cuda.synchronize(x.device)
-        with torch.cuda.graph(graph):
-            # gn: the chunk's x_{t-1} with the fused update, else its noise prediction
-            if fused:
-                gn = torch.empty_like(gx)
-                self._next_x_rows(gx, self._chunk_t, gframes, gn)
-            else:
-                gn = self.pred_noise(gx, self._chunk_t, **gframes)
-        self._chunk_graphs[key] = (graph, gx, gn, gframes)
-        return self._chunk_graphs[key]
-
-    def _chunk_graph_step(self, x: torch.Tensor, t: int, i: int, frames: dict) -> torch.Tensor:
-        """Replay every chunk's graph; returns the step's x_{t-1}.  The graphs are keyed by whether the step fuses the
-        update (_fuses_update): those captured without it give the noise prediction, which pred_next_x then takes."""
+    def _chunk_graph_step(self, x: torch.Tensor, t: int, frames: dict, fused: bool) -> torch.Tensor:
+        """Replay the graph of every chunk of the step on its rows, capturing it first when its key is new; returns the
+        step's x_{t-1} with `fused` (the graphs are keyed by it), else its noise prediction."""
         flen = len(x)
         chunks = self.get_chunks(flen)                                      # the same host draws as eager stepping
         if not self._chunk_graphs:
             self._check_chunk_lengths(flen)                                 # before anything is captured
-        inject = self.injecting(t)
-        if not inject and any(k[3] for k in self._chunk_graphs):
-            # the schedule is a prefix of the steps: the injected graphs never run again
-            self._chunk_graphs = {k: v for k, v in self._chunk_graphs.items() if not k[3]}
-        conv = self.conv_injecting(t)
-        if self.pnp_f_t is not None and not conv and any(k[4] for k in self._chunk_graphs):
-            # so is the conv schedule
-            self._chunk_graphs = {k: v for k, v in self._chunk_graphs.items() if not k[4]}
+        phase = self._phase(t)
+        # the PnP schedules are prefixes of the steps: a graph captured with an injection that has ended never runs
+        # again
+        self._chunk_graphs = {k: g for k, g in self._chunk_graphs.items()
+                              if all(now or not then for then, now in zip(g.phase, phase))}
         if self._chunk_t is None:
             self._chunk_t = torch.tensor(int(t), device=x.device, dtype=torch.long)
         self._chunk_t.fill_(int(t))
-        fused = self._fuses_update(x)
-        out = torch.empty_like(x)                       # x_{t-1} with the fused update, else the noise prediction
-        for k, chunk in enumerate(chunks):
-            lo, hi = int(chunk[0]), int(chunk[-1]) + 1
-            key = (hi - lo, self.merge_global and k == 0, tuple(x.shape[1:]), inject)
-            if self.pnp_f_t is not None:
-                key = key + (conv,)
-            key = key + (fused,)
-            entry = self._chunk_graphs.get(key)
-            if entry is None:
-                entry = self._capture_chunk(key, x[lo:hi], _rows(frames, lo, hi))
-            graph, gx, gn, gframes = entry
-            gx.copy_(x[lo:hi])
-            for name, g in gframes.items():
-                g.copy_(frames[name][lo:hi])
-            graph.replay()
-            out[lo:hi].copy_(gn)
-        return out if fused else self.pred_next_x(x, out, i)
+        out = torch.empty_like(x)
+        for k, (lo, hi) in enumerate(_spans(chunks)):
+            first = self.merge_global and k == 0        # whether the blocks' stores are empty when the chunk runs
+            key = (hi - lo, first, tuple(x.shape[1:])) + phase + (fused,)
+            g = self._chunk_graphs.get(key)
+            if g is None:
+                g = self._chunk_graphs[key] = self._record(x[lo:hi], self._chunk_t, _rows(frames, lo, hi),
+                                                           [(0, hi - lo)], fused=fused, first=first, key=key,
+                                                           phase=phase)
+            g.x.copy_(x[lo:hi])
+            for name, v in g.frames.items():
+                v.copy_(frames[name][lo:hi])
+            g.graph.replay()
+            out[lo:hi].copy_(g.out)
+        return out
 
     # one iteration of generate.py:211-224
     @torch.no_grad()
     def step(self, x: torch.Tensor, i: int) -> torch.Tensor:
         t = self.timesteps[i]
         frames = {}                                                          # the per-frame inputs, cast to x's dtype
-        if self.depth is not None:
-            _check_depth(self.depth, x, self.unet)
         if self.source_latents is not None:                                 # generate.py:226-231 (pre_iter)
             pnp.register_time(self.unet, t, modules=self._pnp_targets)
             frames["src"] = self.source_latents(t).to(x)
-        if self.controlnet is not None:
-            if len(self.control_images) != len(x):
-                raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
-            frames["ctrl"] = self.control_images.to(x)                      # prepare_data's .to(self.init_noise)
-            self._serving.before_step()
-        if self.depth is not None:
-            frames["depth"] = self.depth.to(x)                              # prepare_data's .to(self.init_noise)
+        frames = self._frames(x, frames)
         if self.chunk_graphs and self.merge_global and x.is_cuda and not self._stores:
             self._install_stores()
-        if self._fuses_update(x) or x.device in self._tables:             # KS's step index, read on the device
+        fused = self._fuses_update(x)
+        if fused or x.device in self._tables:                               # KS's step index, read on the device
             self.step_tables(x.device)[1].fill_(i)
-        if self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.chunk_graphs:
-            x = self._chunk_graph_step(x, t, i, frames)
-        elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup and self.capture_global:
-            out, fused = self._slot_noises(x, t, frames)
-            x = out if fused else self.pred_next_x(x, out, i)
-        elif self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup:
-            if self._graph is None or self._graph[4] != self._graph_key(x, t):
-                self._capture(x, t, frames)
-            graph, gx, gt, gn, _, gframes, fused = self._graph
-            gx.copy_(x, non_blocking=True)
-            for k, g in gframes.items():
-                g.copy_(frames[k], non_blocking=True)
-            gt.fill_(int(t))
-            graph.replay()
-            x = gn.clone() if fused else self.pred_next_x(x, gn, i)     # the next replay rewrites gn
-        else:
+        if not (self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup):
             self._eager_steps += 1
-            if self._fuses_update(x):
-                x = self._all_next_x(x, t, frames, torch.empty_like(x))
-            else:
-                x = self.pred_next_x(x, self._all_noises(x, t, frames), i)
+            out = torch.empty_like(x) if fused else torch.zeros_like(x)
+            for lo, hi in _spans(self._step_chunks(len(x))):
+                self._chunk_into(x, t, frames, out, lo, hi, fused)
+        elif self.chunk_graphs:
+            out = self._chunk_graph_step(x, t, frames, fused)
+        else:
+            out, fused = self._replay(x, t, frames)
+        x = out if fused else self.pred_next_x(x, out, i)
         if self.merge_global:
             self._reset_global()
         return x
@@ -795,7 +763,7 @@ class ChunkedDenoiser:
         self._serving.close()
 
 
-class ChunkedInverter:
+class ChunkedInverter(_Driver):
     """DDIM inversion of source latents in frame batches, invert.py:117-211 (`Inverter.ddim_inversion`, `pred_noise`,
     `pred_next_x(..., inversion=True)`): the trajectory PnP generation reads (`ChunkedDenoiser(source_latents=...)`).
 
@@ -853,32 +821,20 @@ class ChunkedInverter:
         save_steps = n_timesteps if save_steps is None else save_steps
         if not isinstance(save_steps, int) or save_steps <= 0:
             raise ValueError(f"save_steps must be a positive int (got {save_steps!r})")
-        if (controlnet is None) != (control_images is None):
-            raise ValueError("controlnet and control_images go together")
-        if control_images is not None and (control_images.dim() != 4 or control_images.shape[1] != 3):
-            raise ValueError(f"control_images must be [F, 3, H, W] (got {tuple(control_images.shape)})")
+        super().__init__(unet, controlnet, control_images, control_scale, depth)
         if cond is not None and (cond.dim() != 3 or cond.shape[1] != 77):
             raise ValueError(f"cond must be [F | 1, 77, D] (got {tuple(cond.shape)})")
         if cuda_graph and int(graph_warmup) < 1:
             raise ValueError(f"cuda_graph=True needs graph_warmup >= 1 (got {graph_warmup!r}): the modules' packed "
                              f"weights are created by an eager step, outside the graph's memory pool")
-        _check_depth_arg(depth, controlnet)
         from . import dist as _dist
         if shard and not _dist.initialized():
             raise ValueError("shard=True needs an initialised torch.distributed process group (one rank per process)")
         self.shard = bool(shard)
-        self.depth = depth
-        self.unet = unet
         self.batch_size = batch_size
         self.cond = cond
-        self.controlnet = controlnet
-        self.control_images = control_images
-        self.control_scale = control_scale
-        self._serving = _ControlNetServing(controlnet)
         self.cuda_graph = bool(cuda_graph)
         self.graph_warmup = int(graph_warmup)
-        self.alphas_cumprod = ddim_alphas_cumprod()
-        self.final_alpha_cumprod = self.alphas_cumprod[0]     # set_alpha_to_one=False in SD's config
         self.timesteps = ddim_timesteps(n_timesteps)[::-1]    # invert.py:120: reversed(scheduler.timesteps)
         self.sample_timesteps = ddim_timesteps(n_timesteps)   # invert.py:145: reconstruct() runs forward
         to_save = set(ddim_timesteps(save_steps)) if save_intermediate else set()
@@ -893,24 +849,14 @@ class ChunkedInverter:
     def _patched(self) -> bool:
         return any(hasattr(m, "_tome_info") for m in self._models())
 
-    def _models(self) -> List[torch.nn.Module]:
-        return [self.unet] + ([self.controlnet] if self.controlnet is not None else [])
-
     def coefficients(self, i: int):
         """(a, b, c, d) of step i for x <- c * ((x - a * eps) / b) + d * eps: (sigma_prev, mu_prev, mu, sigma),
         invert.py:182-211 with inversion=True."""
-        t = self.timesteps[i]
-        alpha_prod_t = self.alphas_cumprod[t]
-        alpha_prod_t_prev = self.alphas_cumprod[self.timesteps[i - 1]] if i > 0 else self.final_alpha_cumprod
-        mu, sigma = float(alpha_prod_t ** 0.5), float((1 - alpha_prod_t) ** 0.5)
-        mu_prev, sigma_prev = float(alpha_prod_t_prev ** 0.5), float((1 - alpha_prod_t_prev) ** 0.5)
-        return sigma_prev, mu_prev, mu, sigma
+        return ddim_coefficients(self._alpha(self.timesteps, i - 1), self._alpha(self.timesteps, i))
 
     # invert.py:182-211 (inversion=True branch)
     def pred_next_x(self, x: torch.Tensor, eps: torch.Tensor, i: int) -> torch.Tensor:
-        sigma_prev, mu_prev, mu, sigma = self.coefficients(i)
-        pred_x0 = (x - sigma_prev * eps) / mu_prev
-        return mu * pred_x0 + sigma * eps
+        return ddim_step(x, eps, self.coefficients(i))
 
     # invert.py:159-179
     @torch.no_grad()
@@ -931,18 +877,11 @@ class ChunkedInverter:
         """(a, b, c, d) of reconstruction step i for x <- c * ((x - a * eps) / b) + d * eps: (sigma, mu, mu_prev,
         sigma_prev) over the forward timesteps `sample_timesteps`, final_alpha_cumprod at the last step; the floats
         ChunkedDenoiser.coefficients gives for the same schedule."""
-        ts = self.sample_timesteps
-        alpha_prod_t = self.alphas_cumprod[ts[i]]
-        alpha_prod_t_prev = self.alphas_cumprod[ts[i + 1]] if i < len(ts) - 1 else self.final_alpha_cumprod
-        mu, sigma = float(alpha_prod_t ** 0.5), float((1 - alpha_prod_t) ** 0.5)
-        mu_prev, sigma_prev = float(alpha_prod_t_prev ** 0.5), float((1 - alpha_prod_t_prev) ** 0.5)
-        return sigma, mu, mu_prev, sigma_prev
+        return ddim_coefficients(self._alpha(self.sample_timesteps, i), self._alpha(self.sample_timesteps, i + 1))
 
     def sample_next_x(self, x: torch.Tensor, eps: torch.Tensor, i: int) -> torch.Tensor:
         """Reconstruction step i in torch ops (invert.py:182-211 with inversion=False)."""
-        sigma, mu, mu_prev, sigma_prev = self.sample_coefficients(i)
-        pred_x0 = (x - sigma * eps) / mu
-        return mu_prev * pred_x0 + sigma_prev * eps
+        return ddim_step(x, eps, self.sample_coefficients(i))
 
     def _check_cond(self, flen: int):
         if self.cond is not None and self.cond.shape[0] not in (1, flen):
@@ -971,15 +910,7 @@ class ChunkedInverter:
         and of {"ctrl" | "depth"} and cond (all frames unless shard=True), and whether KI updates them."""
         if x.dim() != 4:
             raise ValueError(f"latents must be [F, 4, h, w] (got {tuple(x.shape)})")
-        frames = {}
-        if self.controlnet is not None:
-            if len(self.control_images) != len(x):
-                raise ValueError(f"control_images has {len(self.control_images)} frames, the latents {len(x)}")
-            frames["ctrl"] = self.control_images.to(x)
-            self._serving.before_step()
-        if self.depth is not None:
-            _check_depth(self.depth, x, self.unet)
-            frames["depth"] = self.depth.to(x)
+        frames = self._frames(x, {})
         self._check_cond(len(x))                                             # the row count, up front
         kernel = x.is_cuda and x.dtype == torch.float16
         if self.cuda_graph and not kernel:
