@@ -57,7 +57,8 @@ extern "C" {
  *     src = positions [0, src_len), dst = positions [src_len, N).
  *     With `coin_dev` != NULL the global stage's coin (vidtome/patch.py:62, `torch.rand(1) > global_rand`) stays on the
  *     device: the sequence is stored as [local tokens (first src_len rows) | global tokens (the other N - src_len)],
- *     and the kernels compare the fp32 draw *coin_dev, widened to double, against `coin_threshold`:
+ *     and the kernels compare the fp32 draw *coin_dev in fp32 against `coin_threshold` rounded to the nearest float,
+ *     as torch compares an fp32 tensor with a Python float (a draw equal to fp32(global_rand) is never greater):
  *       coin > threshold:     src = [0, src_len), dst = [src_len, N)  (the reference's [local | global], patch.py:63-66);
  *       otherwise:            src = [src_len, N), dst = [0, src_len)  (its [global | local], patch.py:68-71, with
  *                             positions numbered in storage order).
@@ -83,7 +84,7 @@ typedef struct vtm_split {
   int32_t src_len;
   const int32_t* randf_dev; /* optional device-resident randf (mode 0), NULL = use `randf` */
   const float* coin_dev;    /* optional device-resident global coin (mode 1), NULL = plain prefix split */
-  double coin_threshold;    /* global_rand: the halves swap roles when !(coin > coin_threshold) */
+  double coin_threshold;    /* global_rand: the halves swap roles when !(coin > (float)coin_threshold) */
   const int32_t* glob_len_dev; /* mode 2: device-resident length of the global set, 1 <= *glob_len_dev <= glob_cap */
   int32_t glob_cap;            /* mode 2: capacity of the global set */
 } vtm_split_t;

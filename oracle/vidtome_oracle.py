@@ -272,6 +272,9 @@ def compute_merge(x: np.ndarray, size: Tuple[int, int], *, batch_size: int, loca
             # merge.py:45-46: identity ops and unm_num = tnum; no RNG draw happens
             unm += (N - unm) // curF
         else:
+            if min(target_stride, curF) < 2:
+                # every frame is dst: nothing merges and curF never falls, so the reference loops forever
+                raise ValueError(f"target_stride {target_stride}: the local levels never reduce the frame count")
             rf = int(draw_randf(min(target_stride, curF)))
             randfs.append(rf)
             m = bipartite_soft_matching_randframe(local_tokens, curF, local_merge_ratio, unm, rf,
@@ -288,7 +291,8 @@ def compute_merge(x: np.ndarray, size: Tuple[int, int], *, batch_size: int, loca
         if global_tokens is not None:                                         # :60
             coin = float(draw_coin())
             g = global_tokens.astype(local_tokens.dtype)                      # .to(local_tokens) :65,:70
-            if coin > global_rand:                                            # :62
+            # :62 torch compares its fp32 draw with the Python float in fp32: global_rand rounds to nearest first
+            if np.float32(coin) > np.float32(global_rand):
                 src_len = local_tokens.shape[1]
                 tokens = np.concatenate([local_tokens, g], axis=1)            # :64-65
                 local_chunk = 0

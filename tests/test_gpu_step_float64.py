@@ -226,7 +226,7 @@ class Replay:
         assert "mu_g" in call and "tau" in call, "the library ran no global stage where global tokens exist"
         mu_g = call["mu_g"].long()[:, :plan["M"]]
         Lg = call["cat_len"] - L
-        if plan["host_coin"] and plan["coin"] <= call["rand"]:
+        if plan["host_coin"] and not np.float32(plan["coin"]) > np.float32(call["rand"]):    # patch.py:62, in fp32
             # [global | local] in the host-coin path (patch.py:68-71): as positions of [local | global]
             mu_g = torch.where(mu_g < Lg, mu_g + L, mu_g - Lg)
         if store.shape[1] < Lg:

@@ -44,7 +44,8 @@ class VtmSplit(C.Structure):
     def prefix_coin(cls, L: int, coin, global_rand: float) -> "VtmSplit":
         """The global stage's split with its coin left on the device: the sequence is stored as [local (L rows) |
         global (L rows)], and the kernels read `coin` (a 1-element fp32 CUDA tensor, kept alive on the descriptor)
-        to pick the roles.  coin > global_rand: src = local, dst = global; otherwise src = global, dst = local."""
+        to pick the roles.  coin > global_rand, compared in fp32 as torch compares the reference's fp32 draw with a
+        Python float (patch.py:62): src = local, dst = global; otherwise src = global, dst = local."""
         import torch
         if not (isinstance(coin, torch.Tensor) and coin.is_cuda and coin.dtype == torch.float32 and coin.numel() == 1):
             raise RuntimeError("VtmSplit.prefix_coin: coin must be a 1-element float32 CUDA tensor")
@@ -59,9 +60,9 @@ class VtmSplit(C.Structure):
     def prefix_coin_dev(cls, L: int, glob_len_dev, glob_cap: int, coin, global_rand: float) -> "VtmSplitDev":
         """The global stage's split when the two token sets may differ in length (mode 2): the sequence is stored as
         [local (L rows) | global (*glob_len_dev rows, at most glob_cap)], and the coin picks the src half as in
-        prefix_coin.  The counts that follow from the draw (Ns, Nd, r, the merged length) stay on the device
-        (ops.split_counts_dev); `glob_len_dev` is a 1-element int32 CUDA tensor, kept alive on the descriptor with
-        the coin."""
+        prefix_coin (compared in fp32).  The counts that follow from the draw (Ns, Nd, r, the merged length) stay on
+        the device (ops.split_counts_dev); `glob_len_dev` is a 1-element int32 CUDA tensor, kept alive on the
+        descriptor with the coin."""
         import torch
         if not (isinstance(coin, torch.Tensor) and coin.is_cuda and coin.dtype == torch.float32 and coin.numel() == 1):
             raise RuntimeError("VtmSplit.prefix_coin_dev: coin must be a 1-element float32 CUDA tensor")

@@ -22,7 +22,7 @@ struct Split {
   int Ns, Nd;
   const int32_t* randf_dev;  // device-resident randf (NULL = the value above); see resolve_split()
   const float* coin_dev;     // device-resident global coin (NULL = no swap)
-  float coin_floor;          // the largest float <= coin_threshold: for a float c, c > coin_floor <=> c > coin_threshold
+  float coin_floor;          // fp32(coin_threshold), rounded to nearest: the kernels compare the fp32 coin with it
   // mode 2 (device counts): src_len = L local rows, the global set's length is *glob_len_dev (<= gcap); randf = 1 when the
   // local half is src.  On the host N, Ns and Nd hold capacities (src_len + gcap, cap, cap); resolve_split sets them.
   const int32_t* glob_len_dev;
@@ -31,7 +31,7 @@ struct Split {
 };
 
 // Kernels call this first: with a device-resident draw, fetch it (the counts do not depend on it, make_split).
-// The coin decides as the host path decides, `float(coin) > global_rand` in double precision (see coin_floor).
+// The coin decides as the reference decides, `torch.rand(1) > global_rand` in fp32 (see coin_floor).
 // DC: the kernel serves device-count (mode 2) splits; without it that code is compiled out, so the kernels that never see
 // one keep their register budgets.
 template <bool DC = false>
@@ -53,10 +53,10 @@ __host__ inline int make_split(const vtm_split_t* s, Split* o) {
   o->randf_dev = s->mode == 0 ? s->randf_dev : nullptr;
   o->coin_dev = s->mode == 1 || s->mode == 2 ? s->coin_dev : nullptr;
   o->glob_len_dev = nullptr; o->gcap = 0; o->cap = 0;
-  // round the threshold down to a float, so that the kernels compare in fp32 and decide exactly as the double
-  // comparison does (a NaN threshold stays NaN: never greater, as in double)
+  // torch compares an fp32 tensor with a Python float in fp32: the threshold is rounded to the nearest float, so a
+  // coin equal to fp32(global_rand) is never greater even when that float lies above global_rand (a NaN threshold
+  // stays NaN: never greater)
   o->coin_floor = static_cast<float>(s->coin_threshold);
-  if (static_cast<double>(o->coin_floor) > s->coin_threshold) o->coin_floor = nextafterf(o->coin_floor, -INFINITY);
   if (s->N <= 0) return VTM_E_SPLIT;
   if (s->mode == 0) {
     if (o->randf_dev) {

@@ -23,8 +23,8 @@ import torch
 
 from . import attention, feedforward, merge, ops
 from ._lib import VtmSplit
-from .utils import (draw_coin, draw_randf, func_warper, init_generator, isinstance_str, join_frame, join_warper,
-                    split_frame, split_warper)
+from .utils import (coin_above, draw_coin, draw_randf, func_warper, init_generator, isinstance_str, join_frame,
+                    join_warper, split_frame, split_warper)
 
 
 @dataclass
@@ -191,9 +191,9 @@ class GlobalTokenStore:
     CUDA tensor), allocated once, eagerly, outside any CUDA-graph pool.  Set it as `module.global_tokens` and
     build_merge_plan runs the global stage of patch.py:59-82 with the counts that depend on the coin kept on the device
     (VtmSplit.prefix_coin_dev), eagerly or under capture, so that chunks of different lengths can follow each other in
-    one captured sequence.  `cap` is the local merged length of a chunk of `max_frames` frames.  `filled` is the host's
-    knowledge of whether the store holds tokens (the reference's `global_tokens is not None`); `reset()` empties it,
-    as `update_patch(global_tokens=None)` does for a plain tensor."""
+    one captured sequence.  `cap` is the longest local merged set of a chunk of at most `max_frames` frames, over every
+    draw (local_merged_len).  `filled` is the host's knowledge of whether the store holds tokens (the reference's
+    `global_tokens is not None`); `reset()` empties it, as `update_patch(global_tokens=None)` does for a plain tensor."""
 
     def __init__(self, max_frames: int):
         if not isinstance(max_frames, int) or max_frames <= 0:
@@ -216,7 +216,7 @@ class GlobalTokenStore:
             return
         if torch.cuda.is_current_stream_capturing():
             raise RuntimeError("GlobalTokenStore: the store is allocated by an eager call, before any capture")
-        cap = local_merged_len(self.max_frames, tsize, args)
+        cap = max(local_merged_len(f, tsize, args) for f in range(1, self.max_frames + 1))
         self.tokens = torch.zeros((B, cap, C), dtype=torch.float16, device=device)
         self.length = torch.zeros(1, dtype=torch.int32, device=device)
         self.filled = False
@@ -228,21 +228,44 @@ class GlobalTokenStore:
         self.filled = True
 
 
+def _check_progress(stride: int) -> None:
+    """A local level with stride < 2 makes every frame dst (merge.py:58-60): nothing is merged and the frame count
+    never falls, so the reference's `while curF > 1` (patch.py:44) loops forever, drawing as it goes.  Refuse it."""
+    if stride < 2:
+        raise ValueError(f"target_stride must be at least 2 to merge a chunk of several frames (got {stride}): with "
+                         f"one dst frame per frame the local levels never reduce the frame count")
+
+
 def local_merged_len(frames: int, tsize: int, args: Dict[str, Any]) -> int:
-    """Length of the local merged token set of a chunk of `frames` frames of `tsize` tokens (the counts of
-    build_merge_plan's local levels, computed on the host; with F % stride != 0 they assume the draw randf = 0)."""
-    L, unm, curF = frames * tsize, 0, frames
+    """Length of the longest local merged token set a chunk of `frames` frames of `tsize` tokens can produce: the
+    counts of build_merge_plan's local levels, computed on the host, maximised over the draws of every level whose
+    counts depend on its draw (F % stride != 0).  randf = 0 gives such a level the most dst frames, but the later
+    levels floor int(Ns * ratio) over different splits, so another draw can leave a token more (a 10-frame chunk of 84
+    tokens at ratio 0.9, stride 4: 160 tokens for randf 0 or 1, 161 for randf 2 or 3)."""
     ratio = args["local_merge_ratio"]
-    while curF > 1:
-        if ratio <= 0:
-            unm += (L - unm) // curF
-        else:
-            ns, nd = ops.split_counts(VtmSplit.local(L, unm, curF, args["target_stride"], 0))
-            r = ops.merge_count(ns, ratio)
-            unm += ns - r
-            L = ns - r + nd
-        curF = (L - unm) // tsize
-    return L
+    memo: Dict[Tuple[int, int, int], int] = {}
+
+    def longest(L: int, unm: int, curF: int) -> int:
+        if curF <= 1:
+            return L
+        key = (L, unm, curF)
+        if key not in memo:
+            if ratio <= 0:
+                unm_next = unm + (L - unm) // curF
+                memo[key] = longest(L, unm_next, (L - unm_next) // tsize)
+            else:
+                stride = min(args["target_stride"], curF)
+                _check_progress(stride)
+                best = 0
+                for randf in (range(stride) if curF % stride else (0,)):
+                    ns, nd = ops.split_counts(VtmSplit.local(L, unm, curF, args["target_stride"], randf))
+                    r = ops.merge_count(ns, ratio)
+                    L_next, unm_next = ns - r + nd, unm + ns - r
+                    best = max(best, longest(L_next, unm_next, (L_next - unm_next) // tsize))
+                memo[key] = best
+        return memo[key]
+
+    return longest(frames * tsize, 0, frames)
 
 
 def _global_stage_store(module, store: GlobalTokenStore, table, mu, pi, ln, args, levels, tsize):
@@ -364,6 +387,7 @@ def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[s
             unm += (L - unm) // curF                                         # merge.py:45-46 (no draw)
         else:
             stride = min(args["target_stride"], curF)                        # merge.py:55
+            _check_progress(stride)
             randf = draw_randf(generator, stride, curF)                      # merge.py:56-57
             randfs.append(randf)
             split = VtmSplit.local(L, unm, curF, args["target_stride"], randf)
@@ -426,7 +450,7 @@ def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[s
             coin = draw_coin(generator, on_device=False)                     # patch.py:62
             g = g.to(local_tokens).contiguous()                              # patch.py:65,70
             Lg = g.shape[1]
-            if coin > args["global_rand"]:
+            if coin_above(coin, args["global_rand"]):                        # in fp32, as torch compares
                 src_len, tokens, off = L, torch.cat([local_tokens, g], dim=1), 0          # patch.py:63-66
             else:
                 src_len, tokens, off = Lg, torch.cat([g, local_tokens], dim=1), Lg        # patch.py:68-71

@@ -1,6 +1,7 @@
 """Token / RNG helpers with the reference's names and semantics (vidtome/utils.py:4-60)."""
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 
@@ -106,4 +107,11 @@ def draw_coin(generator: torch.Generator, on_device: bool = None):
             raise RuntimeError("draw_coin: a device-resident coin needs a CUDA generator")
         return fn()
     return float(draw_scalar(generator, fn))
+
+
+def coin_above(coin: float, global_rand: float) -> bool:
+    """`torch.rand(1) > global_rand` of vidtome/patch.py:62 for a coin read back as a Python float: torch compares an
+    fp32 tensor with a Python scalar in fp32, so global_rand is rounded to the nearest float first.  A draw equal to
+    fp32(global_rand) is then never greater, even where that float lies above global_rand (0.3, 0.6, 0.8, ...)."""
+    return bool(np.float32(coin) > np.float32(global_rand))
 
