@@ -275,8 +275,31 @@ class ChunkedDenoiser(_Driver):
         131-132), repeated over the batch ([x | x], or [source | x | x] with PnP) and appended as a fifth channel
         (generate.py:255-262).  Depth combines with PnP (the reference's default `control: "pnp"`) and with every graph
         mode, in each of which the depth maps are a static input like the control images; graph keys do not change.
-        Depth with `controlnet` is refused: the reference's ControlNets are SD1.5 models with a 4-channel input."""
+        Depth with `controlnet` is refused: the reference's ControlNets are SD1.5 models with a 4-channel input.
+
+        `cond` of shape [K, S, 77, D] (S = 2, or 3 with PnP) runs K edits of one video in one pass: step() takes and
+        returns latents [K, flen, 4, h, w] and every UNet call carries the chunk of all K edits, edit-major: edit k's
+        slice is exactly the batch a single-prompt run builds with cond[k] ([source |] uncond | cond, each chunk-long),
+        and the per-frame inputs (source latents, control images, depth) are shared by all edits.  Edit k is the
+        single-prompt run of cond[k] from the same RNG state: every draw (get_chunks, the blocks' randints and coins)
+        is issued once per step, as by one run.  The model must be patched for K edits (apply_patch, then
+        update_patch(model, edits=K)); shard=True is refused with K > 1.  Every graph mode runs it; graph keys and
+        static buffers include K."""
         super().__init__(unet, controlnet, control_images, control_scale, depth, source_latents)
+        # K for a [K, S, 77, D] cond (K edits, latents [K, flen, ...]), None for the single-prompt [S, 77, D]
+        self.edits = None
+        if cond is not None and cond.dim() == 4:
+            if cond.shape[0] < 1 or cond.shape[1] not in (2, 3):
+                raise ValueError(f"cond of several edits must be [K, S, 77, D] with S = 2 or 3 (got "
+                                 f"{tuple(cond.shape)})")
+            self.edits = int(cond.shape[0])
+        K = self.edits or 1
+        if shard and K > 1:
+            raise ValueError("shard=True does not run several edits (cond [K, S, 77, D] with K > 1)")
+        for model in self._models():
+            if hasattr(model, "_tome_info") and patch.edits_of(model) != K:
+                raise ValueError(f"the model is patched with edits={patch.edits_of(model)}, the cond has {K} edit(s): "
+                                 f"set it with update_patch(model, edits={K})")
         # shard=True: this process is one rank of a torch.distributed job and takes chunks i % world == rank of every
         # step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
         # lock-step once per step (dist.check_step_lockstep)
@@ -307,6 +330,10 @@ class ChunkedDenoiser(_Driver):
         self._tables = {}           # device -> (KS's coefficient table, its step index), made on first use
         self._lane_count = LANES    # streams of a captured step (LANES; fewer when the KB1 sorts would not fit)
         self._lanes = {}            # device -> its lane streams, made before the first capture
+        # with K edits, whether a lane capture runs edits 1..K-1 of each merged block on side streams of the lane
+        # (patch.LaneEdges.edit_streams; off again when their KB1 sorts would not fit beside each other)
+        self._branch_edits = True
+        self._branches = {}         # device -> {lane stream handle: its K - 1 side streams}, made before any capture
         self.chunk_size = chunk_size
         self.guidance_scale = guidance_scale
         self.merge_global = merge_global
@@ -345,13 +372,20 @@ class ChunkedDenoiser(_Driver):
         if args is None or args["batch_size"] != 3 or not args["align_batch"]:
             raise ValueError("PnP (source_latents) needs a model patched with batch_size=3 and align_batch=True "
                              "(generate.py:96-98): the source, uncond and cond samples of every UNet call")
-        if self.cond is None or self.cond.dim() != 3 or self.cond.shape[0] != 3 or self.cond.shape[1] != 77:
-            raise ValueError("PnP (source_latents) needs cond = [3, 77, D]: the pnp guidance, uncond and cond text "
-                             "embeddings (generate.py:101-109)")
+        if self.cond is None or self.cond.dim() not in (3, 4) or self.cond.shape[-3] != 3 or self.cond.shape[-2] != 77:
+            raise ValueError("PnP (source_latents) needs cond = [3, 77, D] (or [K, 3, 77, D] for K edits): the pnp "
+                             "guidance, uncond and cond text embeddings (generate.py:101-109)")
         qk_t = int(n_timesteps * pnp_attn_t)
         self.pnp_schedule = self.timesteps[:qk_t] if qk_t >= 0 else []
         pnp.register_attention_control(self.unet, self.pnp_schedule, num_inputs=3, modules=modules)
         self._pnp_targets = pnp._targets(self.unet, modules)
+        if (self.edits or 1) > 1:
+            for m in self.unet.modules():
+                f = vars(m).get("forward")
+                if (f is not None and hasattr(m, "injection_schedule") and not getattr(f, "_vtm_pnp_forward", False)
+                        and not getattr(f, "_vtm_pnp_conv_forward", False)):
+                    raise ValueError(f"{type(m).__name__} carries the reference's PnP forward, which takes the source "
+                                     f"sample by position over the whole batch; it cannot serve several edits")
 
     def injecting(self, t: int) -> bool:
         """True if the self-attention of step t takes its map from the source sample (pnp.injection_active)."""
@@ -401,7 +435,13 @@ class ChunkedDenoiser(_Driver):
 
     # generate.py:274-279
     def guide(self, eps: torch.Tensor, batch_size: int) -> torch.Tensor:
-        """Classifier-free guidance on the raw UNet output of `batch_size` samples."""
+        """Classifier-free guidance on the raw UNet output of `batch_size` samples (of each edit: [K, ...] with K
+        edits)."""
+        if self.edits is None:
+            return self._guide_edit(eps, batch_size)
+        return torch.stack([self._guide_edit(e, batch_size) for e in eps.chunk(self.edits)])
+
+    def _guide_edit(self, eps: torch.Tensor, batch_size: int) -> torch.Tensor:
         noise_pred_uncond, noise_pred_cond = eps.chunk(batch_size)[-2:]
         return noise_pred_uncond + self.guidance_scale * (noise_pred_cond - noise_pred_uncond)
 
@@ -409,7 +449,10 @@ class ChunkedDenoiser(_Driver):
     def unet_output(self, x: torch.Tensor, t: int, src: Optional[torch.Tensor] = None,
                     ctrl: Optional[torch.Tensor] = None, depth: Optional[torch.Tensor] = None):
         """The raw UNet output of the chunk's batch ([source |] uncond | cond, each len(x) frames) and its number of
-        samples, before the guidance combine of pred_noise."""
+        samples, before the guidance combine of pred_noise.  With K edits (x [K, c, ...]) the batch is edit-major: K
+        such batches of one edit each, in edit order."""
+        if self.edits is not None:
+            return self._edits_output(x, t, src, ctrl, depth)
         flen = len(x)
         text = None if self.cond is None else self.cond.repeat_interleave(flen, dim=0)
         latent_model_input = torch.cat([x, x])                                # classifier-free guidance
@@ -417,8 +460,24 @@ class ChunkedDenoiser(_Driver):
         if src is not None:
             latent_model_input = torch.cat([src.to(x), latent_model_input])
             batch_size += 1
+        return self._call_models(latent_model_input, t, text, batch_size, ctrl, depth), batch_size
+
+    def _edits_output(self, x: torch.Tensor, t, src, ctrl, depth):
+        """unet_output of K edits x [K, c, ...]: edit k's slice of the batch is [source |] x[k] | x[k] with cond[k]'s
+        rows repeated over its c frames, as a single-prompt run builds it."""
+        text = None if self.cond is None else self.cond.repeat_interleave(x.shape[1], dim=1).flatten(0, 1)
+        lead = [] if src is None else [src.to(x)]
+        latent_model_input = torch.cat([r for xk in x for r in lead + [xk, xk]])
+        batch_size = 2 + len(lead)
+        return self._call_models(latent_model_input, t, text, batch_size, ctrl, depth, repeats=len(x)), batch_size
+
+    def _call_models(self, latent_model_input: torch.Tensor, t, text, batch_size: int, ctrl, depth, repeats: int = 1):
+        """The ControlNet (with `ctrl`) and the UNet on `repeats` batches of `batch_size` samples each; the per-frame
+        inputs are repeated over every sample, as generate.py:255-273 repeats them."""
+        batch_size = batch_size * repeats
         if depth is not None:                                                 # generate.py:256-262
-            latent_model_input = torch.cat([latent_model_input, depth.repeat(batch_size, 1, 1, 1).to(x)], dim=1)
+            latent_model_input = torch.cat([latent_model_input, depth.repeat(batch_size, 1, 1, 1).to(latent_model_input)],
+                                           dim=1)
         kwargs = {}
         if ctrl is not None:                                                  # generate.py:264-273
             controlnet_cond = ctrl.repeat(batch_size, 1, 1, 1)
@@ -427,8 +486,7 @@ class ChunkedDenoiser(_Driver):
             down = [d * self.control_scale for d in down]                    # utils/utils.py:288-292
             mid *= self.control_scale
             kwargs = {"down_block_additional_residuals": down, "mid_block_additional_residual": mid}
-        eps = self.unet(latent_model_input, t, encoder_hidden_states=text, **kwargs).sample
-        return eps, batch_size
+        return self.unet(latent_model_input, t, encoder_hidden_states=text, **kwargs).sample
 
     # generate.py:281-311 (inversion=False branch)
     def pred_next_x(self, x: torch.Tensor, eps: torch.Tensor, i: int) -> torch.Tensor:
@@ -458,20 +516,30 @@ class ChunkedDenoiser(_Driver):
         """The chunk of frames lo..hi-1 of `x` (with those rows of the per-frame inputs `frames`) into the same rows of
         `out`: with `fused` its x_{t-1} by KS at the step index that step() set, else its noise prediction
         (pred_noise).  Fused, a UNet output of another dtype gets pred_noise's guidance combine in torch, rounded to
-        the latents' dtype as the torch path stores it, and KI's update of the same step."""
-        x, frames, out = x[lo:hi], _rows(frames, lo, hi), out[lo:hi]
+        the latents' dtype as the torch path stores it, and KI's update of the same step.  With K edits, KS (or KI)
+        runs once per edit on its rows and its slice of the UNet output."""
+        x, frames, out = self._frame_rows(x, lo, hi), _rows(frames, lo, hi), self._frame_rows(out, lo, hi)
         if not fused:
             out.copy_(self.pred_noise(x, t, **frames))
             return
         from . import ops
         coef, step = self.step_tables(x.device)
         eps, samples = self.unet_output(x, t, **frames)
-        if eps.dtype == torch.float16:
-            ops.cfg_ddim_update(x, eps.contiguous(), samples, self.guidance_scale, coef, step, out)
-            return
-        noise = self.guide(eps, samples).to(x.dtype)
-        out.copy_(x)
-        ops.ddim_update(out, noise.contiguous(), coef, step)
+        edits = [(x, eps, out)] if self.edits is None else list(zip(x, eps.chunk(self.edits), out))
+        for x, eps, out in edits:
+            if eps.dtype == torch.float16:
+                ops.cfg_ddim_update(x, eps.contiguous(), samples, self.guidance_scale, coef, step, out)
+                continue
+            noise = self._guide_edit(eps, samples).to(x.dtype)
+            out.copy_(x)
+            ops.ddim_update(out, noise.contiguous(), coef, step)
+
+    def _frame_rows(self, x: torch.Tensor, lo: int, hi: int) -> torch.Tensor:
+        """Frames lo..hi-1 of latents x: [flen, ...], or [K, flen, ...] with K edits."""
+        return x[lo:hi] if self.edits is None else x[:, lo:hi]
+
+    def _flen(self, x: torch.Tensor) -> int:
+        return x.shape[0 if self.edits is None else 1]
 
     def _step_chunks(self, flen: int) -> List[torch.Tensor]:
         chunks = self.get_chunks(flen)
@@ -514,33 +582,52 @@ class ChunkedDenoiser(_Driver):
             lanes.append(torch.cuda.Stream(device))
         return lanes[:n] if n > 1 else []
 
-    def _lane_edges(self, lanes: list):
-        """patch.LaneEdges over every merged block of the models, for a capture on `lanes` (None on one stream)."""
+    def _lane_edges(self, lanes: list, branches: Optional[dict] = None):
+        """patch.LaneEdges over every merged block of the models, for a capture on `lanes` (None on one stream), with
+        the side streams `branches` of _edit_branches."""
         if not lanes:
             return None
-        return patch.LaneEdges(m for model in self._models() for m in model.modules()
-                               if type(m).__name__ == "ToMeBlock")
+        return patch.LaneEdges((m for model in self._models() for m in model.modules()
+                                if type(m).__name__ == "ToMeBlock"), branches=branches)
 
-    def _lanes_fit(self, lanes: list, grids: List[int], device) -> bool:
+    def _edit_branches(self, device, lanes: list) -> dict:
+        """With K > 1 edits and `lanes`: {lane stream handle: K - 1 side streams}, on which a lane capture runs edits
+        1..K-1 of each merged block (their merge paths do not depend on each other), made once per driver and device
+        before any capture.  Empty without lanes, with one edit, or once _branch_edits is off."""
+        K = getattr(self, "edits", None) or 1
+        if K < 2 or not lanes or not self._branch_edits:
+            return {}
+        made = self._branches.setdefault(device, {})
+        for lane in lanes:
+            side = made.setdefault(lane.cuda_stream, [])
+            while len(side) < K - 1:
+                side.append(torch.cuda.Stream(device))
+        return {lane.cuda_stream: made[lane.cuda_stream][:K - 1] for lane in lanes}
+
+    def _lanes_fit(self, lanes: list, grids: List[int], device, per_lane: int = 1) -> bool:
         """Whether the KB1 sorts of a capture on `lanes` (their CTA counts `grids`) can all be resident together:
         a sort of at most ops.sort_co_resident CTAs is one launch whose CTAs wait for each other at spin barriers, so
-        the sorts that several lanes may run at once must fit on the device side by side."""
+        the sorts that several lanes, each with `per_lane` concurrent branches, may run at once must fit on the device
+        side by side."""
         from . import ops
         cap = ops.sort_co_resident(device)
-        return len(lanes) * max([c for c in grids if c <= cap], default=0) <= cap
+        return len(lanes) * per_lane * max([c for c in grids if c <= cap], default=0) <= cap
 
     def _record(self, x: torch.Tensor, t: torch.Tensor, frames: dict, spans: List[tuple], *, fused: bool,
                 first: bool, key: tuple, phase: tuple) -> _Graph:
         """Capture the chunks `spans` ((lo, hi) rows) of inputs shaped like `x`, with its per-frame inputs `frames` and
         the UNet's timestep input `t`, into one graph: chunk k by _chunk_into on lane k % LANES (run_on_lanes).  The
         global tokens start as at the first chunk of a step (`first`: none) or at a later one (the stores' tokens).
-        When the KB1 sorts of the lanes would not fit on the device together, it captures again on one stream.  Called
+        With K edits, the K merge paths of each merged block run on branches of the lane (_edit_branches).  When the
+        KB1 sorts of the lanes and branches would not fit on the device together, it captures again without the
+        branches, then on one stream.  Called
         after the eager warm-up steps, so that every lazily created piece of state — generators forked by the hook,
         cached packed weights, the library handle, allocator pools — already exists."""
         from . import ops
         gx = x.clone()
         gframes = {k: v.clone() for k, v in frames.items()}                # the per-frame inputs, set per replay
         lanes = self._lane_streams(x.device, len(spans))
+        branches = self._edit_branches(x.device, lanes)
         graph = torch.cuda.CUDAGraph()
         for g in self._block_generators():
             graph.register_generator_state(g)
@@ -552,9 +639,12 @@ class ChunkedDenoiser(_Driver):
         with ops.recording_sort_grids() as grids, torch.cuda.graph(graph):
             out = torch.empty_like(gx) if fused else torch.zeros_like(gx)
             run_on_lanes(len(spans), lanes, lambda k: self._chunk_into(gx, t, gframes, out, *spans[k], fused),
-                         self._lane_edges(lanes))
-        if not self._lanes_fit(lanes, grids, x.device):
-            self._lane_count = 1
+                         self._lane_edges(lanes, branches))
+        if not self._lanes_fit(lanes, grids, x.device, 1 + max(map(len, branches.values()), default=0)):
+            if branches:
+                self._branch_edits = False
+            else:
+                self._lane_count = 1
             return self._record(x, t, frames, spans, fused=fused, first=first, key=key, phase=phase)
         return _Graph(graph=graph, x=gx, t=t, out=out, key=key, frames=gframes, fused=fused, phase=phase)
 
@@ -568,15 +658,16 @@ class ChunkedDenoiser(_Driver):
                                f"{patch.GLOBAL_EXCHANGE!r}): the cross-rank exchange is not captured")
         self._graph = None                                                   # release the previous graph first
         cs = self.chunk_size
-        spans = ([(lo, lo + cs) for lo in range(0, len(x), cs)] if self.capture_global
-                 else _spans(self._step_chunks(len(x))))
+        flen = self._flen(x)
+        spans = ([(lo, lo + cs) for lo in range(0, flen, cs)] if self.capture_global
+                 else _spans(self._step_chunks(flen)))
         gt = torch.tensor(int(t), device=x.device, dtype=torch.long)      # the UNet's timestep input, set per replay
         graph = self._record(x, gt, frames, spans, fused=self._fuses_update(x), first=True,
                              key=self._graph_key(x, t), phase=self._phase(t))
         if self.capture_global:
             # the pinned buffer is rewritten only after its last upload has run (the event)
-            graph = graph._replace(slots=(torch.empty((2, len(x)), dtype=torch.int64, device=x.device),
-                                          torch.empty((2, len(x)), dtype=torch.int64).pin_memory(),
+            graph = graph._replace(slots=(torch.empty((2, flen), dtype=torch.int64, device=x.device),
+                                          torch.empty((2, flen), dtype=torch.int64).pin_memory(),
                                           torch.cuda.Event()))
         self._graph = graph
 
@@ -599,7 +690,8 @@ class ChunkedDenoiser(_Driver):
         whether that is x_{t-1} rather than the noise prediction (a graph replays the path it was captured with).
         With capture_global the step still draws its chunk order on the host with get_chunks, as eager stepping does,
         and applies it as data: one index_select of the inputs into the slots, one of the output back."""
-        flen = len(x)
+        flen = self._flen(x)
+        fd = 0 if self.edits is None else 1                           # the latents' frame dim
         if self.capture_global:
             if flen % self.chunk_size != 0:
                 raise RuntimeError(f"capture_global=True needs a frame count divisible by chunk_size (got {flen} "
@@ -619,13 +711,13 @@ class ChunkedDenoiser(_Driver):
             index_host.copy_(order)
             index.copy_(index_host, non_blocking=True)
             copied.record()
-            torch.index_select(x, 0, index[0], out=g.x)                # latents -> slots
+            torch.index_select(x, fd, index[0], out=g.x)               # latents -> slots
             for k, v in g.frames.items():
                 torch.index_select(frames[k], 0, index[0], out=v)
         g.t.fill_(int(t))
         g.graph.replay()
         if g.slots is not None:
-            return torch.index_select(g.out, 0, index[1]), g.fused     # slots -> frames
+            return torch.index_select(g.out, fd, index[1]), g.fused    # slots -> frames
         return (g.out.clone() if g.fused else g.out), g.fused           # the next replay rewrites out
 
     @staticmethod
@@ -677,8 +769,9 @@ class ChunkedDenoiser(_Driver):
         for model in self._models():
             for m in model.modules():
                 if type(m).__name__ == "ToMeBlock":
-                    m.global_tokens = patch.GlobalTokenStore(self.chunk_size)
-                    self._stores.append(m.global_tokens)
+                    stores = [patch.GlobalTokenStore(self.chunk_size) for _ in range(patch.edits_of(m))]
+                    m.global_tokens = stores[0] if len(stores) == 1 else stores       # one per edit
+                    self._stores.extend(stores)
 
     def _reset_global(self):
         if self._stores:
@@ -692,7 +785,7 @@ class ChunkedDenoiser(_Driver):
     def _chunk_graph_step(self, x: torch.Tensor, t: int, frames: dict, fused: bool) -> torch.Tensor:
         """Replay the graph of every chunk of the step on its rows, capturing it first when its key is new; returns the
         step's x_{t-1} with `fused` (the graphs are keyed by it), else its noise prediction."""
-        flen = len(x)
+        flen = self._flen(x)
         chunks = self.get_chunks(flen)                                      # the same host draws as eager stepping
         if not self._chunk_graphs:
             self._check_chunk_lengths(flen)                                 # before anything is captured
@@ -705,30 +798,37 @@ class ChunkedDenoiser(_Driver):
             self._chunk_t = torch.tensor(int(t), device=x.device, dtype=torch.long)
         self._chunk_t.fill_(int(t))
         out = torch.empty_like(x)
+        # the shape of a frame, and with K edits K
+        shape = tuple(x.shape[1:]) if self.edits is None else (self.edits,) + tuple(x.shape[2:])
         for k, (lo, hi) in enumerate(_spans(chunks)):
             first = self.merge_global and k == 0        # whether the blocks' stores are empty when the chunk runs
-            key = (hi - lo, first, tuple(x.shape[1:])) + phase + (fused,)
+            key = (hi - lo, first, shape) + phase + (fused,)
+            rows = self._frame_rows(x, lo, hi)
             g = self._chunk_graphs.get(key)
             if g is None:
-                g = self._chunk_graphs[key] = self._record(x[lo:hi], self._chunk_t, _rows(frames, lo, hi),
+                g = self._chunk_graphs[key] = self._record(rows, self._chunk_t, _rows(frames, lo, hi),
                                                            [(0, hi - lo)], fused=fused, first=first, key=key,
                                                            phase=phase)
-            g.x.copy_(x[lo:hi])
+            g.x.copy_(rows)
             for name, v in g.frames.items():
                 v.copy_(frames[name][lo:hi])
             g.graph.replay()
-            out[lo:hi].copy_(g.out)
+            self._frame_rows(out, lo, hi).copy_(g.out)
         return out
 
     # one iteration of generate.py:211-224
     @torch.no_grad()
     def step(self, x: torch.Tensor, i: int) -> torch.Tensor:
+        """One denoising step of latents x [flen, 4, h, w], or [K, flen, 4, h, w] with K edits."""
+        if self.edits is not None and (x.dim() != 5 or x.shape[0] != self.edits):
+            raise ValueError(f"latents of {self.edits} edits must be [{self.edits}, flen, C, h, w] "
+                             f"(got {tuple(x.shape)})")
         t = self.timesteps[i]
         frames = {}                                                          # the per-frame inputs, cast to x's dtype
         if self.source_latents is not None:                                 # generate.py:226-231 (pre_iter)
             pnp.register_time(self.unet, t, modules=self._pnp_targets)
             frames["src"] = self.source_latents(t).to(x)
-        frames = self._frames(x, frames)
+        frames = self._frames(x if self.edits is None else x[0], frames)    # shared by every edit
         if self.chunk_graphs and self.merge_global and x.is_cuda and not self._stores:
             self._install_stores()
         fused = self._fuses_update(x)
@@ -737,7 +837,7 @@ class ChunkedDenoiser(_Driver):
         if not (self.cuda_graph and x.is_cuda and self._eager_steps >= self.graph_warmup):
             self._eager_steps += 1
             out = torch.empty_like(x) if fused else torch.zeros_like(x)
-            for lo, hi in _spans(self._step_chunks(len(x))):
+            for lo, hi in _spans(self._step_chunks(self._flen(x))):
                 self._chunk_into(x, t, frames, out, lo, hi, fused)
         elif self.chunk_graphs:
             out = self._chunk_graph_step(x, t, frames, fused)
@@ -750,6 +850,10 @@ class ChunkedDenoiser(_Driver):
 
     @torch.no_grad()
     def sample(self, x: torch.Tensor) -> torch.Tensor:
+        """Every step from x.  With K edits, x [flen, 4, h, w] starts every edit (the reference's one init_noise for
+        all prompts); [K, flen, 4, h, w] gives each its own."""
+        if self.edits is not None and x.dim() == 4:
+            x = x.expand(self.edits, *x.shape).contiguous()
         for i in range(len(self.timesteps)):
             x = self.step(x, i)
         return x

@@ -107,6 +107,93 @@ _UNMERGED = 0
 # The LaneEdges of the lane capture in progress (lane_edges), else None.
 _LANE_EDGES = None
 
+# The SharedDraws of the multi-edit block call in progress (_for_each_edit), else None; and the edit it is running.
+_SHARED_DRAWS = None
+_EDIT = None
+
+
+class SharedDraws:
+    """The draws of one block call of a multi-edit batch (update_patch(edits=K)): the first edit issues them from the
+    block's generator and every later edit is handed the same values in the same order.  Every draw of the merge path
+    is data-independent (one randint per local level, one coin per global stage), so edit k then builds the plan a
+    single-edit run builds from the same generator state, and the generator advances once per call whatever K is."""
+
+    def __init__(self, streams: bool = False):
+        self.values: List[Any] = []
+        self.events: List[Any] = []
+        self.next: Optional[int] = None        # None while the first edit draws, else the next value to hand back
+        self.streams = streams                 # edits run on streams of their own (LaneEdges.edit_streams)
+
+    def take(self, draw: Callable[[], Any]):
+        if self.next is None:
+            value = draw()
+            self.values.append(value)
+            event = None
+            if self.streams and isinstance(value, torch.Tensor) and value.is_cuda:
+                event = torch.cuda.Event()                  # a device draw: other edits read it after it is made
+                event.record()
+            self.events.append(event)
+            return value
+        if self.next >= len(self.values):
+            raise RuntimeError("multi-edit merge: an edit drew more than the first edit did")
+        value, event = self.values[self.next], self.events[self.next]
+        if event is not None:
+            stream = torch.cuda.current_stream()
+            stream.wait_event(event)
+            value.record_stream(stream)
+        self.next += 1
+        return value
+
+    def rewind(self) -> None:
+        """Start handing the first edit's draws back, from the first one."""
+        if self.next is not None and self.next != len(self.values):
+            raise RuntimeError("multi-edit merge: an edit drew less than the first edit did")
+        self.next = 0
+
+
+def _draw(draw: Callable[[], Any]):
+    """draw(), or with edits sharing their draws (_for_each_edit) the shared value."""
+    return draw() if _SHARED_DRAWS is None else _SHARED_DRAWS.take(draw)
+
+
+def _for_each_edit(module: torch.nn.Module, x: torch.Tensor, edits: int, batch_size: int, streams: bool = False):
+    """(k, rows of edit k) for the edit-major batch `x` of a block patched for K edits (update_patch(edits=K)): K equal
+    slices, each the batch a single-edit run gives the block.  While edit k runs, `module.global_tokens` is that
+    edit's own (a list of K entries between calls; None stands for K Nones), the block's draws are shared
+    (SharedDraws; `streams`: the edits run on streams of their own) and a lane capture's recurrence edges are edit k's
+    (LaneEdges)."""
+    global _SHARED_DRAWS, _EDIT
+    batch = edits * batch_size
+    if x.shape[0] % batch:
+        raise ValueError(f"multi-edit merge: {x.shape[0]} samples are not {edits} edits of batch_size "
+                         f"{batch // edits} x frames")
+    n = x.shape[0] // edits
+    g = getattr(module, "global_tokens", None)
+    tokens = [None] * edits if g is None else g
+    if not isinstance(tokens, list) or len(tokens) != edits:
+        raise ValueError(f"multi-edit merge: global_tokens must be None or a list of {edits} entries, one per edit "
+                         f"(got {type(g).__name__})")
+    (prev, prev_edit), _SHARED_DRAWS = (_SHARED_DRAWS, _EDIT), SharedDraws(streams)
+    try:
+        for k in range(edits):
+            module.global_tokens, _EDIT = tokens[k], k
+            yield k, x[k * n:(k + 1) * n]
+            tokens[k] = module.global_tokens
+            _SHARED_DRAWS.rewind()
+    finally:
+        _SHARED_DRAWS, _EDIT = prev, prev_edit
+        module.global_tokens = None if all(t is None for t in tokens) else tokens
+
+
+def _tome_args(module: torch.nn.Module) -> Dict[str, Any]:
+    return module._tome_info["args"]
+
+
+def edits_of(module: torch.nn.Module) -> int:
+    """The `edits` a patched module was patched with (apply_patch), 1 for any other module."""
+    info = getattr(module, "_tome_info", None)
+    return 1 if info is None else int(info["args"].get("edits", 1))
+
 
 class LaneEdges:
     """The global-token recurrence as the only edge between the chunks of a step captured on several streams ("lanes",
@@ -117,34 +204,51 @@ class LaneEdges:
     writer's stream while the reader may still copy them.  `event` and `current_stream` are the CUDA ones; they can be
     replaced by stand-ins."""
 
-    def __init__(self, modules: Iterable[torch.nn.Module], event: Callable = None, current_stream: Callable = None):
+    def __init__(self, modules: Iterable[torch.nn.Module], event: Callable = None, current_stream: Callable = None,
+                 branches: Optional[Dict[int, list]] = None):
         self._event = event or torch.cuda.Event
         self._current_stream = current_stream or torch.cuda.current_stream
-        self.events: Dict[int, Any] = {}
-        self.recorded = set()                  # ids of the modules whose event some chunk has recorded
+        self.events: Dict[Any, Any] = {}
+        self.recorded = set()                  # keys of the events some chunk has recorded
+        # a lane's stream handle -> the side streams the edits 1..K-1 of a multi-edit block call branch to
+        self.branches = branches or {}
         for m in modules:
             if id(m) not in self.events:
                 self.events[id(m)] = self._event()
 
+    def _key(self, module):
+        """The recurrence a global stage belongs to: the module's, and with several edits (_for_each_edit) the edit's
+        within it, so that edit k of a chunk waits only on edit k of the previous chunk."""
+        return id(module) if _EDIT is None else (id(module), _EDIT)
+
     def _of(self, module):
-        ev = self.events.get(id(module))
-        if ev is None:
+        if id(module) not in self.events:
             raise RuntimeError(f"lane capture: {type(module).__name__} has no recurrence event; every merged block of "
                                f"the captured models must be given one")
-        return ev
+        key = self._key(module)
+        if key not in self.events:
+            self.events[key] = self._event()
+        return self.events[key]
 
     def wait(self, module, tokens) -> None:
         """Before `module` reads `tokens`, its stored global tokens: order the read after the previous chunk's store."""
         ev = self._of(module)
         stream = self._current_stream()
-        if id(module) in self.recorded:
+        if self._key(module) in self.recorded:
             stream.wait_event(ev)
         tokens.record_stream(stream)
 
     def record(self, module) -> None:
         """After `module` stored its global tokens: the next chunk's read of them waits on this."""
         self._of(module).record(self._current_stream())
-        self.recorded.add(id(module))
+        self.recorded.add(self._key(module))
+
+    def edit_streams(self, edits: int) -> Optional[list]:
+        """The streams the `edits` edits of a block call run on inside this capture: the current stream for edit 0 and
+        side streams of its own for the others, or None when none were made for the current stream."""
+        main = self._current_stream()
+        side = self.branches.get(main.cuda_stream, [])
+        return [main] + side[:edits - 1] if len(side) >= edits - 1 else None
 
 
 @contextlib.contextmanager
@@ -283,7 +387,7 @@ def _global_stage_store(module, store: GlobalTokenStore, table, mu, pi, ln, args
         local = ops.gather_rows(table, mu, ln=ln)
         store.write(local)
         return local, pi, None, None
-    coin = draw_coin(module.generator, on_device=True)                      # patch.py:62
+    coin = _draw(lambda: draw_coin(module.generator, on_device=True))      # patch.py:62
     gratio = args["global_merge_ratio"]
     if gratio <= 0:
         raise ValueError("not enough values to unpack (expected 3, got 2)")  # as the host-coin path
@@ -323,7 +427,7 @@ def _global_stage_device_coin(module, table, mu, pi, g, ln, args, levels):
     Returns (merged tokens, composed unmerge map, coin tensor)."""
     B, _, C = table.shape
     L = mu.shape[1]
-    coin = draw_coin(module.generator, on_device=True)                      # patch.py:62
+    coin = _draw(lambda: draw_coin(module.generator, on_device=True))      # patch.py:62
     gratio = args["global_merge_ratio"]
     if gratio <= 0:
         raise ValueError("not enough values to unpack (expected 3, got 2)")  # as the host-coin path
@@ -388,7 +492,7 @@ def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[s
         else:
             stride = min(args["target_stride"], curF)                        # merge.py:55
             _check_progress(stride)
-            randf = draw_randf(generator, stride, curF)                      # merge.py:56-57
+            randf = _draw(lambda: draw_randf(generator, stride, curF))      # merge.py:56-57
             randfs.append(randf)
             split = VtmSplit.local(L, unm, curF, args["target_stride"], randf)
             m = merge.match_level(table, mu, split, ratio, align, ln)        # patch.py:45-46
@@ -447,7 +551,7 @@ def build_merge_plan(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[s
         if local_tokens is None:
             local_tokens = ops.gather_rows(table, mu, ln=ln)                 # merged local tokens [B, L, C]
         if g is not None:                                                    # patch.py:60
-            coin = draw_coin(generator, on_device=False)                     # patch.py:62
+            coin = _draw(lambda: draw_coin(generator, on_device=False))     # patch.py:62
             g = g.to(local_tokens).contiguous()                              # patch.py:65,70
             Lg = g.shape[1]
             if coin_above(coin, args["global_rand"]):                        # in fp32, as torch compares
@@ -488,6 +592,9 @@ def compute_merge(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[str,
     """Reference signature and return triple (patch.py:14,91): (merge op, unmerge op, merged tokens).
     The merge op is returned for interface parity only — like the reference's diffusers block
     (patch.py:149-152) nothing here calls it: the merged tokens are already the third element."""
+    edits = tome_info["args"].get("edits", 1)
+    if edits > 1:
+        return _compute_merge_per_edit(module, x, tome_info, edits)
     plan = build_merge_plan(module, x, tome_info)
     if plan is None:
         return merge.do_nothing, merge.do_nothing, x                         # patch.py:86-88
@@ -498,6 +605,23 @@ def compute_merge(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[str,
     def u(y: torch.Tensor, **kwarg) -> torch.Tensor:
         return plan.unmerge(y)
     m.plan = u.plan = plan
+    return m, u, merged
+
+
+def _compute_merge_per_edit(module: torch.nn.Module, x: torch.Tensor, tome_info: Dict[str, Any], edits: int):
+    """compute_merge on an edit-major batch of `edits` edits: one plan per edit on its own rows (_for_each_edit), the
+    merged tokens of the edits stacked in edit order, and an unmerge that takes each edit's rows back with its plan."""
+    with contextlib.closing(_for_each_edit(module, x, edits, tome_info["args"]["batch_size"])) as slices:     # its state is restored on an error too
+        plans = [build_merge_plan(module, rows, tome_info) for _, rows in slices]
+    if plans[0] is None:
+        return merge.do_nothing, merge.do_nothing, x                         # patch.py:86-88
+    merged = torch.cat([p.merged_tokens for p in plans])
+
+    def m(_x: torch.Tensor, **kwarg) -> torch.Tensor:
+        return merged
+    def u(y: torch.Tensor, **kwarg) -> torch.Tensor:
+        return torch.cat([p.unmerge(rows) for p, rows in zip(plans, y.chunk(edits))])
+    m.plans = u.plans = plans
     return m, u, merged
 
 
@@ -535,10 +659,58 @@ def _pnp_shared_items(attn: torch.nn.Module, batch: int) -> Optional[int]:
     return 0 if batch % num_inputs else batch // num_inputs
 
 
+def _reference_pnp_forward(attn: torch.nn.Module) -> bool:
+    """True if `attn` carries a PnP forward other than pnp.py's: the reference's own closure (utils/pnp_utils.py:99-101),
+    which takes the source sample's Q/K by position over the whole batch (`q[:B // num_inputs]`)."""
+    override = vars(attn).get("forward")
+    return (override is not None and not getattr(override, "_vtm_pnp_forward", False)
+            and hasattr(attn, "injection_schedule"))
+
+
 def _self_attention_stage(block, hidden_states, attention_mask, encoder_hidden_states, timestep, class_labels,
                           cross_attention_kwargs):
     """norm1 -> [merge] -> attn1 -> [unmerge] + residual (patch.py:139-169).  Returns the hidden states and, for an
-    AdaNorm-zero norm1, its (shift_mlp, scale_mlp, gate_mlp) for the feed-forward, else None."""
+    AdaNorm-zero norm1, its (shift_mlp, scale_mlp, gate_mlp) for the feed-forward, else None.  A block patched with
+    edits=K > 1 (update_patch) runs the stage once per edit on that edit's rows (_for_each_edit): its own merge plan,
+    global tokens and PnP source sample, with the draws shared.  Inside a lane capture whose LaneEdges has side streams
+    for the current lane, edit k runs on a branch of its own, forked from the lane and joined back into it, since the
+    edits' merge paths do not depend on each other."""
+    edits = 1 if _UNMERGED > 0 or block._vtm_unmerged else _tome_args(block).get("edits", 1)
+    if edits == 1:
+        return _edit_self_attention(block, hidden_states, attention_mask, encoder_hidden_states, timestep,
+                                    class_labels, cross_attention_kwargs)
+    if block.use_ada_layer_norm or block.use_ada_layer_norm_zero:
+        raise ValueError("update_patch(edits > 1): blocks with an AdaNorm norm1 are not supported")
+    if _reference_pnp_forward(block.attn1):
+        raise ValueError("update_patch(edits > 1): attn1 carries the reference's PnP forward, which takes the source "
+                         "sample by position over the whole batch; register PnP with vidtome_b200.pnp instead")
+    B = hidden_states.shape[0]
+    per_edit = lambda t, k: t[k * (B // edits):(k + 1) * (B // edits)] if (   # noqa: E731
+        isinstance(t, torch.Tensor) and t.dim() > 0 and t.shape[0] == B) else t
+    out = torch.empty_like(hidden_states)
+    streams = _LANE_EDGES.edit_streams(edits) if _LANE_EDGES is not None and hidden_states.is_cuda else None
+    for s in streams[1:] if streams else ():
+        s.wait_stream(streams[0])                                              # fork from the lane
+    try:
+        with contextlib.closing(_for_each_edit(block, hidden_states, edits, _tome_args(block)["batch_size"],
+                                                    streams is not None)) as slices:
+            for k, rows in slices:                                             # state restored on an error too
+                with torch.cuda.stream(streams[k]) if streams else contextlib.nullcontext():
+                    if streams and k:
+                        hidden_states.record_stream(streams[k])
+                        out.record_stream(streams[k])
+                    out[k * len(rows):(k + 1) * len(rows)], _ = _edit_self_attention(
+                        block, rows, per_edit(attention_mask, k), per_edit(encoder_hidden_states, k), timestep,
+                        class_labels, cross_attention_kwargs)
+    finally:
+        for s in streams[1:] if streams else ():
+            streams[0].wait_stream(s)                                          # join into the lane
+    return out, None
+
+
+def _edit_self_attention(block, hidden_states, attention_mask, encoder_hidden_states, timestep, class_labels,
+                         cross_attention_kwargs):
+    """_self_attention_stage on the batch of one edit."""
     unmerged = _UNMERGED > 0 or block._vtm_unmerged
     only_cross = getattr(block, "only_cross_attention", False)
 
@@ -868,6 +1040,8 @@ def apply_patch(
      - max_downsample: merge only in layers with at most this downsampling (1, 2, 4 or 8).
      - seed: stored, unused (as in the reference).   - batch_size: number of video chunks per pass (2 = CFG, 3 = PnP).
      - align_batch: share one matching across the batch (PnP).   - target_stride: one target frame per this many frames.
+    Several edits of one video in one call (not in the reference) are set afterwards with
+    `update_patch(model, edits=K)`.
     """
     # start from an unpatched model: a second apply_patch must not stack hooks or subclasses
     remove_patch(model)
@@ -963,14 +1137,30 @@ def update_patch(model: torch.nn.Module, **kwargs):
     """Set attributes on every module that carries `_tome_info` (the UNet, each patched block and — on a
     pipeline that has one — the ControlNet and its blocks), e.g. `update_patch(pipe, global_tokens=None)`
     after each denoising step (patch.py:358-370, generate.py:233-236).  Like the reference, the return
-    value is the last root walked (its loop variable shadows `model`), not the object passed in."""
+    value is the last root walked (its loop variable shadows `model`), not the object passed in.
+
+    `edits=K` (not in the reference) is a patch argument rather than an attribute: it goes to
+    `_tome_info["args"]["edits"]` (absent means 1).  Every call then carries K edits of one video, edit-major: the batch
+    is K slices of batch_size * frames samples, each the batch a single-edit run gives the block.  Every edit gets its
+    own merge plans and global tokens (a list of K entries in `global_tokens`), and all edits share each draw
+    (SharedDraws).  With edits=1 every block takes the single-edit path."""
     roots = _roots_of(model, model)                      # `.controlnet` is looked up on the object passed in
+    edits = kwargs.pop("edits", None)
+    if edits is not None:
+        _check_edits(edits)
     for root in roots:
         for _, module in root.named_modules():
             if hasattr(module, "_tome_info"):
+                if edits is not None:                    # a patch argument (apply_patch), not a module attribute
+                    module._tome_info["args"]["edits"] = edits
                 for key, value in kwargs.items():
                     setattr(module, key, value)
     return roots[-1]
+
+
+def _check_edits(edits) -> None:
+    if isinstance(edits, bool) or not isinstance(edits, int) or edits < 1:
+        raise ValueError(f"edits must be a positive int (got {edits!r})")
 
 
 def collect_from_patch(model: torch.nn.Module, attr="tome"):

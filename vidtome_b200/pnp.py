@@ -19,7 +19,7 @@ model (the skeleton) must pass the attention modules explicitly through `modules
 """
 from __future__ import annotations
 
-from typing import Iterable, Optional, Sequence
+from typing import Callable, Iterable, Optional, Sequence
 
 import torch
 
@@ -216,22 +216,46 @@ def conv_library_forward(resnet: torch.nn.Module, input_tensor: torch.Tensor, te
     return ops.resnet_tail(h, shortcut, num_inputs, resnet.output_scale_factor, inject)
 
 
-def _conv_forward(resnet: torch.nn.Module, num_inputs: int):
-    def forward(input_tensor, temb=None, **kwargs):
+def _conv_forward(resnet: torch.nn.Module, num_inputs: int, edits_of: Callable[[], int]):
+    def one_edit(input_tensor, temb):
         if conv_eligible(resnet, input_tensor, temb):
             return conv_library_forward(resnet, input_tensor, temb)
         return _conv_torch_forward(resnet, num_inputs, input_tensor, temb)
+
+    def forward(input_tensor, temb=None, **kwargs):
+        edits = 1 if patch.unmerged_active() else edits_of()            # inversion runs frame batches, not edits
+        if edits == 1:
+            return one_edit(input_tensor, temb)
+        # an edit-major batch: each edit's slice is the batch of a single-edit run, with its own source samples
+        B = input_tensor.shape[0]
+        if B % edits:
+            raise ValueError(f"PnP conv injection: a batch of {B} samples is not {edits} edits")
+        n = B // edits
+        rows = lambda t, k: t[k * n:(k + 1) * n] if t is not None and t.shape[0] == B else t   # noqa: E731
+        return torch.cat([one_edit(rows(input_tensor, k), rows(temb, k)) for k in range(edits)])
 
     forward._vtm_pnp_conv_forward = True
     return forward
 
 
 def register_conv_control(model, injection_schedule: Optional[Sequence[int]], num_inputs: int,
-                          modules: Optional[Iterable[torch.nn.Module]] = None):
+                          modules: Optional[Iterable[torch.nn.Module]] = None, edits: Optional[int] = None):
     """Same call as the reference's (utils/pnp_utils.py:108): mark `unet.up_blocks[1].resnets[1]` (or `modules`) for
-    source-sample conv-feature injection during the timesteps in `injection_schedule`."""
+    source-sample conv-feature injection during the timesteps in `injection_schedule`.  `edits` (not in the reference)
+    is the number of edits of an edit-major batch: each ResNet call then runs once per edit's slice, so that every
+    edit takes its own source samples' features.  By default it is read at every call from what `model` is patched
+    with (patch.edits_of, so update_patch(edits=K) may come before or after this call); inside inversion
+    (patch._unmerged_blocks) the batch is always one run's."""
+    if edits is not None:
+        patch._check_edits(edits)
+    root = None if model is None else (model.unet if hasattr(model, "unet") else model)
+
+    def edits_of() -> int:
+        if edits is not None:
+            return edits
+        return 1 if root is None else patch.edits_of(root)
     for resnet in _conv_targets(model, modules):
-        resnet.forward = _conv_forward(resnet, int(num_inputs))
+        resnet.forward = _conv_forward(resnet, int(num_inputs), edits_of)
         resnet.injection_schedule = injection_schedule
         resnet._vtm_pnp_conv = int(num_inputs)
     return model
