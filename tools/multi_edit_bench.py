@@ -21,6 +21,16 @@ private memory pools.  One JSON line per workload goes to stdout, with the card'
 read in the same run.
 
     python tools/multi_edit_bench.py --workloads dog c3 --edits 2 4
+
+--shard runs the edits split over the ranks of a torch.distributed job instead (ChunkedDenoiser(cond=[K, ...],
+shard=True): rank r runs edits k % world == r).  Start it with torchrun, one rank per GPU; every rank builds two arms
+per edit count K, the unsharded K-edit run and its sharded share of the edits, steps both --check-steps times from the
+same RNG state (reporting max |x - unsharded| / max |unsharded| over its own edits), then times --rounds rounds of
+--steps steps each, the ranks aligned by a barrier before every round.  Each rank prints one JSON line per workload and
+K with its steps/s in both arms.  With one rank the two arms run the same K edits, so the line shows what the sharded
+path costs on its own; the speed-up over N GPUs is that of N ranks' lines.
+
+    torchrun --nproc-per-node 4 tools/multi_edit_bench.py --shard --workloads dog --edits 4
 """
 from __future__ import annotations
 
@@ -42,8 +52,10 @@ WORKLOADS = ("dog", "c3")
 MAX_EDITS = 4
 
 
-def make(workload: str, K: int, edit: int = 0):
+def make(workload: str, K: int, edit: int = 0, shard: bool = False):
+    """The arm of K edits (K = 1: the single-prompt run of edit `edit`); with `shard` this rank's share of K edits."""
     import vidtome_b200
+    from vidtome_b200 import dist as vd
     from vidtome_b200.driver import ChunkedDenoiser
     from vidtome_b200.skeleton import make_skeleton, pnp_attention_modules, pnp_conv_module
     torch.manual_seed(123)
@@ -51,7 +63,7 @@ def make(workload: str, K: int, edit: int = 0):
     net = make_skeleton("sd21" if dog else "sd15", hot_path_only=False, device="cuda", pnp_conv=dog)
     vidtome_b200.apply_patch(net, local_merge_ratio=0.9, merge_global=True, global_merge_ratio=0.8, global_rand=0.5,
                              batch_size=3 if dog else 2, align_batch=dog)
-    vidtome_b200.update_patch(net, edits=K)
+    vidtome_b200.update_patch(net, edits=len(vd.shard_edits(K)) if shard else K)
     gc = torch.Generator(device="cuda").manual_seed(5)
     cond = torch.randn((MAX_EDITS, 3 if dog else 2, 77, 1024 if dog else 768), generator=gc, device="cuda",
                        dtype=torch.float16)
@@ -68,7 +80,7 @@ def make(workload: str, K: int, edit: int = 0):
         kw = dict(chunk_graphs=True, randomize_chunks=True, source_latents=source, pnp_attn_t=0.5,
                   pnp_modules=pnp_attention_modules(net), pnp_f_t=0.8, pnp_conv_modules=[pnp_conv_module(net)])
     return ChunkedDenoiser(net, n_timesteps=N_STEPS, chunk_size=4, merge_global=True, chunk_ord="mix-4",
-                           cond=cond if K > 1 else cond[edit], cuda_graph=True, graph_warmup=2, **kw)
+                           cond=cond if K > 1 else cond[edit], cuda_graph=True, graph_warmup=2, shard=shard, **kw)
 
 
 def graph_pool_mib(den):
@@ -121,6 +133,38 @@ def run(workload: str, edits, rounds: int, steps: int, check_steps: int):
             "max_allocated_GiB": round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)}
 
 
+def run_shard(workload: str, K: int, rounds: int, steps: int, check_steps: int):
+    """This rank's steps/s of the unsharded K-edit run and of its share of the sharded one (see the module's doc)."""
+    import numpy as np
+    import torch.distributed as dist
+    from vidtome_b200 import dist as vd
+    rows = vd.shard_edits(K)
+    g = torch.Generator(device="cuda").manual_seed(123)
+    x0 = torch.randn((K, FRAMES, 4, LATENT, LATENT), generator=g, device="cuda", dtype=torch.float16)
+    end = 25 if workload == "dog" else N_STEPS
+    arms = {"unsharded": Chain(make(workload, K), x0, end=end),
+            "sharded": Chain(make(workload, K, shard=True), x0[rows], end=end)}
+    for ch in arms.values():
+        torch.manual_seed(2024)
+        np.random.seed(2024)
+        for _ in range(check_steps):
+            ch.step()
+    torch.cuda.synchronize()
+    ref = arms["unsharded"].x[rows].float()
+    diff = round(float((arms["sharded"].x.float() - ref).abs().max() / ref.abs().max()), 6)
+    rates = {name: [] for name in arms}
+    for _ in range(rounds):
+        for name, ch in arms.items():
+            dist.barrier()
+            rates[name].append(timed(ch, steps))
+    out = {"rank": vd.rank(), "world": vd.world(), "edits": K, "rank_edits": rows,
+           "rel_diff_to_unsharded": diff, "finite": bool(torch.isfinite(arms["sharded"].x).all())}
+    for name, r in rates.items():
+        r = sorted(r)
+        out[name] = {"steps_per_s_median": round(r[len(r) // 2], 2), "min": round(r[0], 2), "max": round(r[-1], 2)}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--workloads", nargs="+", choices=WORKLOADS, default=list(WORKLOADS))
@@ -129,12 +173,34 @@ def main():
     ap.add_argument("--rounds", type=int, default=5, help="rounds alternating the arms")
     ap.add_argument("--check-steps", type=int, default=6,
                     help="steps from the same RNG state before the comparison (2 eager + captures + replays)")
+    ap.add_argument("--shard", action="store_true", help="split the edits over the ranks of a torchrun job")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("multi_edit_bench.py needs a CUDA device")
     if any(not 1 < K <= MAX_EDITS for K in args.edits):
         raise SystemExit(f"--edits: counts from 2 to {MAX_EDITS}")
     name, power, clock = card()
+    if args.shard:
+        import torch.distributed as dist
+        local = int(os.environ.get("LOCAL_RANK", 0))
+        torch.cuda.set_device(local)
+        os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
+        os.environ.setdefault("MASTER_PORT", "29511")
+        dist.init_process_group("nccl", rank=int(os.environ.get("RANK", 0)),
+                                world_size=int(os.environ.get("WORLD_SIZE", 1)),
+                                device_id=torch.device("cuda", local))
+        try:
+            for w in args.workloads:
+                for K in args.edits:
+                    line = {"tool": "multi_edit_bench", "leg": "shard", "workload": w, "card": name,
+                            "power_limit": power, "max_sm_clock": clock, "frames": FRAMES, "latent": LATENT,
+                            "steps_per_round": args.steps, "rounds": args.rounds}
+                    line.update(run_shard(w, K, args.rounds, args.steps, args.check_steps))
+                    print(json.dumps(line), flush=True)
+                    torch.cuda.empty_cache()
+        finally:
+            dist.destroy_process_group()
+        return
     for w in args.workloads:
         torch.cuda.reset_peak_memory_stats()
         line = {"tool": "multi_edit_bench", "workload": w, "card": name, "power_limit": power,

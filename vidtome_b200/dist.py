@@ -17,10 +17,14 @@ tests).  Two cases:
 
 DDIM inversion and reconstruction (driver.ChunkedInverter(shard=True)) shard the frame batches (`shard_batches`):
 nothing crosses GPUs during the steps, and one all-gather at the end (`gather_batches`) gives every rank all frames.
+Generation of K edits (driver.ChunkedDenoiser(cond=[K, S, 77, D], shard=True), K > 1) shards the edits the same way
+(`shard_edits`, `gather_edits`): every rank makes the draws of the whole job, so each edit is what the unsharded run
+computes for it, with the reference's own global-token recurrence.  `check_ranks_agree` verifies up front that the ranks
+would draw alike.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Sequence, Tuple
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
@@ -84,6 +88,35 @@ def gather_batches(local: torch.Tensor, flen: int, batch_size: int, frame_dim: i
         for j, (lo, hi) in enumerate(shard_batches(flen, batch_size, r, w)):
             full.narrow(frame_dim, lo, hi - lo).copy_(out[r].narrow(frame_dim, j * batch_size, hi - lo))
     return full
+
+
+def shard_edits(K: int, rank_: Optional[int] = None, world_: Optional[int] = None) -> List[int]:
+    """The edits of a K-edit generation this rank runs: k with k % world == rank (the batches of one edit each of
+    shard_batches)."""
+    return [lo for lo, _ in shard_batches(K, 1, rank_, world_)]
+
+
+def gather_edits(local: torch.Tensor, K: int, group=None) -> torch.Tensor:
+    """Every rank's edits `local` [K_r, flen, ...] (its shard_edits, in order) as the full [K, flen, ...] in edit
+    order, on every rank: one all-gather of slabs padded to ceil(K / world) edits (gather_batches with batches of one
+    edit).  Without sharding (world 1) `local` is returned as it is."""
+    return gather_batches(local, K, 1, 0, group)
+
+
+def check_ranks_agree(entry: Dict[str, Any], group=None) -> None:
+    """Collective check before a job whose ranks must make the same draws: all-gathers every rank's `entry` (the same
+    keys on every rank) and raises ValueError on ALL ranks, naming the keys, when any value differs between ranks, so
+    that no rank is left waiting in a later collective."""
+    w = world()
+    if w == 1:
+        return
+    everyone = [None] * w
+    dist.all_gather_object(everyone, entry, group=group)
+    differ = [k for k in everyone[0] if any(e.get(k) != everyone[0][k] for e in everyone)]
+    if differ:
+        raise ValueError("vidtome_b200.dist: the ranks disagree on " + ", ".join(differ) + ": " +
+                         "; ".join(f"rank {r}: " + ", ".join(f"{k}={e.get(k)!r}" for k in differ)
+                                   for r, e in enumerate(everyone)))
 
 
 def check_step_lockstep(local_chunk_lens: Sequence[int], group=None) -> bool:

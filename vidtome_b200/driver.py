@@ -283,8 +283,17 @@ class ChunkedDenoiser(_Driver):
         and the per-frame inputs (source latents, control images, depth) are shared by all edits.  Edit k is the
         single-prompt run of cond[k] from the same RNG state: every draw (get_chunks, the blocks' randints and coins)
         is issued once per step, as by one run.  The model must be patched for K edits (apply_patch, then
-        update_patch(model, edits=K)); shard=True is refused with K > 1.  Every graph mode runs it; graph keys and
-        static buffers include K."""
+        update_patch(model, edits=K)).  Every graph mode runs it; graph keys and static buffers include K.
+
+        `shard=True` with K > 1 edits splits the edits over the ranks of an initialised torch.distributed job: rank r
+        runs the K_r edits k with k % world == r (dist.shard_edits) as a plain K_r-edit pass, with no chunk sharding, so
+        KS, lanes and every graph mode apply.  `cond` is the whole [K, S, 77, D] on every rank; the model is patched with
+        update_patch(model, edits=K_r).  step() takes and returns the rank's [K_r, flen, 4, h, w]; sample() takes
+        [K, flen, ...] (and keeps its rows), [K_r, flen, ...] or one [flen, ...] for all edits, and returns the gathered
+        [K, flen, 4, h, w] on every rank (dist.gather_edits).  Every rank makes the draws of the whole job, so each edit
+        is what the unsharded K-edit run computes for it: nothing crosses ranks during the steps.  sample() first checks
+        that the ranks agree on K, the latents' shape, the steps, the mode and the RNG states (dist.check_ranks_agree).
+        Needs world <= K and patch.GLOBAL_EXCHANGE == "recurrence"."""
         super().__init__(unet, controlnet, control_images, control_scale, depth, source_latents)
         # K for a [K, S, 77, D] cond (K edits, latents [K, flen, ...]), None for the single-prompt [S, 77, D]
         self.edits = None
@@ -293,15 +302,30 @@ class ChunkedDenoiser(_Driver):
                 raise ValueError(f"cond of several edits must be [K, S, 77, D] with S = 2 or 3 (got "
                                  f"{tuple(cond.shape)})")
             self.edits = int(cond.shape[0])
-        K = self.edits or 1
+        K = self.job_edits = self.edits or 1
+        # shard=True with K > 1 edits: this rank runs the edits dist.shard_edits(K) (their rows of cond) as a plain
+        # K_r-edit pass, with no chunk sharding; sample() gathers all K.  None otherwise.
+        self.edit_rows: Optional[List[int]] = None
         if shard and K > 1:
-            raise ValueError("shard=True does not run several edits (cond [K, S, 77, D] with K > 1)")
+            from . import dist as _dist
+            if not _dist.initialized():
+                raise ValueError("shard=True needs an initialised torch.distributed process group (one rank per process)")
+            if _dist.world() > K:
+                raise ValueError(f"shard=True with {K} edits needs at most {K} ranks (world size {_dist.world()}): "
+                                 f"the edits are split over the ranks")
+            self._check_edit_exchange()
+            self.edit_rows = _dist.shard_edits(K)
+            cond = cond[self.edit_rows]
+            self.edits = len(self.edit_rows)
+            shard = False
         for model in self._models():
-            if hasattr(model, "_tome_info") and patch.edits_of(model) != K:
-                raise ValueError(f"the model is patched with edits={patch.edits_of(model)}, the cond has {K} edit(s): "
-                                 f"set it with update_patch(model, edits={K})")
-        # shard=True: this process is one rank of a torch.distributed job and takes chunks i % world == rank of every
-        # step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
+            if hasattr(model, "_tome_info") and patch.edits_of(model) != (self.edits or 1):
+                runs = (f"this rank runs {self.edits} of the {K} edits" if self.edit_rows is not None
+                        else f"the cond has {K} edit(s)")
+                raise ValueError(f"the model is patched with edits={patch.edits_of(model)}, {runs}: set it with "
+                                 f"update_patch(model, edits={self.edits or 1})")
+        # shard=True (one edit): this process is one rank of a torch.distributed job and takes chunks i % world == rank
+        # of every step (dist.shard_chunks); with merge_global and a collective exchange mode the ranks are checked for
         # lock-step once per step (dist.check_step_lockstep)
         self.shard = bool(shard)
         self.cuda_graph = bool(cuda_graph)
@@ -379,7 +403,7 @@ class ChunkedDenoiser(_Driver):
         self.pnp_schedule = self.timesteps[:qk_t] if qk_t >= 0 else []
         pnp.register_attention_control(self.unet, self.pnp_schedule, num_inputs=3, modules=modules)
         self._pnp_targets = pnp._targets(self.unet, modules)
-        if (self.edits or 1) > 1:
+        if self.job_edits > 1:                  # on every rank of a sharded job, whatever its share of the edits
             for m in self.unet.modules():
                 f = vars(m).get("forward")
                 if (f is not None and hasattr(m, "injection_schedule") and not getattr(f, "_vtm_pnp_forward", False)
@@ -823,6 +847,8 @@ class ChunkedDenoiser(_Driver):
         if self.edits is not None and (x.dim() != 5 or x.shape[0] != self.edits):
             raise ValueError(f"latents of {self.edits} edits must be [{self.edits}, flen, C, h, w] "
                              f"(got {tuple(x.shape)})")
+        if self.edit_rows is not None:
+            self._check_edit_exchange()
         t = self.timesteps[i]
         frames = {}                                                          # the per-frame inputs, cast to x's dtype
         if self.source_latents is not None:                                 # generate.py:226-231 (pre_iter)
@@ -851,12 +877,56 @@ class ChunkedDenoiser(_Driver):
     @torch.no_grad()
     def sample(self, x: torch.Tensor) -> torch.Tensor:
         """Every step from x.  With K edits, x [flen, 4, h, w] starts every edit (the reference's one init_noise for
-        all prompts); [K, flen, 4, h, w] gives each its own."""
+        all prompts); [K, flen, 4, h, w] gives each its own.  With the edits sharded (shard=True, K > 1) x may also be
+        the rank's [K_r, flen, 4, h, w], and every rank returns all K edits."""
+        if self.edit_rows is not None:
+            self._check_edit_lockstep(x)
+            if x.dim() == 5 and x.shape[0] == self.job_edits:
+                x = x[self.edit_rows]
         if self.edits is not None and x.dim() == 4:
             x = x.expand(self.edits, *x.shape).contiguous()
         for i in range(len(self.timesteps)):
             x = self.step(x, i)
+        if self.edit_rows is not None:
+            from . import dist as _dist
+            x = _dist.gather_edits(x, self.job_edits)
         return x
+
+    @staticmethod
+    def _check_edit_exchange():
+        if patch.GLOBAL_EXCHANGE != "recurrence":
+            raise ValueError(f"shard=True over several edits needs patch.GLOBAL_EXCHANGE='recurrence' (got "
+                             f"{patch.GLOBAL_EXCHANGE!r}): every rank runs the whole recurrence of its own edits, and "
+                             f"the exchange modes, made for chunk sharding, would mix edits between ranks")
+
+    def _check_edit_lockstep(self, x: torch.Tensor):
+        """Before a sharded sample(): ValueError on every rank unless all ranks agree on what decides their draws and
+        their shapes (dist.check_ranks_agree).  The draws are those of get_chunks (torch's CPU generator, and numpy's
+        with randomize_chunks), of the blocks' generators once forked, else of the default generator of x's device from
+        which they are forked."""
+        import hashlib
+        from . import dist as _dist
+        digest = hashlib.sha256(torch.get_rng_state().numpy().tobytes())
+        if x.is_cuda:
+            digest.update(torch.cuda.get_rng_state(x.device).numpy().tobytes())
+        for model in self._models():
+            for m in model.modules():
+                g = getattr(m, "generator", None)
+                if isinstance(g, torch.Generator):
+                    digest.update(g.get_state().numpy().tobytes())
+        if self.randomize_chunks:
+            name, keys, pos, gauss, cached = np.random.get_state()
+            digest.update(keys.tobytes() + repr((name, pos, gauss, cached)).encode())
+        _dist.check_ranks_agree({
+            "edits": self.job_edits,
+            "latents": (x.dim() == 4 or (x.dim() == 5 and x.shape[0] in (self.job_edits, self.edits)),
+                        tuple(x.shape[-4:])),
+            "n_timesteps": len(self.timesteps),
+            "mode": (self.cuda_graph, self.capture_global, self.chunk_graphs, self.graph_warmup, self.merge_global,
+                     self.chunk_size, self.chunk_ord, self.perm_div, self.randomize_chunks),
+            "exchange": patch.GLOBAL_EXCHANGE,
+            "rng": digest.hexdigest()[:16],
+        })
 
     def close(self):
         """Release the captured graphs and give a ControlNet this driver served its own classes back.  The driver may
